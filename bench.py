@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — 512x512 images/s of the one-step image-translation path on N B200s (BASELINE.json metric).
+"""bench.py — 512x512 images/s of the one-step image-translation path on N H100s (BASELINE.json metric).
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -11,10 +11,13 @@ batch of synthetic 512x512 inputs.  The HEADLINE (`value`, `e2e`, `roofline`) is
 edge_to_image, bf16, batch 8 per GPU, random-init weights, LoRA folded.  The same JSON line carries a `configs` block with
 the other BASELINE configs at the N it was launched with: #3 cyclegan day_to_night fp16 batch 16/GPU, #4 pix2pix
 sketch_to_image_stochastic (TwinConv, noise map, gamma = 0.4) bf16 batch 8/GPU, #5 cyclegan clear_to_rainy fp16 per-GPU batch
-sweep 1..32.  N > 1 shards images across ranks (weak scaling, no data-path collective) plus ONE NCCL all-gather of the
+sweep 1..16.  N > 1 shards images across ranks (weak scaling, no data-path collective) plus ONE NCCL all-gather of the
 output latents per step.  Prints one JSON line on rank 0.
 
   --model/--stochastic/--batch/--dtype pick another headline workload; --configs none|3,4,5 limits the extra block.
+  --dump-outputs DIR writes what the last timed step computed (output images and latents, and at N > 1 the all-gathered
+  latents; float32 .npy) for comparing builds.  --steps / --warmup apply as given to every GPU timed loop of the line; the
+  product arm's `cpu_baseline` is a separate one-image host sample (its size is stated in its `sample` field).
 """
 import argparse
 import json
@@ -45,9 +48,9 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return (d.get("bf16_tflops_sustained", 1407.3), d.get("bf16_tflops", 1655.4), d.get("hbm_gbs", 6576.4),
+        return (d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), d.get("hbm_gbs", 3350.0),
                 "measured (MEASURED_PEAKS.json)")
-    return 1400.0, 1650.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 989.0, 3350.0, "NVIDIA H100 SXM data sheet (dense BF16, HBM3; 700 W card)"
 
 
 class ClockSampler:
@@ -141,21 +144,21 @@ def cpu_oracle_images_per_s(sd, size, steps, warmup, cross_dim, cfg):
 
 
 def run_reference(args):
-    """--impl reference: the reference's own CPU implementation of the path.  diffusers/peft are not installable here
-    (not in /opt/wheelhouse, no network; DESIGN.md), so this times oracle/ — the restatement of the same algorithm —
-    with every host thread.  One step = one 512x512 image (a bounded sample of the batch-8 workload)."""
+    """--impl reference: the reference's own CPU implementation of the path.  diffusers/peft are not a dependency of this
+    project (DESIGN.md), so this times oracle/ — the restatement of the same algorithm —
+    with every host thread.  One step = one image of --size (batch 1); --steps / --warmup are taken as given."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
     import weights as W
     sd = W.make_state_dict("pix2pix", W.SD_TURBO, seed=0)
-    steps, warmup = max(1, min(args.steps, 3)), max(1, min(args.warmup, 1))
+    steps, warmup = args.steps, args.warmup
     ips, sec = cpu_oracle_images_per_s(sd, args.size, steps, warmup, 1024, W.SD_TURBO)
     cores = CPU_THREADS
     line = {"impl": "reference", "metric": "512x512 images/sec", "value": ips, "unit": "images/s", "n_gpus": args.gpus,
             "steps": steps, "warmup": warmup, "ms_per_step": sec * 1e3, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-            "config": {"workload": WORKLOAD, "note": "CPU arm: fp32, batch 1 per step (bounded sample), all host threads"},
+            "config": {"workload": WORKLOAD, "note": "CPU arm: fp32, batch 1 per step, all host threads"},
             "cpu_baseline": {"value": ips, "unit": "images/s", "cores": cores, "kind": "port",
                              "sample": f"{steps} x one {args.size}x{args.size} image, oracle fp32 (steps/warmup capped at 3/1)"},
             "e2e": {"value": ips, "unit": "images/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
@@ -228,15 +231,14 @@ def make_step(w, world, dist):
     Default: the collective is issued on the compute stream after every step.  I2IT_OVERLAP_GATHER=1 issues it on a SIDE stream
     so that step i+1 computes while the all-gather of step i is in flight (two alternating latent / gather buffers; a step
     waits for the gather that read its buffer two steps back; `finish` joins the side stream into the timed stream before the
-    closing event, so all K collectives complete inside the timed region).  Measured on 2 x B200 (round 2, runs E, DESIGN
-    section 5): both variants cost the same 1.4-2.0 ms per 36.5 ms step although the all-gather alone takes 15 us — the loss is
-    the per-step synchronisation of GPUs whose step times differ (power capping: 2 % between GPUs, sigma 0.7-1.0 ms per step),
-    not the transfer — so the simpler synchronous form stays the default."""
+    closing event, so all K collectives complete inside the timed region).  The synchronous form is the default."""
     if world == 1:
         return w.step, None, "none"
     B, S, dt = w.B, w.S, w.dt
     if os.environ.get("I2IT_OVERLAP_GATHER") is None:
         gathered = torch.empty(world * B, 4, S // 8, S // 8, device="cuda", dtype=dt)
+
+        w.gathered = gathered
 
         def step_sync():
             w.step()
@@ -260,6 +262,7 @@ def make_step(w, world, dist):
         with torch.cuda.stream(side):
             side.wait_event(ev)
             dist.all_gather_into_tensor(gath[i], lats[i])
+            w.gathered = gath[i]
             gdone[i] = torch.cuda.Event()
             gdone[i].record(side)
         cnt[0] += 1
@@ -298,6 +301,24 @@ def timed(step_fn, K, Wm, world, dist, flush, finish=None):
     return t.item(), mine
 
 
+def dump_outputs(out_dir, wl):
+    """What the timed step hands its caller, as float32: this rank's output images [B, 3, S, S] and latents [B, 4, S/8, S/8],
+    and at N > 1 the all-gathered latents of every rank [N*B, 4, S/8, S/8] (out_latent_gathered).  At most 64 MB in all: a batch
+    too large for that is cut to its first images."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    gathered = getattr(wl, "gathered", None)
+    per_image = 4 * (wl.out[0].numel() + wl.lat[0].numel())
+    budget = (64 << 20) - (4 * gathered.numel() if gathered is not None else 0)
+    keep = max(1, min(wl.out.shape[0], budget // per_image))
+    arrays = [("out", wl.out[:keep]), ("out_latent", wl.lat[:keep])]
+    if gathered is not None:
+        arrays.append(("out_latent_gathered", gathered))
+    for name, t in arrays:
+        np.save(os.path.join(out_dir, name + ".npy"), t.float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -313,7 +334,12 @@ def main():
     ap.add_argument("--configs", default="3,4,5", help="extra BASELINE configs reported in the `configs` block ('none' to skip)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--profile-out", default="", help="write the per-launch timing table (JSON) here")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the last step's outputs as DIR/<name>.npy (float32): rank 0's images and "
+                         "latents, and at --gpus > 1 the all-gathered latents of every rank")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         return run_reference(args)
 
@@ -334,7 +360,7 @@ def main():
     if args.batch is None:
         args.batch = 8 if args.model == "pix2pix" else 16
     dt = torch.bfloat16 if args.dtype == "bf16" else torch.float16
-    B, S, K, Wm = args.batch, args.size, args.steps, max(args.warmup, 3)
+    B, S, K, Wm = args.batch, args.size, args.steps, args.warmup
     head_id = "4" if args.stochastic else ("2" if args.model == "pix2pix" else "3")
     workload = WORKLOADS[head_id]
     extra = [] if args.configs == "none" else [c for c in args.configs.split(",") if c in ("2", "3", "4", "5") and c != head_id]
@@ -350,7 +376,7 @@ def main():
     build_s = {"weights_init_s": round(wl.t_weights, 2), "engine_upload_fold_plan_first_forward_s": round(wl.t_engine, 2),
                "prep_launches": eng.prep_launch_count()}
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # > 50 MB L2
     step, finish, collective = make_step(wl, world, dist)
 
     sampler = ClockSampler(local)
@@ -364,6 +390,8 @@ def main():
         finish()
     ms_step, ms_mine = timed(step, K, 0, world, dist, flush, finish)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, wl)
     value = world * B / (ms_step / 1e3)
     finite = bool(torch.isfinite(wl.out.float()).all().item())
 
@@ -388,7 +416,7 @@ def main():
 
     def e2e_loop(fn_in, fn_call, fn_out, gather_buf):
         with torch.no_grad():
-            for _ in range(2):
+            for _ in range(Wm):
                 fn_out(fn_call(fn_in()))
             torch.cuda.synchronize()
             if world > 1:
@@ -422,10 +450,9 @@ def main():
         call_u8 = lambda x: wl.model.forward_u8(x)
     e2e_u8_value = e2e_loop(lambda: u8_in.cuda(non_blocking=True), call_u8, lambda y: u8_out.copy_(y, non_blocking=True), gathered_u8)
 
-    # ---- the other BASELINE configs, same N, same timing rules (fewer steps) ----
+    # ---- the other BASELINE configs, same N, same timing rules, same --steps / --warmup ----
     configs = {head_id: {"workload": workload, "value": value, "ms_per_step": ms_step, "per_gpu_batch": B, "dtype": args.dtype,
                          "finite": finite}}
-    Kx = max(3, min(K, 5))
     cyc = None
     for cid in extra:
         try:
@@ -437,19 +464,19 @@ def main():
                 w2 = Workload("pix2pix", True, torch.bfloat16, 8, S, rank, text_stack)
             else:
                 w2 = Workload("pix2pix", False, torch.bfloat16, 8, S, rank, text_stack)
-            sweep = [1, 2, 4, 8, 16, 32] if cid == "5" else [w2.B]
+            sweep = [1, 2, 4, 8, 16] if cid == "5" else [w2.B]     # batch 32 does not fit next to the cached plans in 80 GB
             rows = []
             for b in sweep:
                 w2.set_batch(b)
                 step2, fin2, _ = make_step(w2, world, dist)
-                ms2, _ = timed(step2, Kx, 3, world, dist, flush, fin2)
+                ms2, _ = timed(step2, K, Wm, world, dist, flush, fin2)
                 if fin2 is not None:
                     fin2()
                     torch.cuda.synchronize()
                 rows.append({"per_gpu_batch": b, "global_batch": world * b, "value": world * b / (ms2 / 1e3), "ms_per_step": ms2,
                              "finite": bool(torch.isfinite(w2.out.float()).all().item()),
                              "step_tensor_frac_of_sustained_peak": (b * FLOPS_PER_IMAGE / (ms2 * 1e-3)) / 1e12 / measured_peaks()[0]})
-            entry = {"workload": WORKLOADS[cid], "dtype": "fp16" if w2.dt == torch.float16 else "bf16", "steps": Kx, "warmup": 3,
+            entry = {"workload": WORKLOADS[cid], "dtype": "fp16" if w2.dt == torch.float16 else "bf16", "steps": K, "warmup": Wm,
                      "n_gpus": world}
             if cid == "5":
                 entry["sweep"] = rows
@@ -484,20 +511,14 @@ def main():
     tg_ms, tg_fl = sum(p["ms"] for p in tg), sum(p["flops"] for p in tg)
     all_ms = sum(p["ms"] for p in prof)
     achieved = tg_fl / (tg_ms * 1e-3) / 1e12 if tg_ms > 0 else 0.0
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "tapgemm_dram_traffic.json")     # from the committed ncu capture of this command
-    if os.path.exists(tpath) and head_id == "2" and B == 8 and S == 512:
-        traffic = json.load(open(tpath)).get("dram_bytes_per_step")
     gn_ms = sum(v["ms"] for k, v in by_kind.items() if k.startswith("gn_"))
     gn_bytes = sum(v["bytes"] for k, v in by_kind.items() if k.startswith("gn_"))
-    roofline = {"bound": "tensor", "kernel": "tapgemm_kernel + tapgemm2_kernel (tcgen05 implicit GEMM: conv3x3/1x1/linear/attention; "
-                                             "all launches of a step, CTA-pair variant for the large layers)",
-                # launches are timed one at a time (isolated), so the burst cuBLAS figure is the honest denominator
+    roofline = {"bound": "tensor", "kernel": "tapgemm_kernel (wgmma implicit GEMM: conv3x3/1x1/linear/attention; "
+                                             "all launches of a step)",
                 "achieved": achieved, "peak": peak_burst, "unit": "TFLOP/s", "frac": achieved / peak_burst, "peak_source": peak_src,
                 "frac_of_sustained_peak": achieved / peak_tf,
                 "launches_per_step": len(tg), "avg_launch_ms": tg_ms / max(1, len(tg)),
                 "share_of_step": tg_ms / all_ms if all_ms else None,
-                "traffic": traffic, "traffic_note": "sum of dram__bytes_read+write over the step's tapgemm launches (ncu, profiles/)",
                 "algorithmic_bytes": sum(p["bytes"] for p in tg),
                 "step_tensor_frac": (B * FLOPS_PER_IMAGE / (ms_step * 1e-3)) / 1e12 / peak_tf,
                 "step_tensor_frac_note": "whole step in graph replay (long run): images x 4467.6 GFLOP / step time / SUSTAINED peak",

@@ -18,8 +18,7 @@ import i2it
 import weights as W
 
 SD_TURBO_DIR_ENV = "I2IT_SD_TURBO_DIR"      # optional local snapshot of stabilityai/sd-turbo (offline boxes)
-DEVICE = "cuda"      # where the wrappers stage tensors.  tests/cpu_stub_engine.py (a TEST DOUBLE of i2it.Engine used to run the
-                     # unmodified reference CLIs on GPU-less hosts) sets this to "cpu"; the product never does.
+DEVICE = "cuda"      # where the wrappers stage tensors (the engine runs on the current CUDA device)
 
 
 def _cur_dev() -> int:
@@ -27,7 +26,7 @@ def _cur_dev() -> int:
 
 
 # ------------------------------------------------------------------------------------------------
-# scheduler mirror: make_1step_sched() of /root/reference/src/model.py:7-11, as closed-form constants
+# scheduler mirror: make_1step_sched() of src/model.py:7-11, as closed-form constants
 # ------------------------------------------------------------------------------------------------
 class OneStepDDPM:
     """DDPMScheduler(scaled_linear 0.00085->0.012, 1000 steps, trailing, 1 inference step) reduced to t=999."""
@@ -68,7 +67,7 @@ class HashTokenizer:
 
 
 def build_text_stack(cross_dim: int = 1024, seed: int = 1234):
-    """(tokenizer, text_encoder).  Mirrors /root/reference/src/pix2pix_turbo.py:32-33."""
+    """(tokenizer, text_encoder).  Mirrors src/pix2pix_turbo.py:32-33."""
     from transformers import CLIPTextConfig, CLIPTextModel
     local = os.environ.get(SD_TURBO_DIR_ENV)
     srcs = ([local] if local else []) + ["stabilityai/sd-turbo"]
@@ -140,7 +139,7 @@ class NetHandle:
         return self
 
     def enable_xformers_memory_efficient_attention(self, *a, **k):
-        # /root/reference/src/inference_unpaired.py:36 calls this; attention here is already a fused tensor-core path
+        # src/inference_unpaired.py:36 calls this; attention here is already a fused tensor-core path
         return self
 
     def set_adapters(self, names, weights=None):
@@ -152,8 +151,8 @@ class TurboBase(torch.nn.Module):
     MODEL_KIND = i2it.PIX2PIX
 
     def _init_common(self, cfg, dtype, text_stack, use_cuda_graph=True, keep_stages=False):
-        # I2IT_CFG=tiny: reduced-width network when the caller cannot pass `cfg` — the unmodified reference CLIs in the test suite
-        # (tests/test_reference_cli.py); the default is always the SD-Turbo geometry
+        # I2IT_CFG=tiny: reduced-width network when the caller cannot pass `cfg` (e.g. an unmodified inference script under test);
+        # the default is always the SD-Turbo geometry
         if cfg is None and os.environ.get("I2IT_CFG") == "tiny":
             cfg = W.TINY
         self._cfg = cfg or W.SD_TURBO

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libi2it (sm_100a only).
+// Shared device/host helpers for libi2it (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -73,11 +73,10 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + ex2_approx(-1.4426950408889634f * x)); }
 // Programmatic dependent launch (PDL).  Every kernel of a forward plan calls pdl_sync() before its first access to global
-// memory: launch_dependents lets the NEXT kernel's CTAs become resident (and run their barrier/TMEM prologue) as soon as all
+// memory: launch_dependents lets the NEXT kernel's CTAs become resident (and run their barrier prologue) as soon as all
 // CTAs of this grid have started; wait blocks until the PREVIOUS grid has completed and its writes are visible.  Because
 // every kernel waits, completion is transitive along the stream (C waits for B, B waited for A), which keeps the pool's
-// buffer recycling safe.  Kernels that allocate TMEM call it AFTER the allocation, so an early-resident successor can never
-// take tensor memory a predecessor CTA still has to allocate.  Without the launch attribute both instructions are no-ops.
+// buffer recycling safe.  Without the launch attribute both instructions are no-ops.
 __device__ __forceinline__ void pdl_sync() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");

@@ -109,8 +109,8 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CUDA(cudaSetDevice(c.device));
   cudaDeviceProp prop;
   I2IT_CUDA(cudaGetDeviceProperties(&prop, c.device));
-  I2IT_CHECK(prop.major == 10, "libi2it is built for sm_100a (B200) only; found compute capability " +
-                                   std::to_string(prop.major) + "." + std::to_string(prop.minor));
+  I2IT_CHECK(prop.major == 9 && prop.minor == 0, "libi2it is built for sm_90a (H100) only; found compute capability " +
+                                                  std::to_string(prop.major) + "." + std::to_string(prop.minor));
   num_sms = prop.multiProcessorCount;
   I2IT_CUDA(cudaFuncSetAttribute(tapgemm_kernel<__half, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
   I2IT_CUDA(cudaFuncSetAttribute(tapgemm_kernel<__half, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
@@ -118,11 +118,7 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CUDA(cudaFuncSetAttribute(tapgemm_kernel<__nv_bfloat16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
-  I2IT_CUDA(cudaFuncSetAttribute(flash_attn_v1_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
-  I2IT_CUDA(cudaFuncSetAttribute(flash_attn_v1_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
   use_flash = std::getenv("I2IT_NO_FLASH") == nullptr;
-  flash_v1 = std::getenv("I2IT_FLASH_V1") != nullptr;       // round-1 softmax scheme (A/B)
-  use_pair = std::getenv("I2IT_NO_PAIR") == nullptr;
   use_pdl = std::getenv("I2IT_PDL") != nullptr;     // programmatic dependent launch: measured neutral (1 CTA/SM kernels cannot co-reside), opt-in
 #ifdef I2IT_TRACE_BUILD
   trace_on = std::getenv("I2IT_TRACE") != nullptr;
@@ -134,15 +130,8 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   use_gnepi = std::getenv("I2IT_NO_GNEPI") == nullptr;     // GroupNorm statistics in the producing GEMM's epilogue
   use_splitk = std::getenv("I2IT_NO_SPLITK") == nullptr;   // split-K for the 8x8 1280-channel convs
   use_catfuse = std::getenv("I2IT_NO_CATFUSE") == nullptr; // UNet skip concatenations written in place (no copy kernels)
-  pair_min_tiles = std::getenv("I2IT_PAIR_MIN_TILES") ? atoll(std::getenv("I2IT_PAIR_MIN_TILES")) : 2ll * num_sms;
-  // identity residual as a K-slab: round 1's default; with the round-2 epilogue (coalesced residual through the store box) and the
-  // faster halo path the residual is cheaper in the epilogue (9-tap halo conv 409 us vs 10-tap 585 us, run J), so it is opt-in now
+  // identity residual as a K-slab (opt-in): the coalesced residual through the store box is the default
   use_idres = std::getenv("I2IT_IDRES") != nullptr && std::getenv("I2IT_NO_IDRES") == nullptr;
-  use_halo = std::getenv("I2IT_NO_HALO") == nullptr;   // 3x3 convs: one halo tile per k-chunk instead of nine shifted A boxes
-  I2IT_CUDA(cudaFuncSetAttribute(tapgemm2_kernel<__half, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG2_SMEM));
-  I2IT_CUDA(cudaFuncSetAttribute(tapgemm2_kernel<__half, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG2_SMEM));
-  I2IT_CUDA(cudaFuncSetAttribute(tapgemm2_kernel<__nv_bfloat16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG2_SMEM));
-  I2IT_CUDA(cudaFuncSetAttribute(tapgemm2_kernel<__nv_bfloat16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG2_SMEM));
   int* h = nullptr;
   I2IT_CUDA(cudaHostAlloc(&h, sizeof(int), cudaHostAllocMapped));
   *h = 0;
@@ -170,7 +159,7 @@ void Engine::check_device_error() {
   if (err_host_ && *err_host_ != 0) {
     const int code = *err_host_;
     throw Error("tapgemm watchdog tripped (pipeline stage code " + std::to_string(code) +
-                ": 1=producer/empty 2=mma/tmem_empty 3=mma/full 4=epilogue/tmem_full)");
+                ": 1=producer/empty 2=producer/epilogue-done 3=consumer/full)");
   }
 }
 
@@ -578,26 +567,20 @@ bool Engine::tma_eligible(const TapGemmParams& p, bool out_from_io) const {
 static void fill_strides(TmapSpec& s);
 
 void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemmParams& p_in, bool out_from_io,
-                         const char* kind, double k_valid, double bytes, const TmapSpec* sa2p, const TmapSpec* sb2p,
-                         const TmapSpec* shalo) {
+                         const char* kind, double k_valid, double bytes, const TmapSpec* sa2p, const TmapSpec* sb2p) {
   TapGemmParams p = p_in;
   for (int t = 0; t < p.num_taps; ++t)
     if (p.tap_kc[t] == 0) p.tap_kc[t] = p.kchunks;          // single-source callers only set kchunks
   if (p.nprim == 0) p.nprim = p.num_taps;
   const long long m_tiles = 1ll * p.tdim[0] * p.tdim[1] * p.tdim[2] * p.tdim[3];
   const long long total_tiles = m_tiles * p.n_tiles * (p.ksplit > 1 ? p.ksplit : 1);
-  // CTA-pair kernel: weights/B shared by every M tile (no per-tile B batch coordinates), enough tiles to fill the chip twice
-  const bool pair = use_pair && p.ksplit <= 1 && p.b_mul[0] == 0 && p.b_mul[1] == 0 && p.b_mul[2] == 0 && (p.BN % 32) == 0 &&
-                    total_tiles >= pair_min_tiles && m_tiles >= 2;
-  TmapSpec sb2 = sb2p ? *sb2p : sb;
-  if (pair) { sb.box[1] = p.BN / 2; sb2.box[1] = p.BN / 2; p.idesc = make_idesc2(dtype, p.BN); }
-  p.halo = (pair && shalo != nullptr && use_halo) ? 1 : 0;
+  I2IT_CHECK(p.BN % 16 == 0 && p.BN <= 256, "tapgemm: BN must be a multiple of 16 up to 256");
+  const TmapSpec sb2 = sb2p ? *sb2p : sb;
   p.tma_out = tma_eligible(p, out_from_io) ? 1 : 0;
-  {  // smem ring geometry: B stage = the real (half) tile rounded to the 1024-byte swizzle atom, as many stages as fit
-    const int brows = pair ? p.BN / 2 : p.BN;
-    p.b_stage = (brows * TG_BK * 2 + 1023) / 1024 * 1024;
-    int budget = pair ? (p.halo ? TG2_DATA_BYTES - TG2_HALO_REGION : TG2_DATA_BYTES) : TG_STAGES * (TG_A_STAGE + TG_B_STAGE);
-    const int per = (p.halo ? 0 : TG_A_STAGE) + p.b_stage;
+  {  // smem ring geometry: B stage = the real tile rounded to the 1024-byte swizzle atom, as many stages as fit
+    p.b_stage = (p.BN * TG_BK * 2 + 1023) / 1024 * 1024;
+    int budget = TG_STAGES * (TG_A_STAGE + TG_B_STAGE);
+    const int per = TG_A_STAGE + p.b_stage;
     // a second store box per epilogue warp out of the ring's last 32 KB when at least 4 stages remain and the tile's mainloop
     // is short (<= 48 k-steps, i.e. <= 96 * BN tensor cycles): those launches wait on TMA-store drain, not on operands; the
     // long-K launches hide their epilogue anyway and keep the deeper ring
@@ -608,21 +591,14 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
     p.stages = std::max(2, std::min(TG_MAX_STAGES, budget / per));
   }
   const CUtensorMap ta = encode_tmap(sa, dtype), tb = encode_tmap(sb, dtype);
-  const CUtensorMap th = p.halo ? encode_tmap(*shalo, dtype) : ta;
   const CUtensorMap ta2 = sa2p ? encode_tmap(*sa2p, dtype) : ta, tb2 = sb2p ? encode_tmap(sb2, dtype) : tb;
   const int dt = dtype;
   Plan* plan = &P;
   const double m_valid = 1.0 * p.ext[0] * p.ext[1] * p.ext[2] * p.ext[3];
-  int grid;
-  if (pair) {
-    const long long pairs = ((m_tiles + 1) / 2) * p.n_tiles;
-    grid = 2 * static_cast<int>(std::min<long long>(pairs, num_sms / 2));
-  } else {
-    grid = static_cast<int>(std::min<long long>(total_tiles, num_sms));
-  }
+  const int grid = static_cast<int>(std::min<long long>(total_tiles, num_sms));
   char shp[160];
-  snprintf(shp, sizeof shp, "M=%.0f N=%d K=%.0f taps=%d BN=%d tiles=%lld grid=%d st=%d%s%s%s", m_valid, p.N, k_valid, p.num_taps, p.BN,
-           total_tiles, grid, p.stages, pair ? (p.halo ? " pair halo" : " pair") : "", p.tma_out ? (p.ostg2 ? " tma2" : " tma") : "",
+  snprintf(shp, sizeof shp, "M=%.0f N=%d K=%.0f taps=%d BN=%d tiles=%lld grid=%d st=%d%s%s", m_valid, p.N, k_valid, p.num_taps, p.BN,
+           total_tiles, grid, p.stages, p.tma_out ? (p.ostg2 ? " tma2" : " tma") : "",
            (p.gn_part && p.tma_out) ? " gn" : "");
   // TMA-store epilogue: the output tensor map has the tile's row dims (extents = logical extents, so ragged edges are clipped
   // by the hardware) and a box of 64 columns x the 32 rows one epilogue warp owns
@@ -651,8 +627,8 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
     I2IT_CUDA(cudaMemset(p.trace, 0, static_cast<size_t>(grid) * 16 * sizeof(unsigned long long)));
     P.traces.push_back({p.trace, grid, std::string(kind) + " " + shp});
   }
-  {  // division-free tile decode (see fast_div): dividends are tile indices (pair kernel: up to 2 * m-tile index + 1)
-    const long long maxd = std::max<long long>(total_tiles, 2 * m_tiles + 2) + grid;
+  {  // division-free tile decode (see fast_div): dividends are tile indices
+    const long long maxd = std::max<long long>(total_tiles, m_tiles) + grid;
     p.magic[0] = make_magic(maxd, p.n_tiles);
     for (int d = 0; d < 4; ++d) p.magic[d + 1] = make_magic(maxd, p.tdim[d]);
     for (int d = 0; d < 5; ++d) I2IT_CHECK(p.magic[d] != 0, "tapgemm: tile space too large for the division-free tile decode");
@@ -660,21 +636,12 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
     while ((1 << p.gn_shift) < p.gn_red) ++p.gn_shift;
   }
   const bool lean = use_lean && p.tma_out && p.act == TG_ACT_NONE;      // the epilogue variant without activation / direct-store code
-  if (pair) {
-    add_op(P, [ta, tb, ta2, tb2, th, to, p, grid, dt, out_from_io, plan, lean](cudaStream_t st) {
-      TapGemmParams q = p;
-      if (out_from_io) q.out = plan->io.out;
-      if (lean) { DISPATCH_T(dt, (launch_k(tapgemm2_kernel<T, true>, dim3(grid), dim3(TG_THREADS), TG2_SMEM, st, 2, ta, tb, ta2, tb2, th, to, q))); }
-      else { DISPATCH_T(dt, (launch_k(tapgemm2_kernel<T, false>, dim3(grid), dim3(TG_THREADS), TG2_SMEM, st, 2, ta, tb, ta2, tb2, th, to, q))); }
-    }, kind, 2.0 * m_valid * p.N * k_valid, bytes, shp);
-  } else {
-    add_op(P, [ta, tb, ta2, tb2, to, p, grid, dt, out_from_io, plan, lean](cudaStream_t st) {
-      TapGemmParams q = p;
-      if (out_from_io) q.out = plan->io.out;
-      if (lean) { DISPATCH_T(dt, (launch_k(tapgemm_kernel<T, true>, dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q))); }
-      else { DISPATCH_T(dt, (launch_k(tapgemm_kernel<T, false>, dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q))); }
-    }, kind, 2.0 * m_valid * p.N * k_valid, bytes, shp);
-  }
+  add_op(P, [ta, tb, ta2, tb2, to, p, grid, dt, out_from_io, plan, lean](cudaStream_t st) {
+    TapGemmParams q = p;
+    if (out_from_io) q.out = plan->io.out;
+    if (lean) { DISPATCH_T(dt, (launch_k(tapgemm_kernel<T, true>, dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q))); }
+    else { DISPATCH_T(dt, (launch_k(tapgemm_kernel<T, false>, dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q))); }
+  }, kind, 2.0 * m_valid * p.N * k_valid, bytes, shp);
 }
 
 static void fill_strides(TmapSpec& s) {
@@ -726,19 +693,10 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
   std::memset(&p, 0, sizeof p);
   int tw, th, tn;
   const long long ldo = o.to_io_out_nchw ? 0 : out.ld;
-  // halo mode (CTA-pair kernel): 8 x 16 output tiles whose nine taps share one halo tile per k-chunk
-#ifdef I2IT_HALO_X2
-  const bool halo_x2_ok = true;      // experimental build: the second-source taps ride a small A ring next to the halo stages
-#else
-  const bool halo_x2_ok = !o.x2;
-#endif
-  const bool want_halo = use_halo && use_pair && o.stride == 1 && k == 3 && !sub && halo_x2_ok && !o.to_io_out_nchw && x.H >= 16 &&
-                         x.W >= 8 && x.C % 64 == 0;
   if (o.stride == 1) {
     tw = (x.H == 1) ? std::min(128, pow2ceil(x.W)) : std::min(o.to_io_out_nchw ? 32 : 16, pow2ceil(x.W));
     th = std::min(128 / tw, pow2ceil(x.H));
     tn = 128 / (tw * th);
-    if (want_halo) { tw = 8; th = 16; tn = 1; }
     sa.base = x.p;
     sa.dim[0] = x.C; sa.dim[1] = x.W; sa.dim[2] = x.H; sa.dim[3] = x.N; sa.dim[4] = 1;
     sa.stride[0] = x.ld * 2ull; sa.stride[1] = 2ull * x.W * x.ld; sa.stride[2] = 2ull * x.H * x.W * x.ld;
@@ -823,7 +781,6 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
   sb.box[0] = 64; sb.box[1] = p.BN; sb.box[2] = 1; sb.box[3] = 1; sb.box[4] = 1;
   p.num_taps = taps;
   p.nprim = taps;
-  p.idesc = make_idesc(dtype, p.BN);
   p.ocol = 1;
   p.out_fp32 = o.out_fp32 ? 1 : 0;
   if (o.to_io_out_nchw) {
@@ -908,7 +865,6 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
     p.BN = 256;
     p.n_tiles = ceil_div(gemm_n, p.BN);
     sb.box[1] = p.BN;
-    p.idesc = make_idesc(dtype, p.BN);
   }
 
   TmapSpec sa2, sb2;
@@ -951,10 +907,7 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
     const double bytes = 2.0 * (1.0 * x.N * x.H * x.W * w.cin + m_valid * outc * (o.out_fp32 ? 2 : 1) + 1.0 * gemm_n * k_valid +
                                 (o.res ? m_valid * outc : 0) + m_valid * k2);
     const char* kind = sub ? "tapgemm:conv_up2x" : (k == 3) ? (o.stride == 2 ? "tapgemm:conv3x3s2" : "tapgemm:conv3x3") : "tapgemm:linear";
-    TmapSpec sh = sa;
-    sh.box[1] = TG2_HALO_W; sh.box[2] = TG2_HALO_H; sh.box[3] = 1;
-    launch_gemm(P, sa, sb, p, o.to_io_out_nchw, kind, k_valid, bytes, o.x2 ? &sa2 : nullptr, o.x2 ? &sb2 : nullptr,
-                want_halo ? &sh : nullptr);
+    launch_gemm(P, sa, sb, p, o.to_io_out_nchw, kind, k_valid, bytes, o.x2 ? &sa2 : nullptr, o.x2 ? &sb2 : nullptr);
   }
   if (splitk) {
     const float* part = static_cast<const float*>(sk_hold.get());
@@ -1139,7 +1092,6 @@ Act Engine::vt_proj(Plan& P, const Act& x, int B, int ntok, const PW& wv) {
   sb.box[0] = 64; sb.box[1] = p.BN;
   p.num_taps = 1;
   p.kchunks = ceil_div(x.C, 64);
-  p.idesc = make_idesc(dtype, p.BN);
   p.out = vt.p;
   p.ostride[0] = ldv; p.ostride[1] = 0; p.ostride[2] = static_cast<long long>(C) * ldv; p.ostride[3] = 0;
   p.ocol = 1;
@@ -1192,7 +1144,6 @@ Act Engine::attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B,
     sb.box[0] = 64; sb.box[1] = p.BN;
     p.num_taps = 1;
     p.kchunks = d / 64;
-    p.idesc = make_idesc(dtype, p.BN);
     p.out = S;
     p.out_fp32 = 1;
     p.ostride[0] = lds; p.ostride[1] = static_cast<long long>(Nq) * lds; p.ostride[2] = static_cast<long long>(heads) * Nq * lds;
@@ -1247,7 +1198,6 @@ Act Engine::attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B,
     sb.box[0] = 64; sb.box[1] = p.BN;
     p.num_taps = 1;
     p.kchunks = ceil_div(Nk, 64);
-    p.idesc = make_idesc(dtype, p.BN);
     p.out = out.p;
     p.ostride[0] = out.ld; p.ostride[1] = d; p.ostride[2] = static_cast<long long>(Nq) * out.ld;
     p.ocol = 1;
@@ -1289,17 +1239,14 @@ Act Engine::flash_attention(Plan& P, const Act& q, const Act& k, const Act& vt, 
   fp.scale_log2e = (1.0f / sqrtf(static_cast<float>(d))) * 1.4426950408889634f;
   fp.out = out.p;
   fp.ldo = out.ld;
-  fp.idesc = make_idesc(dtype, FA_BN);
   fp.err = d_err;
   fp.causal = causal ? 1 : 0;
   const CUtensorMap tq = encode_tmap(sq, dtype), tk = encode_tmap(sk, dtype), tv = encode_tmap(sv, dtype);
   const int grid = fp.q_tiles * heads * B, dt = dtype;
   char shp[96];
   snprintf(shp, sizeof shp, "B=%d h=%d Nq=%d Nk=%d d=%d", B, heads, Nq, Nk, d);
-  const bool v1 = flash_v1;
   add_op(P, [=](cudaStream_t st) {
-    if (v1) { DISPATCH_T(dt, (launch_k(flash_attn_v1_kernel<T>, dim3(grid), dim3(FA_THREADS), FA_SMEM, st, 0, tq, tk, tv, fp))); }
-    else { DISPATCH_T(dt, (launch_k(flash_attn_kernel<T>, dim3(grid), dim3(FA_THREADS), FA_SMEM, st, 0, tq, tk, tv, fp))); }
+    DISPATCH_T(dt, (launch_k(flash_attn_kernel<T>, dim3(grid), dim3(FA_THREADS), FA_SMEM, st, 0, tq, tk, tv, fp)));
   }, "flash_attn", 4.0 * B * heads * Nq * Nk * d, 2.0 * (2.0 * B * Nq * C + 2.0 * kv_batch * Nk * C), shp);
   return out;
 }
@@ -1328,7 +1275,7 @@ void Engine::set_text(const void* text, int text_batch, cudaStream_t st) {
 
 // CLIP text tower on the engine (SURVEY 8f #1; transformers models/clip/modeling_clip.py CLIPTextTransformer.forward): token +
 // position embeddings, pre-LN transformer layers with CAUSAL self-attention (16 heads x 64 for SD-Turbo's OpenCLIP-H tower) and a
-// GELU MLP, final LayerNorm -> last_hidden_state, i.e. `text_encoder(tokens)[0]` of /root/reference/src/pix2pix_turbo.py:190-196.
+// GELU MLP, final LayerNorm -> last_hidden_state, i.e. `text_encoder(tokens)[0]` of src/pix2pix_turbo.py:190-196.
 // Same kernels as the image path: tapgemm (fused q|k projection, V^T projection with row bias, GELU in the fc1 epilogue, residual
 // adds in the out_proj / fc2 epilogues), flash_attn with the causal flag, layernorm.
 void Engine::encode_text(const int* tokens, int batch, void* out, cudaStream_t st) {
@@ -1456,8 +1403,8 @@ void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int te
 
 // I2IT_TRACE=1: per GEMM launch, the median over CTAs of each phase stamp relative to the CTA's entry stamp (SM cycles).
 // slots: 1 prologue done | 2 first tile's loads issued | 3 all loads issued | 4 first operands landed | 5 first tile's MMAs
-// issued | 6 all MMAs issued | 7 first bias slice staged | 8 first accumulator ready | 9 first tile stored | 10 all tiles
-// stored | 11 CTA joined | 12 TMEM freed
+// complete | 7 first bias slice staged | 8 first accumulator ready | 9 first tile stored | 10 all tiles
+// stored | 11 CTA joined
 void Engine::dump_trace(Plan& P, cudaStream_t st) {
   I2IT_CUDA(cudaStreamSynchronize(st));
   I2IT_CUDA(cudaStreamSynchronize(gstream_));

@@ -14,8 +14,6 @@
 #include "prep.cuh"
 #include "tapgemm.cuh"
 #include "flash.cuh"
-#include "flash_v1.cuh"
-#include "tapgemm2.cuh"
 
 namespace i2it {
 
@@ -204,7 +202,7 @@ class Engine {
                 int kv_batch);
   Act flash_attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B, int Nq, int Nk, int heads, int kv_batch,
                       bool causal = false);
-  bool use_flash = true, flash_v1 = false;
+  bool use_flash = true;
 
   // ---- weights ----
   bool has(const std::string& key) const;
@@ -243,13 +241,11 @@ class Engine {
     OpMeta m; m.kind = kind; m.flops = flops; m.bytes = bytes; m.shape = shape;
     P.meta.push_back(m);
   }
-  // encodes the tensor maps and appends the launch; picks the CTA-pair kernel (tapgemm2) for big conv/linear layers
+  // encodes the tensor maps and appends the launch
   void launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemmParams& p, bool out_from_io, const char* kind,
-                   double k_valid, double bytes, const TmapSpec* sa2 = nullptr, const TmapSpec* sb2 = nullptr,
-                   const TmapSpec* shalo = nullptr);
-  bool use_pair = true, use_halo = true, use_idres = true, use_pdl = false, trace_on = false, use_tmaout = true, use_gnepi = true, use_splitk = true, use_catfuse = true, use_ostg2 = true, use_lean = true, sync_each = false;
+                   double k_valid, double bytes, const TmapSpec* sa2 = nullptr, const TmapSpec* sb2 = nullptr);
+  bool use_idres = true, use_pdl = false, trace_on = false, use_tmaout = true, use_gnepi = true, use_splitk = true, use_catfuse = true, use_ostg2 = true, use_lean = true, sync_each = false;
   bool tma_eligible(const TapGemmParams& p, bool out_from_io) const;
-  long long pair_min_tiles = 296;   // CTA-pair kernel from two waves of tiles upwards (tunable: I2IT_PAIR_MIN_TILES)
   std::string profile_json(int reps, cudaStream_t st);
   void dump_trace(Plan& P, cudaStream_t st);
   int pick_bn(long long m_tiles, int N, int step) const;   // step 64 / 128: BN restricted to multiples (TMA-store rounds)

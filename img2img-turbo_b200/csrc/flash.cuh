@@ -1,20 +1,17 @@
-// flash_attn_kernel: fused softmax(Q K^T * scale) V for head_dim 64 (all UNet self/cross attention of the path).
+// flash_attn_kernel: fused softmax(Q K^T * scale) V for head_dim 64 (all UNet self/cross attention and the CLIP text tower).
 //
 // Replaces, per attention layer, the three launches  S = QK^T (fp32 logits to HBM) -> softmax -> O = PV  — i.e. what the
-// reference gets from F.scaled_dot_product_attention / xformers FMHA (diffusers AttnProcessor2_0; call sites under
-// /root/reference/src/pix2pix_turbo.py:199 and /root/reference/src/inference_unpaired.py:36).
+// reference gets from F.scaled_dot_product_attention / xformers FMHA (diffusers AttnProcessor2_0).
 //
-// One CTA = one 128-row Q tile of one (batch, head); 192 threads:
-//   warp 4 lane 0 : TMA producer   Q once; (K_j [64 keys x 64], V^T_j [64 d x 64 keys]) through a 3-stage ring
-//   warp 5 lane 0 : MMA issuer     S_j = Q K_j^T (4 x tcgen05.mma M128 N64 K16) -> TMEM S buffer j&1
-//                                  PV_j = P_j V_j  (4 x tcgen05.mma, A = P_j staged in swizzled smem) -> TMEM cols [128,192)
-//                                  QK_{j+1} is issued as soon as the softmax warps have pulled S_j out of TMEM
-//   warps 0..3    : one Q row per thread: S_j is pulled out of TMEM ONCE (64 registers), online softmax in fp32 with a LAZY
-//                   reference maximum, P_j -> bf16/fp16 smem tile; O stays in TMEM (PV accumulates across KV steps) and is only
-//                   rescaled (tcgen05.ld -> mul -> tcgen05.st) when a row's maximum grows by more than 2^8; final O / l written once.
-//                   Round 1 read S twice and the PV tile once per step: 96 KB of TMEM reads per step at 64 B/clk/SM made the
-//                   kernel TMEM-read bound (25 % tensor pipe); this version reads 32 KB per step.
-// 2 CTAs per SM (80 KB smem, 256 TMEM columns each: S double-buffered + PV) so one CTA's MMAs overlap the other's exponentials.
+// One CTA = one 128-row Q tile of one (batch, head); 288 threads:
+//   warp 8        : TMA producer   Q once; (K_j [64 keys x 64], V^T_j [64 d x 64 keys]) through a 3-stage ring
+//   warps 0..7    : two consumer warpgroups, warpgroup g owns Q rows [64g, 64g+64):
+//                   S_j = Q K_j^T      4 x wgmma m64n64k16 (both operands in smem) -> fp32 registers
+//                   online softmax in fp32 on the accumulator fragments (a row lives in 4 lanes of a quad)
+//                   O += P_j V_j       4 x wgmma m64n64k16 with P_j as the REGISTER A operand: the accumulator fragment of
+//                                      S converts to the A fragment of P in place (16-bit pack), P never touches smem
+//                   the row sum l is taken over the ROUNDED probabilities, the same values the numerator uses
+// 2 CTAs per SM (65 KB smem each) so one CTA's MMAs overlap the other's exponentials.
 #pragma once
 #include "tapgemm.cuh"
 
@@ -22,65 +19,37 @@ namespace i2it {
 
 constexpr int FA_BM = 128, FA_BN = 64, FA_D = 64, FA_STAGES = 3;
 constexpr int FA_Q_BYTES = FA_BM * FA_D * 2;            // 16 KiB
-constexpr int FA_KV_DATA = 2 * FA_BN * FA_D * 2;        // K 8 KiB + V^T 8 KiB (what TMA writes per stage)
-// The PV product runs with N = 80: rows 64..79 of every V^T stage are constant — row 64 all ones, the rest zero — so column 64
-// of the O accumulator is the row sum l = sum_k P[m,k] of the ROUNDED probabilities (the same values the numerator uses); the
-// softmax threads no longer add 64 values per row and step (they are the critical path: MUFU + issue slots, profiles/r02g_flash*).
-constexpr int FA_PV_N = 80;
-constexpr int FA_KV_STAGE = FA_KV_DATA + (FA_PV_N - FA_D) * FA_BN * 2;   // + 2 KiB of constant rows
-constexpr int FA_P_BYTES = FA_BM * FA_BN * 2;           // 16 KiB
-constexpr int FA_SMEM = FA_Q_BYTES + FA_STAGES * FA_KV_STAGE + 2 * FA_P_BYTES + 256 + 1024;   // P is double-buffered
-constexpr int FA_THREADS = 192;
+constexpr int FA_KV_STAGE = 2 * FA_BN * FA_D * 2;       // K 8 KiB + V^T 8 KiB
+constexpr int FA_SMEM = FA_Q_BYTES + FA_STAGES * FA_KV_STAGE + 256 + 1024;
+constexpr int FA_THREADS = 288;
 
 struct FlashParams {
   int Nq, Nk, heads, B, q_tiles, kv_bmul;   // kv_bmul: 1 if K/V are per batch item, 0 if one K/V set is shared (text)
   float scale_log2e;                        // softmax scale * log2(e)
   void* out;                                // [B*Nq, ldo] tokens, head h at columns [64h, 64h+64)
   long long ldo;
-  uint32_t idesc;                           // M=128, N=64 (both GEMMs)
   int causal;                               // 1: key j attends only to queries i >= j (CLIP text tower); KV tiles past the diagonal are skipped
   int* err;
 };
 
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld1(uint32_t taddr, uint32_t (&r)[1]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r[0]) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_st1(uint32_t taddr, const uint32_t (&r)[1]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(r[0]) : "memory");
-}
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
+// D[64 x 64] += A[64 x 16] (registers, the m64k16 A fragment) * B[64 x 16]^T (K-major 128B-swizzled smem)
+template <typename T> __device__ __forceinline__ void wgmma_rs64(float* d, const uint32_t (&a)[4], uint64_t b);
+template <> __device__ __forceinline__ void wgmma_rs64<__half>(float* d, const uint32_t (&a)[4], uint64_t b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32, %33, %34, %35}, %36, 1, 1, 1, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
 }
-__device__ __forceinline__ void sts16(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+template <> __device__ __forceinline__ void wgmma_rs64<__nv_bfloat16>(float* d, const uint32_t (&a)[4], uint64_t b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32, %33, %34, %35}, %36, 1, 1, 1, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
 }
 
 template <typename T>
@@ -91,62 +60,30 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sQ = base;
   const uint32_t sKV = base + FA_Q_BYTES;
-  const uint32_t sP = sKV + FA_STAGES * FA_KV_STAGE;
-  const uint32_t bars = sP + 2 * FA_P_BYTES;
+  const uint32_t bars = sKV + FA_STAGES * FA_KV_STAGE;
   const uint32_t q_full = bars;
   auto kv_full = [&](int s) { return bars + 8u * (1 + s); };
   auto kv_empty = [&](int s) { return bars + 8u * (1 + FA_STAGES + s); };
-  // S is double-buffered in TMEM; each buffer has its own full/free barrier so no waiter can fall two phases behind
-  const uint32_t s_full0 = bars + 8u * (1 + 2 * FA_STAGES);
-  auto s_full = [&](int u) { return s_full0 + 8u * u; };
-  auto s_free = [&](int u) { return s_full0 + 16u + 8u * u; };
-  // P_j goes to smem buffer j&1 and PV_j signals pv_done(j&1): the softmax of step j+1 no longer waits for PV_j (only the
-  // buffer's previous user PV_{j-1}... i.e. step j-2's product, and a rescale of O still waits for everything issued so far)
-  auto p_full = [&](int u) { return s_full0 + 32 + 8u * u; };
-  auto pv_done = [&](int u) { return s_full0 + 48 + 8u * u; };
-  const uint32_t tmem_slot = s_full0 + 64;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qt = blockIdx.x % p.q_tiles;
   const int h = (blockIdx.x / p.q_tiles) % p.heads;
   const int b = blockIdx.x / (p.q_tiles * p.heads);
   int nkv = (p.Nk + FA_BN - 1) / FA_BN;
-  if (p.causal) nkv = min(nkv, (qt * FA_BM + FA_BM + FA_BN - 1) / FA_BN);   // same value in all three roles
+  if (p.causal) nkv = min(nkv, (qt * FA_BM + FA_BM + FA_BN - 1) / FA_BN);   // same value in both roles
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < FA_STAGES; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 1); }
-    for (int u = 0; u < 2; ++u) { mbar_init(s_full(u), 1); mbar_init(s_free(u), 4); }
-    for (int u = 0; u < 2; ++u) { mbar_init(p_full(u), 4); mbar_init(pv_done(u), 1); }
+    for (int s = 0; s < FA_STAGES; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmQ)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmK)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmVt)) : "memory");
   }
-  if (warp < 4) {
-    // constant rows 64..79 of each stage's V^T tile (128-byte rows; all 16-byte chunks of a row are equal, so the 128B swizzle
-    // does not matter): row 64 = ones in the activation dtype, rows 65..79 = zeros
-    const uint32_t one2 = Elem<T>::pack(1.0f, 1.0f);
-    for (int i = threadIdx.x; i < FA_STAGES * (FA_PV_N - FA_D) * 8; i += 128) {
-      const int st = i / ((FA_PV_N - FA_D) * 8), r = (i / 8) % (FA_PV_N - FA_D), ch = i & 7;
-      const uint32_t v = (r == 0) ? one2 : 0u;
-      sts16(sKV + st * FA_KV_STAGE + FA_KV_DATA + r * 128 + ch * 16, v, v, v, v);
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 5) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(tmem_slot) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  pdl_sync();   // prologue (barriers, TMEM, descriptor prefetch) overlaps the previous kernel's tail; no global access before here
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
-  const uint32_t tS0 = tmem_base, tPV = tmem_base + 128;   // S buffers at columns [0,64) and [64,128)
+  pdl_sync();   // prologue (barriers, descriptor prefetch) overlaps the previous kernel's tail; no global access before here
 
-  if (warp == 4) {
+  if (warp == 8) {
     // producer: warp-uniform loop, one elected lane issues the TMA
     if (elect_one()) {
       mbar_expect_tx(q_full, FA_Q_BYTES);
@@ -157,195 +94,102 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
       const int s = j % FA_STAGES;
       mbar_wait(kv_empty(s), ((j / FA_STAGES) & 1) ^ 1, p.err, 11);
       if (elect_one()) {
-        mbar_expect_tx(kv_full(s), FA_KV_DATA);
+        mbar_expect_tx(kv_full(s), FA_KV_STAGE);
         tma_load_5d(sKV + s * FA_KV_STAGE, &tmK, kv_full(s), 0, j * FA_BN, h, b * p.kv_bmul, 0);
         tma_load_5d(sKV + s * FA_KV_STAGE + FA_BN * FA_D * 2, &tmVt, kv_full(s), j * FA_BN, 0, h, b * p.kv_bmul, 0);
       }
       __syncwarp();
     }
-  } else if (warp == 5) {
-    // MMA issuer: warp-uniform loop, one elected lane issues tcgen05.mma / commit
+  } else {
+    // ---------------- consumers: thread (warp w, lane l) holds rows r and r + 8, r = 16 (w % 4) + l / 4 of its warpgroup ----
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int q0 = qt * FA_BM + r0, q1 = q0 + 8;
+    const int klim0 = p.causal ? min(p.Nk, q0 + 1) : p.Nk;     // keys [0, klim) are visible to the row
+    const int klim1 = p.causal ? min(p.Nk, q1 + 1) : p.Nk;
+    const float sc = p.scale_log2e;
+    const int ccol = 2 * (lane & 3);
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running maxima (raw logit units) and row sums
     mbar_wait(q_full, 0, p.err, 12);
-    const uint64_t qdesc = umma_desc_sw128(sQ);
-    const uint32_t idesc_pv = (p.idesc & ~(0x3Fu << 17)) | (static_cast<uint32_t>(FA_PV_N >> 3) << 17);   // same shape, N = 80
-    auto issue_qk = [&](int j) {
+    const uint64_t qdesc = wgmma_desc_sw128(sQ + wg * (64 * 128));
+    for (int j = 0; j < nkv; ++j) {
       const int s = j % FA_STAGES;
       mbar_wait(kv_full(s), (j / FA_STAGES) & 1, p.err, 13);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t kdesc = umma_desc_sw128(sKV + s * FA_KV_STAGE);
+      const uint32_t sK = sKV + s * FA_KV_STAGE, sV = sK + FA_BN * FA_D * 2;
+      float sacc[32];
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < FA_D / 16; ++k)
-          tc_mma_f16(tS0 + 64 * (j & 1), qdesc + 2 * k, kdesc + 2 * k, p.idesc, k > 0 ? 1u : 0u);
-        tc_commit(s_full(j & 1));
-      }
-      __syncwarp();
-    };
-    issue_qk(0);
-    for (int j = 0; j < nkv; ++j) {
-      if (j + 1 < nkv) {
-        // S buffer (j+1)&1 was last read by softmax iteration j-1: QK_{j+1} overlaps the exponentials of iteration j
-        if (j >= 1) { mbar_wait(s_free((j + 1) & 1), ((j - 1) >> 1) & 1, p.err, 14); tc_fence_after(); }
-        issue_qk(j + 1);
-      }
-      mbar_wait(p_full(j & 1), (j >> 1) & 1, p.err, 15);   // P_j is in smem buffer j&1 (and any rescale of O is complete)
-      tc_fence_after();
-      const int s = j % FA_STAGES;
-      if (elect_one()) {
-        const uint64_t vdesc = umma_desc_sw128(sKV + s * FA_KV_STAGE + FA_BN * FA_D * 2);
-        const uint64_t pdesc = umma_desc_sw128(sP + (j & 1) * FA_P_BYTES);
-#pragma unroll
-        for (int k = 0; k < FA_BN / 16; ++k)                 // O accumulates in TMEM across the KV steps
-          tc_mma_f16(tPV, pdesc + 2 * k, vdesc + 2 * k, idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-        tc_commit(pv_done(j & 1));
-        tc_commit(kv_empty(s));                     // K_j and V_j are free once everything issued so far retires
-      }
-      __syncwarp();
-    }
-  } else {
-    // ---------------- softmax / output warps: thread = Q row ----------------
-    const int row = warp * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
-    const int qpos = qt * FA_BM + row;
-    const int klim = p.causal ? min(p.Nk, qpos + 1) : p.Nk;     // keys [0, klim) are visible to this row
-    const float sc = p.scale_log2e;
-    constexpr float TAU = 8.0f;                                  // lazy rescale: P <= 2^8 relative to the reference maximum
-    float m = -INFINITY;                                         // reference maximum (raw logit units) of this row
-    for (int j = 0; j < nkv; ++j) {
-      mbar_wait(s_full(j & 1), (j >> 1) & 1, p.err, 16);
-      tc_fence_after();
-      const uint32_t tS = tS0 + 64 * (j & 1);
+      for (int k = 0; k < FA_D / 16; ++k) wgmma_ss<64, T>(sacc, qdesc + 2 * k, wgmma_desc_sw128(sK) + 2 * k, k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
       const int kbase = j * FA_BN;
-      // element-wise masking only where needed (warp-uniform): the last KV tile, or causal tiles that reach this warp's diagonal
-      const bool ragged = (kbase + FA_BN > p.Nk) || (p.causal && kbase + FA_BN - 1 > qt * FA_BM + warp * 32);
-      // S_j leaves TMEM once: 64 fp32 logits per row in registers; the buffer goes back to the MMA warp right away
-      uint32_t raw[64];
-      {
-        uint32_t (&r0)[32] = *reinterpret_cast<uint32_t (*)[32]>(&raw[0]);
-        uint32_t (&r1)[32] = *reinterpret_cast<uint32_t (*)[32]>(&raw[32]);
-        tc_ld32(tS + lane_off, r0);
-        tc_ld32(tS + lane_off + 32, r1);
-        tc_wait_ld();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_free(j & 1));
-      float mx = -INFINITY;
+      // element-wise masking only where needed: the last KV tile, or causal tiles that reach this warp's diagonal
+      const bool ragged = (kbase + FA_BN > p.Nk) || (p.causal && kbase + FA_BN - 1 > qt * FA_BM + wg * 64 + (warp & 3) * 16);
       if (ragged) {
 #pragma unroll
-        for (int i = 0; i < 64; ++i)
-          if (kbase + i < klim) mx = fmaxf(mx, __uint_as_float(raw[i]));
-      } else {
-        // four independent chains of 3-input maxima (FMNMX3): 34 instructions instead of a 64-deep dependent chain
-        float m4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+        for (int g = 0; g < 8; ++g)
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
-#pragma unroll
-          for (int c4 = 0; c4 < 4; ++c4)
-            m4[c4] = fmax3(m4[c4], __uint_as_float(raw[16 * c4 + 2 * i]), __uint_as_float(raw[16 * c4 + 2 * i + 1]));
-        mx = fmax3(fmaxf(m4[0], m4[1]), m4[2], m4[3]);
+          for (int e = 0; e < 4; ++e)
+            if (kbase + 8 * g + ccol + (e & 1) >= (e < 2 ? klim0 : klim1)) sacc[4 * g + e] = -INFINITY;
       }
-      const bool grow = (fmaxf(m, mx) - m) * sc > TAU;          // first tile: m = -inf -> true
-      if (j == 0) {
-        m = mx;
-      } else if (__any_sync(0xffffffffu, grow)) {
-        // some row of this warp outgrew its reference maximum: rescale the warp's 32 O rows in TMEM (factor 1 for the others).
-        // Every PV issued so far must have landed first: PV_{j-1} is the last one (MMAs retire in order).
-        mbar_wait(pv_done((j - 1) & 1), ((j - 1) >> 1) & 1, p.err, 17);
-        tc_fence_after();
-        const float m_new = grow ? fmaxf(m, mx) : m;
-        const float factor = fast_exp2((m - m_new) * sc);
-        uint32_t o[32];
+      float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          tc_ld32(tPV + lane_off + half * 32, o);
-          tc_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * factor);
-          tc_st32(tPV + lane_off + half * 32, o);
-        }
-        {                                                     // ... and the row-sum column
-          uint32_t lcol[1];
-          tc_ld1(tPV + lane_off + FA_D, lcol);
-          tc_wait_ld();
-          lcol[0] = __float_as_uint(__uint_as_float(lcol[0]) * factor);
-          tc_st1(tPV + lane_off + FA_D, lcol);
-        }
-        tc_wait_st();
-        m = m_new;
+      for (int g = 0; g < 8; ++g) {
+        mx0 = fmaxf(mx0, fmaxf(sacc[4 * g], sacc[4 * g + 1]));
+        mx1 = fmaxf(mx1, fmaxf(sacc[4 * g + 2], sacc[4 * g + 3]));
       }
-      // P buffer j&1 was last read by PV_{j-2}
-      if (j >= 2) mbar_wait(pv_done(j & 1), ((j - 2) >> 1) & 1, p.err, 19);
-      const uint32_t sPj = sP + (j & 1) * FA_P_BYTES;
-      const float neg_ms = -m * sc;
-      // p = exp2(s*scale - m*scale) (one FFMA + one MUFU per element), pack to 16 bit, write the
-      // swizzled K-major P tile
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+      const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+      // a row with no visible key yet keeps m = -inf: factor 1 on its (zero) state, and every p below is exp2(-inf) = 0
+      const float f0 = (mn0 == -INFINITY) ? 1.f : fast_exp2((m0 - mn0) * sc);
+      const float f1 = (mn1 == -INFINITY) ? 1.f : fast_exp2((m1 - mn1) * sc);
+      const float ng0 = (mn0 == -INFINITY) ? 0.f : -mn0 * sc, ng1 = (mn1 == -INFINITY) ? 0.f : -mn1 * sc;
+      m0 = mn0; m1 = mn1;
+      // p = exp2(s*scale - m*scale), packed to 16 bit: pk[2g] is row r (keys 8g + ccol, +1), pk[2g+1] row r + 8
+      uint32_t pk[16];
+      float ls0 = 0.f, ls1 = 0.f;
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        uint32_t pk[16];
-        if (ragged) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int k0 = kbase + half * 32 + 2 * i;
-            const float p0 = (k0 < klim) ? fast_exp2(fmaf(__uint_as_float(raw[half * 32 + 2 * i]), sc, neg_ms)) : 0.f;
-            const float p1 = (k0 + 1 < klim) ? fast_exp2(fmaf(__uint_as_float(raw[half * 32 + 2 * i + 1]), sc, neg_ms)) : 0.f;
-            pk[i] = Elem<T>::pack(p0, p1);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float p0 = fast_exp2(fmaf(__uint_as_float(raw[half * 32 + 2 * i]), sc, neg_ms));
-            const float p1 = fast_exp2(fmaf(__uint_as_float(raw[half * 32 + 2 * i + 1]), sc, neg_ms));
-            pk[i] = Elem<T>::pack(p0, p1);
-          }
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {               // 16-byte group g' = half*4+g holds keys 8g'..8g'+7 of this row
-          const int gg = half * 4 + g;
-          sts16(sPj + row * 128 + ((gg ^ (row & 7)) << 4), pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-        }
+      for (int g = 0; g < 8; ++g) {
+        pk[2 * g] = Elem<T>::pack(fast_exp2(fmaf(sacc[4 * g], sc, ng0)), fast_exp2(fmaf(sacc[4 * g + 1], sc, ng0)));
+        pk[2 * g + 1] = Elem<T>::pack(fast_exp2(fmaf(sacc[4 * g + 2], sc, ng1)), fast_exp2(fmaf(sacc[4 * g + 3], sc, ng1)));
+        const float2 a = Elem<T>::unpack(pk[2 * g]), c = Elem<T>::unpack(pk[2 * g + 1]);
+        ls0 += a.x + a.y;
+        ls1 += c.x + c.y;
       }
-      // P_j visible to the async proxy (and any O rescale complete) -> PV_j may start
-      tc_fence_before();
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      ls0 += __shfl_xor_sync(0xffffffffu, ls0, 1); ls0 += __shfl_xor_sync(0xffffffffu, ls0, 2);
+      ls1 += __shfl_xor_sync(0xffffffffu, ls1, 1); ls1 += __shfl_xor_sync(0xffffffffu, ls1, 2);
+      l0 = l0 * f0 + ls0;
+      l1 = l1 * f1 + ls1;
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        o[4 * g] *= f0; o[4 * g + 1] *= f0;
+        o[4 * g + 2] *= f1; o[4 * g + 3] *= f1;
+      }
+      // O += P V: keys [16kk, 16kk+16) of P are the A fragment {row r k, row r+8 k, row r k+8, row r+8 k+8}
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < FA_BN / 16; ++kk) {
+        const uint32_t a[4] = {pk[4 * kk], pk[4 * kk + 1], pk[4 * kk + 2], pk[4 * kk + 3]};
+        wgmma_rs64<T>(o, a, wgmma_desc_sw128(sV) + 2 * kk);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive(p_full(j & 1));
+      if (lane == 0) mbar_arrive(kv_empty(s));                 // K_j and V_j have been read by this warp's MMAs
     }
-    // last PV, then the only read of O
-    mbar_wait(pv_done((nkv - 1) & 1), ((nkv - 1) >> 1) & 1, p.err, 18);
-    tc_fence_after();
-    const int q = qt * FA_BM + row;
-    float inv;
-    {
-      uint32_t lcol[1];
-      tc_ld1(tPV + lane_off + FA_D, lcol);
-      tc_wait_ld();
-      inv = 1.0f / __uint_as_float(lcol[0]);
-    }
-    T* optr = reinterpret_cast<T*>(p.out) + (static_cast<long long>(b) * p.Nq + q) * p.ldo + h * FA_D;
+    const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+    T* const obase = reinterpret_cast<T*>(p.out) + static_cast<long long>(b) * p.Nq * p.ldo + h * FA_D + ccol;
 #pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      uint32_t o[32];
-      tc_ld32(tPV + lane_off + half * 32, o);
-      tc_wait_ld();
-      if (q < p.Nq) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 u;
-          u.x = Elem<T>::pack(__uint_as_float(o[8 * g]) * inv, __uint_as_float(o[8 * g + 1]) * inv);
-          u.y = Elem<T>::pack(__uint_as_float(o[8 * g + 2]) * inv, __uint_as_float(o[8 * g + 3]) * inv);
-          u.z = Elem<T>::pack(__uint_as_float(o[8 * g + 4]) * inv, __uint_as_float(o[8 * g + 5]) * inv);
-          u.w = Elem<T>::pack(__uint_as_float(o[8 * g + 6]) * inv, __uint_as_float(o[8 * g + 7]) * inv);
-          st16(optr + half * 32 + 8 * g, u);
-        }
-      }
+    for (int g = 0; g < 8; ++g) {
+      if (q0 < p.Nq)
+        *reinterpret_cast<uint32_t*>(obase + q0 * p.ldo + 8 * g) = Elem<T>::pack(o[4 * g] * inv0, o[4 * g + 1] * inv0);
+      if (q1 < p.Nq)
+        *reinterpret_cast<uint32_t*>(obase + q1 * p.ldo + 8 * g) = Elem<T>::pack(o[4 * g + 2] * inv1, o[4 * g + 3] * inv1);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem_base) : "memory");
   }
 }
 

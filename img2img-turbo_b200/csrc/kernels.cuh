@@ -9,7 +9,7 @@ namespace i2it {
 // =============================================================================================
 // GroupNorm (+SiLU)   — replaces ATen group_norm + silu at every norm1/norm2/conv_norm_out/
 // Transformer2DModel.norm/attn.group_norm under the reference's vae.encode/unet/vae.decode calls
-// (/root/reference/src/pix2pix_turbo.py:198-203).  Two launches: statistics (from the producing GEMM's epilogue partials, or
+// (src/pix2pix_turbo.py:198-203).  Two launches: statistics (from the producing GEMM's epilogue partials, or
 // one pass over the tensor; deterministic; the last block finalises in double) and apply.
 // =============================================================================================
 template <typename T>
@@ -362,7 +362,7 @@ __global__ void softmax_long_kernel(const float* __restrict__ s, long long lds, 
 
 // =============================================================================================
 // CLIP text embeddings: out[b, t, :] = token_embedding[ids[b, t]] + position_embedding[t]   (fp32 add, one rounding)
-// (transformers models/clip/modeling_clip.py CLIPTextEmbeddings.forward; reference call /root/reference/src/pix2pix_turbo.py:190-196)
+// (transformers models/clip/modeling_clip.py CLIPTextEmbeddings.forward; reference call src/pix2pix_turbo.py:190-196)
 // =============================================================================================
 template <typename T>
 __global__ void clip_embed_kernel(const int* __restrict__ ids, const float* __restrict__ tok, const float* __restrict__ pos,
@@ -432,9 +432,9 @@ __global__ void pack_input_im2col_kernel(const T* __restrict__ x, T* __restrict_
 }
 
 // uint8 HWC boundary (SURVEY section 8f #3).  Input: what the reference CLIs do on the host before the forward —
-//   mode 0  F.to_tensor(img)                      v = u8/255                      (/root/reference/src/inference_paired.py:50)
-//   mode 1  ToTensor + Normalize([0.5],[0.5])     v = (u8/255 - 0.5)/0.5          (/root/reference/src/inference_unpaired.py:45-47)
-//   mode 2  (F.to_tensor(img) < 0.5).float()      v = u8/255 < 0.5 ? 1 : 0        (/root/reference/src/inference_paired.py:56-57)
+//   mode 0  F.to_tensor(img)                      v = u8/255                      (src/inference_paired.py:50)
+//   mode 1  ToTensor + Normalize([0.5],[0.5])     v = (u8/255 - 0.5)/0.5          (src/inference_unpaired.py:45-47)
+//   mode 2  (F.to_tensor(img) < 0.5).float()      v = u8/255 < 0.5 ? 1 : 0        (src/inference_paired.py:56-57)
 // in fp32 followed by the .half()/.to(dtype) rounding — fused with the im2col packing of encoder.conv_in.
 __device__ __forceinline__ float u8_to_input(uint8_t q, int mode) {
   const float v = static_cast<float>(q) / 255.0f;
@@ -470,8 +470,8 @@ __global__ void pack_input_im2col_u8_kernel(const uint8_t* __restrict__ x /*[B,H
     st16(y + i * 32 + g * 8, make_uint4(Elem<T>::pack(v[8 * g], v[8 * g + 1]), Elem<T>::pack(v[8 * g + 2], v[8 * g + 3]),
                                         Elem<T>::pack(v[8 * g + 4], v[8 * g + 5]), Elem<T>::pack(v[8 * g + 6], v[8 * g + 7])));
 }
-// Output: transforms.ToPILImage()(output_image[0].cpu() * 0.5 + 0.5)  (/root/reference/src/inference_paired.py:72,
-// /root/reference/src/inference_unpaired.py:53): three ops in the activation dtype (x*0.5, +0.5, .mul(255)), each rounded, then
+// Output: transforms.ToPILImage()(output_image[0].cpu() * 0.5 + 0.5)  (src/inference_paired.py:72,
+// src/inference_unpaired.py:53): three ops in the activation dtype (x*0.5, +0.5, .mul(255)), each rounded, then
 // .byte() (truncation).  NCHW [B,3,H,W] -> HWC uint8 [B,H,W,3].
 template <typename T>
 __global__ void nchw_to_u8hwc_kernel(const T* __restrict__ x, uint8_t* __restrict__ y, long long HW, long long total) {
@@ -489,7 +489,7 @@ __global__ void nchw_to_u8hwc_kernel(const T* __restrict__ x, uint8_t* __restric
 }
 
 // DiagonalGaussianDistribution.sample() * scaling_factor (+ the stochastic blend of
-// /root/reference/src/pix2pix_turbo.py:210): moments NHWC (ld) -> latent NHWC8 (channels 4..7 zero).
+// src/pix2pix_turbo.py:210): moments NHWC (ld) -> latent NHWC8 (channels 4..7 zero).
 template <typename T>
 __global__ void latent_sample_kernel(const T* __restrict__ mom, int ldm, const T* __restrict__ eps_nchw,
                                      const T* __restrict__ noise_nchw, float r, float sf, T* __restrict__ z,
@@ -517,13 +517,13 @@ __global__ void latent_sample_kernel(const T* __restrict__ mom, int ldm, const T
 }
 
 // DDPMScheduler.step closed form at t=999 and the `/ scaling_factor` feeding vae.decode
-// (/root/reference/src/pix2pix_turbo.py:200-203): x0 = (x - s1*eps_hat)/sa.
+// (src/pix2pix_turbo.py:200-203): x0 = (x - s1*eps_hat)/sa.
 //   three_round == 0  Pix2Pix_Turbo: `timesteps` is a 1-D tensor, so alphas_cumprod[t] is a dimensioned fp32 tensor and the
 //                     whole step is promoted to fp32, then rounded once by .to(model_pred.dtype)  (pix2pix_turbo.py:162,200-201)
 //   three_round == 1  CycleGAN_Turbo: `timesteps[i]` is 0-dim, so alphas_cumprod[t] (moved to the GPU by make_1step_sched,
-//                     /root/reference/src/model.py:10) is a 0-dim CUDA fp32 tensor: it does not promote the fp16/bf16 operands,
+//                     src/model.py:10) is a 0-dim CUDA fp32 tensor: it does not promote the fp16/bf16 operands,
 //                     torch casts it to the activation dtype and every op rounds: c1 = round(s1), c2 = round(sa);
-//                     round(c1*e), round(x - .), round(. / c2) with fp32 op-math  (/root/reference/src/cyclegan_turbo.py:205).
+//                     round(c1*e), round(x - .), round(. / c2) with fp32 op-math  (src/cyclegan_turbo.py:205).
 //                     tests/test_gpu_boundary.py checks this bit for bit against the same torch expression on the GPU.
 template <typename T>
 __global__ void ddpm_step_kernel(const T* __restrict__ zin /*NHWC8*/, const T* __restrict__ pred, int ldp,

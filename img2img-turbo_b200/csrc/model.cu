@@ -1,10 +1,10 @@
 // The model graph of the hot path, appended op by op to a Plan (static shapes => one CUDA graph).
 //
 // Mirrors, layer for layer, what the reference executes through diffusers 0.25.1:
-//   VAE encoder  : my_vae_encoder_fwd        /root/reference/src/model.py:14-27   (+ quant_conv, posterior sample)
-//   UNet         : UNet2DConditionModel call /root/reference/src/pix2pix_turbo.py:199 (SD-Turbo config, t == 999)
-//   DDPM step    : sched.step                /root/reference/src/pix2pix_turbo.py:200 (closed form)
-//   VAE decoder  : my_vae_decoder_fwd        /root/reference/src/model.py:30-54   (skip convs, gamma)
+//   VAE encoder  : my_vae_encoder_fwd        src/model.py:14-27   (+ quant_conv, posterior sample)
+//   UNet         : UNet2DConditionModel call src/pix2pix_turbo.py:199 (SD-Turbo config, t == 999)
+//   DDPM step    : sched.step                src/pix2pix_turbo.py:200 (closed form)
+//   VAE decoder  : my_vae_decoder_fwd        src/model.py:30-54   (skip convs, gamma)
 // with LoRA folded into the weights, the time embedding folded into conv1 biases, TwinConv blended, and
 // NHWC activations so that [B,H,W,C] == [B, HW, C] tokens (no permutes around the transformer blocks).
 #include "engine.cuh"

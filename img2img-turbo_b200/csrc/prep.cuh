@@ -4,8 +4,8 @@
 //
 // Per output element:  v = scale * ( c0*W0[o,i,t] + c1*W1[o,i,t] + sum_a s_a * sum_r B_a[o,r] * A_a[r,i,t] )   in fp32,
 // one rounding to the activation dtype.  Replaces peft's runtime LoRA branches (y = Wx + s*B(A(x)), ~1000 extra
-// kernels per forward in the reference: /root/reference/src/pix2pix_turbo.py:67-78,137-151,
-// /root/reference/src/cyclegan_turbo.py:48-106) and TwinConv (/root/reference/src/pix2pix_turbo.py:16-26).
+// kernels per forward in the reference: src/pix2pix_turbo.py:67-78,137-151,
+// src/cyclegan_turbo.py:48-106) and TwinConv (src/pix2pix_turbo.py:16-26).
 #pragma once
 #include "common.cuh"
 

@@ -7,60 +7,54 @@
 // are all the same implicit GEMM.  Zero padding, ragged edges and channel padding come from TMA
 // out-of-bounds zero fill, never from materialised copies.
 //
-// sm_100a structure (one persistent CTA per SM, 192 threads):
-//   warp 8        : TMA producer   cp.async.bulk.tensor.5d -> 128B-swizzled smem ring (4 stages)
-//   warp 9        : MMA issuer     tcgen05.mma.cta_group::1.kind::f16, M=128, N=BN<=256, K=16
-//                                  accumulators in TMEM (2 stages x 256 fp32 columns)
-//   warps 0..7    : epilogue       tcgen05.ld 32x32b -> bias/residual/GEGLU/clamp -> global
-//   mbarriers     : full/empty per smem stage, tmem_full/tmem_empty per accumulator stage
+// sm_90a structure (one persistent CTA per SM, 384 threads):
+//   warp 8        : TMA producer   cp.async.bulk.tensor.5d -> 128B-swizzled smem ring (4 stages at BN = 256)
+//   warps 0..7    : two consumer warpgroups; warpgroup g owns tile rows [64g, 64g+64):
+//                   mainloop  wgmma.mma_async m64nNk16 (N = 64 blocks, or 16 blocks when BN is not a multiple of 64),
+//                             fp32 accumulators in registers
+//                   epilogue  accumulators -> fp32 staging tile in smem (aliases the operand ring) -> one accumulator ROW per
+//                             thread -> bias/residual/GEGLU/clamp -> TMA store boxes or direct stores
+//   mbarriers     : full/empty per smem stage; epi_done holds the producer off the ring while it is the staging tile
 //
-// Replaces (reference call sites): every nn.Conv2d / nn.Linear / SDPA matmul under
-// vae.encode / unet(...) / vae.decode at /root/reference/src/pix2pix_turbo.py:198-203, which
-// dispatch to cuDNN implicit GEMM, cuBLAS and flash/mem-efficient SDPA in the reference stack.
+// Replaces every nn.Conv2d / nn.Linear / SDPA matmul under vae.encode / unet(...) / vae.decode of the reference
+// pipeline, which dispatch to cuDNN implicit GEMM, cuBLAS and flash/mem-efficient SDPA in the reference stack.
 #pragma once
 #include "common.cuh"
 
 namespace i2it {
 
-constexpr int TG_BM = 128;             // rows per tile (= TMEM lanes)
+constexpr int TG_BM = 128;             // rows per tile (two m64 warpgroup slabs)
 constexpr int TG_BK = 64;              // K elements per stage (= 128 B = one swizzle atom)
 constexpr int TG_STAGES = 4;            // stages when the B tile is the full 32 KiB; smaller tiles get more (<= TG_MAX_STAGES)
-#ifndef I2IT_MAX_STAGES
-#define I2IT_MAX_STAGES 16          // `make STAGES8=1` builds the round-1 ring depth (8) into its own library for A/B runs
-#endif
-constexpr int TG_MAX_STAGES = I2IT_MAX_STAGES;   // small B tiles (BN <= 128) need more stages for the same lookahead in TIME
+constexpr int TG_MAX_STAGES = 16;       // small B tiles (BN <= 128) need more stages for the same lookahead in TIME
 constexpr int TG_MAX_TAPS = 16;
 constexpr int TG_A_STAGE = TG_BM * TG_BK * 2;    // 16 KiB
 constexpr int TG_B_STAGE = 256 * TG_BK * 2;      // 32 KiB (BN <= 256)
-#ifndef I2IT_EPI_WARPS
-#define I2IT_EPI_WARPS 8               // build-time: 8 (default) or 16 (`make EPI16=1`, experimental wide epilogue; see DESIGN §8)
-#endif
-constexpr int TG_EPI_WARPS = I2IT_EPI_WARPS;   // TG_EPI_GROUPS warps per TMEM lane quarter: they take the 32-column rounds in turn
-constexpr int TG_EPI_GROUPS = TG_EPI_WARPS / 4;
-constexpr int TG_EPI_RPW = 8 / TG_EPI_GROUPS;      // rounds per warp at BN = 256
-static_assert(TG_EPI_WARPS == 8, "epilogue warps: 8 (the 16-warp experiment of round 1 does not fit next to the 4 KB store boxes)");
+constexpr int TG_EPI_WARPS = 8;                  // the two consumer warpgroups
+constexpr int TG_EPI_GROUPS = TG_EPI_WARPS / 4;  // warps per 32-row quarter: they take the 32-column rounds in turn
+constexpr int TG_EPI_RPW = 8 / TG_EPI_GROUPS;    // rounds per warp at BN = 256
 constexpr int TG_BAR_BYTES = 512;
-constexpr int TG_BIAS_BYTES = 2 * 256 * 4;       // per-tile bias slice, double-buffered like the accumulators
+constexpr int TG_BIAS_BYTES = 2 * 256 * 4;       // per-tile bias slice, double-buffered across tiles
 // Epilogue store staging: each epilogue warp owns ONE TMA box = 32 rows x 64 output columns (128-byte rows, SWIZZLE_128B: the
 // 16-byte chunk c of row r lives at r*128 + ((c ^ (r & 7)) << 4)).  A thread holds one accumulator ROW, so direct stores touch 32
-// different lines per instruction (r01 trace: ~6000 cycles of LSU transactions per 128x160 tile, the limiter of every
-// K <= ~1152 GEMM).  Through the box the thread writes its row with conflict-free st.shared.v4 and ONE elected lane hands the
-// 4 KB box to the TMA unit (cp.async.bulk.tensor...global.shared::cta = UTMASTG), which writes full lines and clips ragged edges.
-// The residual takes the same road in reverse: coalesced 16-byte global loads (4 rows x 128 B per instruction), transposed
-// through the box, added in place.
+// different lines per instruction.  Through the box the thread writes its row with conflict-free st.shared.v4 and ONE elected
+// lane hands the 4 KB box to the TMA unit, which writes full lines and clips ragged edges.  The residual takes the same road in
+// reverse: coalesced 16-byte global loads (4 rows x 128 B per instruction), transposed through the box, added in place.
 constexpr int TG_OSTG_WARP = 32 * 128;
 constexpr int TG_OSTG_BYTES = TG_EPI_WARPS * TG_OSTG_WARP;
 // manual 1024-byte alignment slack of the dynamic smem base: 512 B are budgeted (a full 1 KB would put the CTA over the
 // 227 KB limit) and the kernels trap with an error word if the runtime base needs more (it is 1 KB aligned in practice).
 constexpr int TG_ALIGN_PAD = 512;
 constexpr int TG_SMEM = TG_STAGES * (TG_A_STAGE + TG_B_STAGE) + TG_BAR_BYTES + TG_BIAS_BYTES + TG_OSTG_BYTES + TG_ALIGN_PAD;
-// + TMA producer warp + MMA issuer warp.  Register reallocation (setmaxnreg) was tried: with two idle warps completing the third
-// warpgroup the epilogue warpgroups can grow to 224 registers while the control warps drop to 64, but ptxas then spills the
-// control roles' hoisted parameter loads (0.5..5 KB of spill traffic depending on the split), so it is compiled out
-// (TG_REGS_EPI = 0); the epilogue fits in the 168 registers a 10-warp CTA gets with ~40 B of spills per round.
-constexpr int TG_REGS_EPI = 0, TG_REGS_CTRL = 64;
-constexpr int TG_THREADS = (TG_EPI_WARPS + (TG_REGS_EPI > 0 ? 4 : 2)) * 32;
-constexpr int TG_ACC_COLS = 256;       // TMEM columns per accumulator stage
+// + one producer warpgroup (warp 8 issues the TMA loads, warps 9..11 idle).  Registers are allocated per warpgroup, so the
+// producer warpgroup gives its registers to the consumers (setmaxnreg): 128 x 40 + 256 x 232 <= 64 K.
+constexpr int TG_THREADS = (TG_EPI_WARPS + 4) * 32;
+constexpr int TG_REGS_PRODUCER = 40, TG_REGS_CONSUMER = 232;
+// fp32 accumulator staging: 128 rows x (BN + 4) floats.  BN is a multiple of 16, so the row pitch is 4 mod 8 words and eight
+// consecutive rows hit eight different 16-byte bank groups (conflict-free row reads).  It lives at the start of the operand ring
+// and must stay clear of the second set of store boxes, which takes the ring's last 32 KB.
+constexpr int TG_STG_BYTES = TG_BM * (256 + 4) * 4;
+static_assert(TG_STG_BYTES <= TG_STAGES * (TG_A_STAGE + TG_B_STAGE) - TG_OSTG_BYTES, "accumulator staging must fit the ring");
 
 enum TgAct : int { TG_ACT_NONE = 0, TG_ACT_CLAMP1 = 1, TG_ACT_GEGLU = 2, TG_ACT_GELU = 3, TG_ACT_QUICKGELU = 4 };   // 3, 4: CLIP MLP
 enum TgBias : int { TG_BIAS_NONE = 0, TG_BIAS_COL = 1, TG_BIAS_ROW = 2 };
@@ -78,11 +72,12 @@ struct TapGemmParams {
   int tap_kc[TG_MAX_TAPS];  // K chunks (of 64) for this tap
   int nprim;                // the first nprim taps share kchunks and are walked k-chunk-outer / tap-inner (same
                             // accumulation order in every kernel variant => bit-identical results); the rest follow
-  int stages, b_stage;      // smem ring: number of stages and bytes per B stage (sized to the actual tile, <= 8 stages)
-  int halo;                 // pair kernel only: 3x3 taps read shifted views of ONE halo tile per k-chunk
+  int stages, b_stage;      // smem ring: number of stages and bytes per B stage (sized to the actual tile, <= TG_MAX_STAGES)
+  int layout_pad0;          // unused; see layout_pad1
   int tap_a[TG_MAX_TAPS][5];
   int tap_b[TG_MAX_TAPS][4];
-  uint32_t idesc;
+  uint32_t layout_pad1;     // unused.  Removing these two words moves every later field by 8 bytes, and with it ptxas's
+                            // register allocation of the (spilling) tapgemm_kernel: -36 % images/s, measured A/B on one H100
   // ---- epilogue ----
   void* out;
   long long ostride[4];   // elements
@@ -103,11 +98,11 @@ struct TapGemmParams {
   // GroupNorm statistics of the OUTPUT tensor, taken from the staged (rounded) tile: per 32-row slot and per `gn_red` columns,
   // (sum, sum of squares) -> gn_part[(slot0 + m_tile*4 + quarter) * (N/gn_red) + col/gn_red][2]; nullptr = off
   float* gn_part;
-  // split-K (1-CTA kernel only): the primary taps' k-chunks are divided over `ksplit` tiles that write fp32 partials
+  // split-K: the primary taps' k-chunks are divided over `ksplit` tiles that write fp32 partials
   // `split_ostride` elements apart (splitk_reduce_kernel sums them in a fixed order); secondary taps go with split 0
   int ksplit, kc_per;
   long long split_ostride;
-  int gn_red, gn_slot0, gn_mtiles;   // gn_mtiles: m-tiles of the launch (the pair kernel's odd tail tile has no slot)
+  int gn_red, gn_slot0, gn_mtiles;   // gn_mtiles: m-tiles of the launch
   int gn_shift;                      // log2(gn_red)
   // tile decode without integer division: magic[i] = floor(2^32 / d_i) + 1 for d = (n_tiles, tdim[0..3]); exact while
   // tile * d < 2^32 (the host refuses larger tile spaces)
@@ -187,45 +182,51 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// register reallocation between warpgroups (all four warps of a warpgroup execute the same instruction)
-template <int N> __device__ __forceinline__ void reg_inc() { if (N >= 24) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N >= 24 ? N : 24)); }
+// ---- Hopper warpgroup MMA (all four warps of a warpgroup execute these together) ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
-
-// K-major, 128B-swizzled operand tile: rows of 128 B, 8-row groups 1024 B apart (SBO), start address
-// advanced by 32 B per UMMA_K=16 step inside the swizzle atom.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-  uint64_t d = static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;   // stride byte offset between 8-row core-matrix groups
-  d |= static_cast<uint64_t>(1) << 46;           // descriptor version (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;           // SWIZZLE_128B
-  return d;
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in 128B-swizzled smem; acc == 0 overwrites D.
+// Fragment of D: register 4*g + e of thread (warp w, lane l) is row 16w + l/4 + 8*(e >> 1), column 8g + 2*(l % 4) + (e & 1).
+template <int N, typename T> __device__ __forceinline__ void wgmma_ss(float* d, uint64_t a, uint64_t b, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma_ss<64, __half>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(acc));
 }
-
-// host: instruction descriptor for kind::f16 (A,B fp16 or bf16 K-major, D fp32), M=128, N=bn
-inline uint32_t make_idesc(int dtype, int bn) {
-  uint32_t fmt = (dtype == DT_BF16) ? 1u : 0u;
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (static_cast<uint32_t>(bn >> 3) << 17) | ((128u >> 4) << 24);
+template <> __device__ __forceinline__ void wgmma_ss<64, __nv_bfloat16>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_ss<16, __half>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_ss<16, __nv_bfloat16>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(acc));
+}
+// K-major, 128B-swizzled operand tile for wgmma: rows of 128 B, 8-row groups 1024 B apart (SBO), start address advanced by
+// 32 B (+2 in the descriptor) per K = 16 step inside the swizzle atom.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
+  uint64_t d = static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;           // leading byte offset (unused for swizzled K-major)
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;   // stride byte offset between 8-row core-matrix groups
+  d |= static_cast<uint64_t>(1) << 62;           // SWIZZLE_128B
+  return d;
 }
 
 __device__ __forceinline__ void sts16(uint32_t saddr, const uint4& u) {
@@ -361,10 +362,10 @@ __device__ __forceinline__ void epilogue_chunk(const TapGemmParams& p, const uin
   }
 }
 
-// The whole epilogue of one output tile for one thread (= one accumulator row).  Shared by the 1-CTA and the 2-CTA kernels.
-// Caller signals tmem_empty afterwards.  Two paths, chosen per launch on the host:
+// The whole epilogue of one output tile for one thread (= one accumulator row, read from the fp32 staging tile at `arow`).
+// Two paths, chosen per launch on the host:
 //   * tma_out: 64-column rounds -> this warp's swizzled 4 KB box in smem -> one TMA store per round (see TG_OSTG_WARP);
-//     the residual is fetched with coalesced loads before the accumulator wait and added from the box; optional GroupNorm
+//     the residual is fetched with coalesced loads and added from the box; optional GroupNorm
 //     statistics of the rounded output come from the box as well;
 //   * direct: each thread stores its own row (fp32 logits, NCHW image, row-bias V^T, channel counts that are not multiples of 64).
 // LEAN (compile time): the launch takes the TMA-store path with no activation (every conv / linear of the path except the GEGLU,
@@ -372,13 +373,13 @@ __device__ __forceinline__ void epilogue_chunk(const TapGemmParams& p, const uin
 // code, fewer instruction-cache misses (17 % of the r02g stall samples were no_inst).
 template <typename T, bool LEAN>
 __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUtensorMap* tmO, const TileCoord& c, int m_tile,
-                                              int row, int warp, int j1, int j2, int j3, int j4, int acc, int aphase,
-                                              uint32_t tmem_base, float* s_bias, uint32_t ostg_base, uint32_t ostg2_base,
-                                              int& box_sel, uint32_t tfull_bar_addr, bool stage_bias, bool stamp = false) {
+                                              int row, int warp, int j1, int j2, int j3, int j4, int acc, uint32_t arow,
+                                              float* s_bias, uint32_t ostg_base, uint32_t ostg2_base, int& box_sel,
+                                              bool stage_bias, bool stamp = false) {
   const int lane = threadIdx.x & 31;
   // this warp's store box(es), 1024-byte aligned; with two boxes the warp alternates per round (box_sel persists across tiles)
   const uint32_t ostg_w0 = ostg_base + warp * TG_OSTG_WARP, ostg_w1 = p.ostg2 ? ostg2_base + warp * TG_OSTG_WARP : ostg_w0;
-  const int grp = warp >> 2;                     // which of the two warps sharing this TMEM lane quarter
+  const int grp = warp >> 2;                     // which of the two warps sharing this 32-row quarter
   const int g1 = c.t[0] * p.box[0] + j1, g2 = c.t[1] * p.box[1] + j2, g3 = c.t[2] * p.box[2] + j3,
             g4 = c.t[3] * p.box[3] + j4;
   const bool row_ok = (g1 < p.ext[0]) && (g2 < p.ext[1]) && (g3 < p.ext[2]) && (g4 < p.ext[3]);
@@ -395,7 +396,13 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
     asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");   // the epilogue warps only
   }
   if (stamp) tg_stamp(p, 7);
-  const uint32_t taddr = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16) + acc * TG_ACC_COLS;
+  auto acc_ld16 = [&](int col, uint32_t (&r)[16]) {          // accumulator columns [col, col+16) of this thread's row
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint4 u = lds16(arow + (col + 4 * i) * 4);
+      r[4 * i] = u.x; r[4 * i + 1] = u.y; r[4 * i + 2] = u.z; r[4 * i + 3] = u.w;
+    }
+  };
   const bool geglu = !LEAN && p.act == TG_ACT_GEGLU;
 
   if (LEAN || p.tma_out) {
@@ -403,8 +410,7 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
     const int acols = geglu ? 128 : 64;                       // accumulator columns per round
     const int nrounds = p.BN >> (geglu ? 7 : 6);              // host guarantees BN % acols == 0 and N % acols == 0
     const bool res_on = p.res != nullptr && !geglu;
-    // Residual prefetch: independent of the accumulator, so it is requested BEFORE the accumulator wait and its latency
-    // overlaps the mainloop.  Instruction i loads rows 4i..4i+3 of the warp's 32 (8 lanes x 16 B = one full 128-byte row
+    // Residual prefetch: one round ahead, so its latency overlaps the previous round's math.  Instruction i loads rows 4i..4i+3 of the warp's 32 (8 lanes x 16 B = one full 128-byte row
     // segment each) -> 4 fully used lines per instruction instead of 32 half-used sectors.
     uint4 rq[8];
     const int lrow = lane >> 3, lch = lane & 7;
@@ -421,8 +427,6 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
       }
     };
     if (res_on) load_res(grp);
-    mbar_wait(tfull_bar_addr, aphase, p.err, 4);
-    tc_fence_after();
     if (stamp) tg_stamp(p, 8);
     const int sw = lane & 7;
 #pragma unroll
@@ -447,8 +451,7 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
         if (r + TG_EPI_GROUPS < nrounds) load_res(r + TG_EPI_GROUPS);   // next round's residual: in flight during this round's math
       }
       const int nq = geglu ? 4 : 2;
-      // 32 accumulator columns per step, software-pipelined: the TMEM load of step q+1 is in flight during the math of step q
-      // (tcgen05.wait::ld waits for ALL outstanding loads, so the next load is issued right after the wait)
+      // 32 accumulator columns per step, in two register buffers
       uint32_t xa0[16], xa1[16], xb0[16], xb1[16];       // two 32-column register buffers
       auto step = [&](int q, const uint32_t (&raw0)[16], const uint32_t (&raw1)[16]) {
         const uint32_t sbq_s = smem_u32(sb + c0 + 32 * q);      // 16-byte aligned: the bias slice comes in as ld.shared.v4
@@ -517,18 +520,14 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
           }
         }
       };
-      tc_ld16(taddr + c0, xa0); tc_ld16(taddr + c0 + 16, xa1);
-      tc_wait_ld();
-      tc_ld16(taddr + c0 + 32, xb0); tc_ld16(taddr + c0 + 48, xb1);
+      acc_ld16(c0, xa0); acc_ld16(c0 + 16, xa1);
+      acc_ld16(c0 + 32, xb0); acc_ld16(c0 + 48, xb1);
       step(0, xa0, xa1);
-      tc_wait_ld();
-      if (!LEAN && nq > 2) { tc_ld16(taddr + c0 + 64, xa0); tc_ld16(taddr + c0 + 80, xa1); }   // warp-uniform (GEGLU rounds)
+      if (!LEAN && nq > 2) { acc_ld16(c0 + 64, xa0); acc_ld16(c0 + 80, xa1); }   // warp-uniform (GEGLU rounds)
       step(1, xb0, xb1);
       if (!LEAN && nq > 2) {
-        tc_wait_ld();
-        tc_ld16(taddr + c0 + 96, xb0); tc_ld16(taddr + c0 + 112, xb1);
+        acc_ld16(c0 + 96, xb0); acc_ld16(c0 + 112, xb1);
         step(2, xa0, xa1);
-        tc_wait_ld();
         step(3, xb0, xb1);
       }
       fence_async_smem();                                    // generic-proxy writes -> visible to the TMA unit
@@ -594,8 +593,8 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
   // ================= direct path =================
   const long long obase = g1 * p.ostride[0] + g2 * p.ostride[1] + g3 * p.ostride[2] + g4 * p.ostride[3] + c.split * p.split_ostride;
   const float rbias = (p.bias_mode == TG_BIAS_ROW && row_ok) ? p.bias[g1] : 0.0f;
-  // Residual reads do not depend on the accumulator: this thread's WHOLE residual slice (its row x the 32-column rounds
-  // r = grp, grp+2, ...; <= 256 B) is requested before the accumulator wait, so global-load latency overlaps the mainloop.
+  // This thread's WHOLE residual slice (its row x the 32-column rounds r = grp, grp+2, ...; <= 256 B) is requested up front,
+  // so the global loads are in flight together.
   const int nrounds = (p.BN + 31) >> 5;
   const bool res_on = p.res != nullptr && row_ok && p.rcol == 1 && !geglu;
   uint4 rq[TG_EPI_RPW][4];
@@ -616,8 +615,6 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
     }
   }
 
-  mbar_wait(tfull_bar_addr, aphase, p.err, 4);
-  tc_fence_after();
   if (stamp) tg_stamp(p, 8);
 
 #pragma unroll
@@ -627,10 +624,8 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
     const int c0 = 32 * r;
     const int nch = min(2, (p.BN - c0) >> 4);
     uint32_t raw0[16], raw1[16];
-    __syncwarp();                                // tcgen05.ld is .sync.aligned: reconverge after the guarded stores
-    tc_ld16(taddr + c0, raw0);
-    if (nch == 2) tc_ld16(taddr + c0 + 16, raw1);
-    tc_wait_ld();
+    acc_ld16(c0, raw0);
+    if (nch == 2) acc_ld16(c0 + 16, raw1);
     const int col0 = n0 + c0;
     if (row_ok) {
       if (col0 < p.N) epilogue_chunk<T>(p, raw0, col0, obase, rbase, rbias, sb + c0, fast[i], rq[i][0], rq[i][1]);
@@ -660,9 +655,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const uint32_t bars = ostg + TG_OSTG_BYTES;
   auto full_bar = [&](int s) { return bars + 8u * s; };
   auto empty_bar = [&](int s) { return bars + 8u * (TG_MAX_STAGES + s); };
-  auto tfull_bar = [&](int a) { return bars + 8u * (2 * TG_MAX_STAGES + a); };
-  auto tempty_bar = [&](int a) { return bars + 8u * (2 * TG_MAX_STAGES + 2 + a); };
-  const uint32_t tmem_slot = bars + 8u * (2 * TG_MAX_STAGES + 4);
+  const uint32_t epi_done = bars + 8u * (2 * TG_MAX_STAGES);
   float* const s_bias = reinterpret_cast<float*>(smem_raw + (bars - smem_u32(smem_raw)) + TG_BAR_BYTES);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -674,8 +667,8 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   for (int t = p.nprim; t < p.num_taps; ++t) sec_steps += p.tap_kc[t];
 
   if (warp == TG_EPI_WARPS && lane == 0) {
-    for (int s = 0; s < NS; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), TG_EPI_WARPS); }
+    for (int s = 0; s < NS; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TG_EPI_WARPS); }
+    mbar_init(epi_done, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
@@ -683,31 +676,23 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB2)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmO)) : "memory");
   }
-  if (warp == TG_EPI_WARPS + 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(tmem_slot) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  pdl_sync();   // prologue (barriers, TMEM, descriptor prefetch) overlaps the previous kernel's tail; no global access before here
+  pdl_sync();   // prologue (barriers, descriptor prefetch) overlaps the previous kernel's tail; no global access before here
   if (threadIdx.x == 0) tg_stamp(p, 1);
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
-  if (TG_REGS_EPI > 0) { if (warp >= TG_EPI_WARPS) reg_dec<TG_REGS_CTRL>(); else reg_inc<TG_REGS_EPI>(); }
 
+  if (warp >= TG_EPI_WARPS) reg_dec<TG_REGS_PRODUCER>(); else reg_inc<TG_REGS_CONSUMER>();
   if (warp == TG_EPI_WARPS) {
     // ================================ TMA producer (whole warp runs the loop, one elected lane issues) ==========
-    // (the single-thread form of the CTA-pair kernel is NOT used here: with it this kernel faulted sporadically in the
-    // timeline-stamp build — different launches each time, clean under compute-sanitizer — so it keeps the round-1 form)
-    int stage = 0, phase = 0;
+    int stage = 0, phase = 0, iter = 0;
     const uint32_t tx_bytes = TG_A_STAGE + static_cast<uint32_t>(p.BN) * (TG_BK * 2);
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
       const TileCoord c = decode_tile(p, tile);
       const int a1 = c.t[0] * p.a_mul[0], a2 = c.t[1] * p.a_mul[1], a3 = c.t[2] * p.a_mul[2],
                 a4 = c.t[3] * p.a_mul[3];
       const int b2 = c.t[1] * p.b_mul[0], b3 = c.t[2] * p.b_mul[1], b4 = c.t[3] * p.b_mul[2];
       const int n0 = c.nt * p.BN;
+      // the ring doubles as the previous tile's accumulator staging tile until its epilogue has read it
+      if (iter > 0) mbar_wait(epi_done, (iter - 1) & 1, p.err, 2);
       auto load_step = [&](int t, int kc) {
         const CUtensorMap* ta = p.tap_src[t] ? &tmA2 : &tmA;
         const CUtensorMap* tb = p.tap_src[t] ? &tmB2 : &tmB;
@@ -731,69 +716,90 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if (tile == static_cast<int>(blockIdx.x) && lane == 0) tg_stamp(p, 2);   // first tile's loads all issued
     }
     if (lane == 0) tg_stamp(p, 3);
-  } else if (warp == TG_EPI_WARPS + 1) {
-    // ================================ MMA issuer (warp-uniform loop, elected lane issues) ================================
-    int stage = 0, phase = 0, iter = 0;
+  } else if (warp < TG_EPI_WARPS) {
+    // ============================ consumers: wgmma mainloop + epilogue (warps 0..7) ============================
+    const int wg = warp >> 2;                    // warpgroup: tile rows [64 wg, 64 wg + 64) in the mainloop
+    const int row = (warp & 3) * 32 + lane;      // epilogue: this thread's accumulator row
+    int rr = row;
+    const int j1 = rr % p.box[0]; rr /= p.box[0];
+    const int j2 = rr % p.box[1]; rr /= p.box[1];
+    const int j3 = rr % p.box[2];
+    const int j4 = rr / p.box[2];
+    const bool n64 = (p.BN & 63) == 0;           // N = 64 MMA blocks; otherwise N = 16 blocks (BN is a multiple of 16)
+    const int nblk = n64 ? (p.BN >> 6) : (p.BN >> 4);
+    const int spitch = p.BN + 4;                 // staging row pitch in floats
+    const uint32_t arow = base + static_cast<uint32_t>(row * spitch * 4);
+    float accum[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) accum[i] = 0.f;
+    int stage = 0, phase = 0, iter = 0, box_sel = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-      const int acc = iter & 1, aphase = (iter >> 1) & 1;
-      mbar_wait(tempty_bar(acc), aphase ^ 1, p.err, 2);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * TG_ACC_COLS;
       int tsteps = steps;
       if (nsplit > 1) {                                                         // this tile's share of the K loop
         const int split = tile / (total_tiles / nsplit);
         const int kc0 = split * p.kc_per, kc1 = min(p.kchunks, kc0 + p.kc_per);
         tsteps = (kc1 - kc0) * p.nprim + (split == 0 ? sec_steps : 0);
       }
+      int prev = -1;
       for (int s = 0; s < tsteps; ++s) {
         mbar_wait(full_bar(stage), phase, p.err, 3);
-        tc_fence_after();
-        if (iter == 0 && s == 0 && lane == 0) tg_stamp(p, 4);                   // first operands landed
-        if (elect_one()) {
-          const uint64_t adesc = umma_desc_sw128(sA + stage * TG_A_STAGE);
-          const uint64_t bdesc = umma_desc_sw128(sB + stage * BST);
+        if (iter == 0 && s == 0 && threadIdx.x == 0) tg_stamp(p, 4);             // first operands landed
+        wgmma_fence();
+        const uint32_t a0 = sA + stage * TG_A_STAGE + wg * (64 * 128), b0 = sB + stage * BST;
 #pragma unroll
-          for (int k = 0; k < TG_BK / 16; ++k)
-            tc_mma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, p.idesc, (s > 0 || k > 0) ? 1u : 0u);
-          tc_commit(empty_bar(stage));               // frees the smem slot when these MMAs retire
-          if (s == tsteps - 1) tc_commit(tfull_bar(acc));  // accumulator complete -> epilogue
+        for (int k = 0; k < TG_BK / 16; ++k) {
+          const uint64_t adesc = wgmma_desc_sw128(a0) + 2 * k;
+          const uint32_t on = (s > 0 || k > 0) ? 1u : 0u;
+          if (n64) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+              if (j < nblk) wgmma_ss<64, T>(&accum[32 * j], adesc, wgmma_desc_sw128(b0 + j * (64 * 128)) + 2 * k, on);
+          } else {
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+              if (j < nblk) wgmma_ss<16, T>(&accum[8 * j], adesc, wgmma_desc_sw128(b0 + j * (16 * 128)) + 2 * k, on);
+          }
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();                                   // the previous step's MMAs have read their stage
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+        prev = stage;
         if (++stage == NS) { stage = 0; phase ^= 1; }
       }
-      if (iter == 0 && lane == 0) tg_stamp(p, 5);                               // first tile fully issued
-    }
-    if (lane == 0) tg_stamp(p, 6);
-  } else if (warp < TG_EPI_WARPS) {
-    // ================================ epilogue (warps 0..7) ================================
-    const int row = (warp & 3) * 32 + lane;
-    int rr = row;
-    const int j1 = rr % p.box[0]; rr /= p.box[0];
-    const int j2 = rr % p.box[1]; rr /= p.box[1];
-    const int j3 = rr % p.box[2];
-    const int j4 = rr / p.box[2];
-    int iter = 0, box_sel = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-      const int acc = iter & 1, aphase = (iter >> 1) & 1;
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(empty_bar(prev));
+      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 5);                        // first tile's MMAs complete
+
+      // accumulators -> fp32 staging tile (the producer is parked on epi_done, so no load writes the ring meanwhile); the
+      // barrier first: the other warpgroup's last MMAs may still be reading the ring stages the staging tile overlays
+      asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
+      {
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+        for (int g = 0; g < 32; ++g) {
+          if (8 * g < p.BN) {
+            const uint32_t a = base + static_cast<uint32_t>((r0 * spitch + 8 * g + c0) * 4);
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(accum[4 * g]), "f"(accum[4 * g + 1]) : "memory");
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a + 8 * spitch * 4), "f"(accum[4 * g + 2]),
+                         "f"(accum[4 * g + 3]) : "memory");
+          }
+        }
+      }
+      asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
       const TileCoord c = decode_tile(p, tile);
-      epilogue_tile<T, LEAN>(p, &tmO, c, fast_div(tile, p.n_tiles, p.magic[0]), row, warp, j1, j2, j3, j4, acc, aphase, tmem_base, s_bias, ostg, ostg2,
-                       box_sel, tfull_bar(acc), p.n_tiles > 1 || iter < 2, iter == 0 && threadIdx.x == 0);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
+      epilogue_tile<T, LEAN>(p, &tmO, c, fast_div(tile, p.n_tiles, p.magic[0]), row, warp, j1, j2, j3, j4, iter & 1, arow,
+                             s_bias, ostg, ostg2, box_sel, p.n_tiles > 1 || iter < 2, iter == 0 && threadIdx.x == 0);
+      // staging tile consumed: the ring goes back to the producer (generic reads ordered before the TMA's async writes)
+      fence_async_smem();
+      asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
+      if (threadIdx.x == 0) mbar_arrive(epi_done);
       if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 9);                        // first tile stored
     }
     if (p.tma_out && lane == 0) bulk_wait_all();      // the store boxes live in this CTA's shared memory
     if (threadIdx.x == 0) tg_stamp(p, 10);
   }
-
-  tc_fence_before();
   __syncthreads();
   if (threadIdx.x == 0) tg_stamp(p, 11);
-  if (warp == TG_EPI_WARPS + 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-    if (lane == 0) tg_stamp(p, 12);
-  }
 }
 
 }  // namespace i2it

@@ -1,4 +1,4 @@
-"""Drop-in mirror of /root/reference/src/cyclegan_turbo.py (CycleGAN_Turbo, VAE_encode, VAE_decode) over libi2it.
+"""Drop-in mirror of src/cyclegan_turbo.py (CycleGAN_Turbo, VAE_encode, VAE_decode) over libi2it.
 
 Same constructor kwargs / attributes / forward signatures, so src/inference_unpaired.py runs unchanged
 (`model.eval()`, `model.unet.enable_xformers_memory_efficient_attention()`, `model.half()`,

@@ -1,8 +1,8 @@
 """ctypes binding of libi2it.so (the C ABI declared in include/i2it.h).
 
 PyTorch is plumbing here: it owns device memory and streams; every FLOP of the image path runs inside
-libi2it's sm_100a kernels.  There is NO fallback: if the library is missing or the device is not a
-B200, construction raises.
+libi2it's sm_90a kernels.  There is NO fallback: if the library is missing or the device is not an
+H100, construction raises.
 """
 from __future__ import annotations
 
@@ -106,7 +106,7 @@ class Engine:
                  device: Optional[int] = None, keep_stages: bool = False, use_cuda_graph: bool = True,
                  text_heads: int = 0, text_act: str = "gelu"):
         if not torch.cuda.is_available():
-            raise RuntimeError("libi2it needs a CUDA device (B200 / sm_100a); no CPU fallback exists")
+            raise RuntimeError("libi2it needs a CUDA device (H100 / sm_90a); no CPU fallback exists")
         self.lib = load_library()
         self.dtype = dtype
         c = Config()

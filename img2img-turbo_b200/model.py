@@ -1,4 +1,4 @@
-"""Mirror of /root/reference/src/model.py's importable names.
+"""Mirror of src/model.py's importable names.
 
 * make_1step_sched        -> closed-form one-step DDPM (model.py:7-11); the engine fuses the step on device.
 * my_vae_encoder_fwd / my_vae_decoder_fwd (model.py:14-54) have no Python body here: the patched VAE forwards

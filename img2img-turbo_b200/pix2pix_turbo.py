@@ -1,4 +1,4 @@
-"""Drop-in mirror of /root/reference/src/pix2pix_turbo.py (Pix2Pix_Turbo, TwinConv) over libi2it.
+"""Drop-in mirror of src/pix2pix_turbo.py (Pix2Pix_Turbo, TwinConv) over libi2it.
 
 Same constructor kwargs, attributes and .forward() signature as the reference, so
 src/inference_paired.py and the gradio apps call it unchanged (put this directory first on sys.path;

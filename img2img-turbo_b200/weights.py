@@ -1,8 +1,8 @@
 """Weight inventory + seeded random initialisation in diffusers/peft key naming.
 
 The reference builds its networks with ``from_pretrained("stabilityai/sd-turbo")`` and then installs
-LoRA adapters / skip convs (/root/reference/src/pix2pix_turbo.py:32-45,131-155;
-/root/reference/src/cyclegan_turbo.py:48-106).  Offline there are no SD-Turbo weights, so the
+LoRA adapters / skip convs (src/pix2pix_turbo.py:32-45,131-155;
+src/cyclegan_turbo.py:48-106).  Offline there are no SD-Turbo weights, so the
 ``pretrained_name=None, pretrained_path=None`` branch (pix2pix_turbo.py:131) is the one every
 BASELINE config uses: PyTorch default layer init for the base model, LoRA "gaussian" init for
 lora_A, skip convs = 1e-5.  ``lora_B`` is drawn N(0, 0.02^2) instead of the default zeros so the

@@ -1,11 +1,11 @@
-/* libi2it — C ABI of the B200-native one-step image-translation path
+/* libi2it — C ABI of the H100-native one-step image-translation path
  *
  *     VAE.encode -> one SD-Turbo UNet step (t = 999) -> DDPM closed form -> VAE.decode
  *
  * This is the boundary the reference's Python wrappers would bind (via ctypes; see INTEGRATION.md) in
  * place of the four diffusers calls at
- *     /root/reference/src/pix2pix_turbo.py:198-203   (deterministic)   and :204-218 (stochastic)
- *     /root/reference/src/cyclegan_turbo.py:199-207  (forward_with_networks)
+ *     src/pix2pix_turbo.py:198-203   (deterministic)   and :204-218 (stochastic)
+ *     src/cyclegan_turbo.py:199-207  (forward_with_networks)
  * i.e.  vae.encode(x).latent_dist.sample()*sf ; unet(z, 999, text).sample ; sched.step(...).prev_sample ;
  *       vae.decode(x0/sf).sample.clamp(-1,1)
  *
@@ -60,7 +60,7 @@ typedef struct i2it_config {
 int i2it_default_config(i2it_config* cfg);
 
 /* Create / destroy an engine.  Replaces AutoencoderKL/UNet2DConditionModel construction
- * (/root/reference/src/pix2pix_turbo.py:36-45; cyclegan_turbo.py:115-124). */
+ * (src/pix2pix_turbo.py:36-45; cyclegan_turbo.py:115-124). */
 int i2it_create(const i2it_config* cfg, i2it_handle** out);
 void i2it_destroy(i2it_handle* h);
 const char* i2it_last_error(const i2it_handle* h);   /* h may be NULL: last error of a failed create */
@@ -69,19 +69,19 @@ const char* i2it_last_error(const i2it_handle* h);   /* h may be NULL: last erro
  * {unet, vae, vae_b2a}; peft spellings ("X.base_layer.weight", "X.lora_A.<adapter>.weight",
  * "X.lora_B.<adapter>.weight") are accepted as-is.  `data` may be a host or device pointer
  * (is_device); dtype is I2IT_F32/F16/BF16.  The engine keeps an fp32 device copy (synchronous).
- * Replaces load_state_dict at /root/reference/src/pix2pix_turbo.py:66-78, cyclegan_turbo.py:162-190. */
+ * Replaces load_state_dict at src/pix2pix_turbo.py:66-78, cyclegan_turbo.py:162-190. */
 int i2it_set_weight(i2it_handle* h, const char* key, const void* data, const int64_t* shape, int ndim,
                     int dtype, int is_device);
 
 /* LoRA scale (lora_alpha / r) of an adapter name ("default", "vae_skip", "default_encoder", ...);
- * replaces peft LoraConfig scaling (/root/reference/src/pix2pix_turbo.py:141-151, cyclegan_turbo.py:66-72). */
+ * replaces peft LoraConfig scaling (src/pix2pix_turbo.py:141-151, cyclegan_turbo.py:66-72). */
 int i2it_set_adapter_scale(i2it_handle* h, const char* adapter, float alpha_over_r);
 
 /* Fold LoRA into the base weights (W' = W + s*w*B@A in fp32, one rounding), blend TwinConv
  * (W = (1-r) W_pre + r W_cur), scale the skip convs by gamma, fold the t=999 time embedding into
  * conv1 biases, re-lay out for the kernels.  Callable again when the runtime weights change
  * (stochastic mode: unet.set_adapters(["default"],[r]), set_weights_and_activate_adapters(vae,...,[r]),
- * decoder.gamma = r, conv_in.r = r  — /root/reference/src/pix2pix_turbo.py:206-217).
+ * decoder.gamma = r, conv_in.r = r  — src/pix2pix_turbo.py:206-217).
  * lora_weight_* multiply the adapter scales of the UNet / VAE adapters; twin_r < 0 means "no TwinConv blend
  * requested" (error if the state dict has a TwinConv). */
 int i2it_finalize_weights(i2it_handle* h, float lora_weight_unet, float lora_weight_vae, float skip_gamma,
@@ -112,11 +112,11 @@ int i2it_forward(i2it_handle* h, const void* x, const void* text_emb, int text_b
  * transformer block (32 small launches, enqueued on `stream`).  text_emb [text_batch, 77, cross] device pointer in the
  * handle dtype; it is consumed before the call returns control to the stream order (the caller may reuse the buffer after
  * the stream reaches this point).  Must be called again after i2it_finalize_weights (the projections carry the LoRA scale).
- * Replaces the per-forward `attn2.to_k / attn2.to_v` calls under unet(...) at /root/reference/src/pix2pix_turbo.py:199. */
+ * Replaces the per-forward `attn2.to_k / attn2.to_v` calls under unet(...) at src/pix2pix_turbo.py:199. */
 int i2it_set_text(i2it_handle* h, const void* text_emb, int text_batch, void* stream);
 
 /* The CLIP text tower on the engine (SURVEY.md section 8f #1): tokens [batch, 77] int32 (device) -> last_hidden_state
- * [batch, 77, hidden] (device, handle dtype), i.e. `self.text_encoder(tokens)[0]` of /root/reference/src/pix2pix_turbo.py:190-196
+ * [batch, 77, hidden] (device, handle dtype), i.e. `self.text_encoder(tokens)[0]` of src/pix2pix_turbo.py:190-196
  * and cyclegan_turbo.py:251-253.  Needs the "text_encoder.<transformers CLIPTextModel key>" tensors registered with
  * i2it_set_weight.  Enqueued on `stream` (no CUDA graph: a prompt is encoded once and cached by the caller). */
 int i2it_encode_text(i2it_handle* h, const int32_t* tokens, int batch, void* out, void* stream);

@@ -6,13 +6,13 @@ repository accelerates:
     VAE.encode -> one SD-Turbo UNet step (t=999) -> DDPM closed-form x0 -> VAE.decode
 
 as executed by the reference wrappers
-    /root/reference/src/pix2pix_turbo.py:186-219   (Pix2Pix_Turbo.forward)
-    /root/reference/src/cyclegan_turbo.py:199-207  (CycleGAN_Turbo.forward_with_networks)
-    /root/reference/src/model.py:14-54             (patched VAE encoder/decoder forwards)
+    src/pix2pix_turbo.py:186-219   (Pix2Pix_Turbo.forward)
+    src/cyclegan_turbo.py:199-207  (CycleGAN_Turbo.forward_with_networks)
+    src/model.py:14-54             (patched VAE encoder/decoder forwards)
 
 PARITY UNPINNED: the arithmetic lives in diffusers==0.25.1 / peft, which are pinned in
-/root/reference/environment.yaml:31-33 but are NOT vendored in /root/reference and are not
-installed in this image; the reference ships no tests or golden vectors for the path.
+environment.yaml:31-33 but are NOT vendored in the reference repository and are not
+installed here; the reference ships no tests or golden vectors for the path.
 This file therefore restates the *published* diffusers 0.25.1 algorithm (AutoencoderKL,
 UNet2DConditionModel, DDPMScheduler, peft LoRA) and is pinned by:
   * exact parameter-count checksums (UNet 865,910,724; VAE 83,653,863; skip convs 491,520),

@@ -14,7 +14,7 @@ torch.set_num_threads(min(32, os.cpu_count() or 1))     # many-core GPU hosts ru
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a GPU host)")
 
 
 @pytest.fixture(scope="session")

@@ -161,7 +161,7 @@ CASES = {
     "attn_cross": lambda: case_attn(hf, 2, 256, 77, 5, 64, kvb=1),
     "attn_4096": lambda: case_attn(bf, 1, 4096, 4096, 2, 64),
     "attn_vae": lambda: case_attn(bf, 1, 1024, 1024, 1, 512),
-    # big enough (>= 2 x 148 tiles) to take the CTA-pair (cta_group::2) kernel
+    # many waves of tiles per persistent CTA (ring / staging-tile reuse across tiles), residual and ragged variants
     "pair_conv": lambda: case_conv(bf, 4, 128, 128, 128, 128, res=True),
     "pair_conv256": lambda: case_conv(hf, 2, 128, 128, 256, 256),
     "halo_ragged": lambda: case_conv(bf, 16, 40, 40, 64, 512, res=True),

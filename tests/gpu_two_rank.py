@@ -1,7 +1,6 @@
 """torchrun target (2 ranks, NCCL): the N-rank sharded forward (dist.sharded_forward: contiguous batch split + ONE all-gather of
 the images) equals the single-rank forward of the whole batch bit for bit, through the public Pix2Pix_Turbo API.
-Launched by tests/test_gpu_boundary.py::test_two_rank_sharded_output_equals_single_rank and by the builder under
-`gpurun --gpus 2` (log in profiles/)."""
+Launched by tests/test_gpu_boundary.py::test_two_rank_sharded_output_equals_single_rank."""
 import os
 import sys
 

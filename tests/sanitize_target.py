@@ -1,5 +1,5 @@
-"""compute-sanitizer target: one tiny forward of the hot path through the C ABI, eager launches (no CUDA graph), both GEMM kernels
-(1-CTA and CTA-pair), flash attention, GroupNorm / LayerNorm, the uint8 boundary and the prompt K/V cache.
+"""compute-sanitizer target: one tiny forward of the hot path through the C ABI, eager launches (no CUDA graph), the GEMM kernel,
+flash attention, GroupNorm / LayerNorm, the uint8 boundary and the prompt K/V cache.
     compute-sanitizer --tool memcheck  python tests/sanitize_target.py
     compute-sanitizer --tool racecheck python tests/sanitize_target.py"""
 import os

@@ -17,17 +17,24 @@ def _run(args, env=None, timeout=600):
 
 
 def test_reference_arm_prints_contract_line():
-    r = _run(["--impl", "reference", "--size", "64", "--steps", "1", "--warmup", "1"])
+    r = _run(["--impl", "reference", "--size", "64", "--steps", "4", "--warmup", "0"])
     assert r.returncode == 0, r.stderr[-2000:]
     lines = [l for l in r.stdout.splitlines() if l.startswith("{")]
     assert len(lines) == 1
     d = json.loads(lines[0])
     assert d["impl"] == "reference" and d["metric"] == "512x512 images/sec" and d["unit"] == "images/s"
     assert d["value"] > 0 and d["ms_per_step"] > 0 and d["higher_is_better"] is True and d["n_gpus"] == 1
+    assert d["steps"] == 4 and d["warmup"] == 0                       # --steps / --warmup are timed as given, never clamped
     assert d["e2e"] == {"value": d["value"], "unit": "images/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
     cb = d["cpu_baseline"]
     assert cb["kind"] == "port" and cb["cores"] >= 1 and cb["value"] == d["value"] and "sample" in cb
     assert "workload" in d["config"] and "model" not in d["config"]
+
+
+def test_steps_that_cannot_be_honoured_are_rejected():
+    for args in (["--steps", "0"], ["--warmup", "-1"]):
+        r = _run(["--impl", "reference", "--size", "64"] + args)
+        assert r.returncode != 0 and "{" not in r.stdout and "--steps must be" in r.stderr
 
 
 def test_reference_arm_other_ranks_are_silent():

@@ -192,8 +192,7 @@ def test_public_api_u8_and_checkpoint_through_engine(tmp_path):
 
 
 def test_two_rank_sharded_output_equals_single_rank(tmp_path):
-    """N-rank sharded forward == 1-rank forward, bit for bit (needs 2 GPUs; the driver's 1-GPU test box skips it — the builder's
-    2-GPU run is logged under profiles/)."""
+    """N-rank sharded forward == 1-rank forward, bit for bit (needs 2 GPUs; skipped on a single-GPU host)."""
     import subprocess
     import sys
     if torch.cuda.device_count() < 2:

@@ -1,6 +1,6 @@
 """-m gpu: the CLIP text tower on the engine (SURVEY.md section 8f #1) against transformers' CLIPTextModel — the one row whose
 oracle IS the reference's own dependency (transformers is importable here), so this parity is pinned: same random-init tensors,
-fp32 reference, engine in fp16 / bf16.  `text_encoder(tokens)[0]` is what /root/reference/src/pix2pix_turbo.py:190-196 feeds the
+fp32 reference, engine in fp16 / bf16.  `text_encoder(tokens)[0]` is what src/pix2pix_turbo.py:190-196 feeds the
 UNet."""
 import pytest
 import torch

@@ -8,7 +8,7 @@ Each test runs the ENGINE at the config's batch size, then checks selected image
 CPU oracle run at batch 1 on the same weights / inputs / eps (image i of a batch == its batch-1 forward bit for bit is tested in
 test_gpu_e2e.py, so two images pin the batch).  Per stage it asserts finiteness and an error bound relative to the stage's scale,
 and PRINTS the north-star band — the fraction of elements with |got - ref| <= 1e-4 + 1e-3*|ref| (rtol 1e-3 / atol 1e-4) — so that
-the tolerance gap of a 16-bit pipeline is a number, not an argument (also written to gpurun_out/parity_bands.json)."""
+the tolerance gap of a 16-bit pipeline is a number, not an argument (also written to $I2IT_PARITY_DIR/parity_bands.json when that directory exists)."""
 import json
 import os
 
@@ -42,8 +42,8 @@ def stage_report(tag, name, got, ref, rel_bound):
 
 
 def _flush_bands():
-    d = os.path.join(ROOT, "gpurun_out")
-    if os.path.isdir(d):
+    d = os.environ.get("I2IT_PARITY_DIR")
+    if d and os.path.isdir(d):
         json.dump(BANDS, open(os.path.join(d, "parity_bands.json"), "w"), indent=1)
 
 
@@ -71,7 +71,6 @@ def _stages(e, pick):
 
 # bounds: relative mean error per stage vs the fp32 oracle (16-bit storage of every activation; the DDPM step multiplies the
 # UNet error by 14.6 and /0.18215 by another 5.5 before the decoder — SURVEY fact 6)
-# measured on B200 (profiles/r02b_parity_bands.json): fp16 0.02 / 0.14 / 0.06-0.09 / 0.2 / 0.2 / 0.15-0.28 %, bf16 x 6-8; bounds = ~3x that
 BOUNDS_FP16 = {"skip0": 1e-3, "skip3": 5e-3, "latent": 3e-3, "model_pred": 7e-3, "x_denoised": 7e-3, "pre_clamp": 1e-2}
 BOUNDS_BF16 = {"skip0": 8e-3, "skip3": 4e-2, "latent": 2e-2, "model_pred": 5e-2, "x_denoised": 5e-2, "pre_clamp": 7e-2}
 

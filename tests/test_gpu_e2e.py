@@ -239,8 +239,7 @@ def test_runtime_switches_agree(monkeypatch):
     assert torch.equal(base, run(I2IT_NO_LEAN="1"))            # the compile-time-stripped epilogue computes the same bits
     assert torch.equal(base, run(I2IT_NO_OSTG2="1"))           # one or two store boxes: data movement only
     assert torch.equal(run(I2IT_NO_GNEPI="1"), run(I2IT_NO_GNEPI="1", I2IT_NO_TMAOUT="1"))
-    for env in ({"I2IT_NO_GNEPI": "1"}, {"I2IT_NO_SPLITK": "1"}, {"I2IT_FLASH_V1": "1"}, {"I2IT_IDRES": "1"},
-                {"I2IT_NO_HALO": "1"}, {"I2IT_NO_PAIR": "1"}):
+    for env in ({"I2IT_NO_GNEPI": "1"}, {"I2IT_NO_SPLITK": "1"}, {"I2IT_IDRES": "1"}):
         y = run(**env)
         d = (y.float() - base.float()).abs()
         # different summation orders of the fp32 statistics / K ranges flip last bits of bf16 activations (1 ulp at 1.0 = 7.8e-3),

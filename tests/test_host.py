@@ -336,7 +336,7 @@ def test_tile_decode_magic_division_is_exact():
         for x in xs:
             if 0 <= x < maxd:
                 assert lib.i2it_debug_fast_div(maxd, d, x) == (-1 if refused else x // d), (maxd, d, x)
-    # exhaustive for one real launch: 16384 m-tiles, pair kernel dividends up to 2 * m_tiles + 2 + grid
+    # exhaustive over a bound above any real launch's dividends (16384 m-tiles: tile index + grid)
     maxd = 2 * 16384 + 2 + 148
     for d in (2, 32, 128):
         assert all(lib.i2it_debug_fast_div(maxd, d, x) == x // d for x in range(maxd))
