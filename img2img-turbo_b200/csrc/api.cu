@@ -5,6 +5,7 @@ using namespace i2it;
 
 struct i2it_handle {
   Engine* eng = nullptr;
+  std::vector<OpMeta> op_meta;     // launch list of the last diagnostic op call (i2it_op_launches)
 };
 static thread_local std::string g_create_error;
 
@@ -181,7 +182,9 @@ int i2it_read_stage(i2it_handle* h, const char* name, float* dst, size_t dst_ele
 // ------------------------------------------------------------------------------------------------
 // diagnostic single-op entry points
 // ------------------------------------------------------------------------------------------------
-static void run_plan(Engine& E, Plan& P, cudaStream_t st) {
+static void run_plan(i2it_handle* h, Plan& P, cudaStream_t st) {
+  Engine& E = *h->eng;
+  h->op_meta = P.meta;
   E.flush_prep();
   I2IT_CUDA(cudaDeviceSynchronize());
   for (auto& op : P.ops) op(st);
@@ -198,28 +201,84 @@ static Act view(const void* p, int N, int H, int W, int C, int ld) {
   return a;
 }
 
-int i2it_op_conv2d(i2it_handle* h, const void* x, int N, int H, int W, int Cin, int ldx, const float* w,
-                   const float* bias, int Cout, int ksize, int stride, int asym_pad, const void* residual, int ldr,
-                   int act, void* out, int ldo, int out_fp32, void* stream) {
+int i2it_op_conv2d_ex(i2it_handle* h, const i2it_conv_desc* d, void* stream) {
   API_BEGIN(h)
-  const int64_t wshape[4] = {Cout, Cin, ksize, ksize};
-  E.set_weight("__op.conv.weight", w, wshape, 4, I2IT_F32, true);
-  if (bias) { const int64_t bshape[1] = {Cout}; E.set_weight("__op.conv.bias", bias, bshape, 1, I2IT_F32, true); }
+  I2IT_CHECK(d && d->x && d->w && d->out, "i2it_op_conv2d_ex: null operand");
+  const int stride = d->stride > 0 ? d->stride : 1, k = d->ksize, oc = (d->act == TG_ACT_GEGLU) ? d->Cout / 2 : d->Cout;
+  I2IT_CHECK(!d->asym_pad || ((d->H | d->W) & 1) == 0, "i2it_op_conv2d_ex: asymmetric padding needs an even map");
+  I2IT_CHECK(!d->up2x || (k == 3 && stride == 1 && d->bias && !d->residual && !d->out_fp32 && d->act == TG_ACT_NONE),
+             "i2it_op_conv2d_ex: up2x is a biased 3x3 stride-1 conv without residual, activation or fp32 output");
+  I2IT_CHECK(!d->tokens || (k == 1 && !d->up2x), "i2it_op_conv2d_ex: token rows need a 1x1 conv");
+  I2IT_CHECK(!d->gn_y || (d->gn_gamma && d->gn_beta && !d->out_fp32), "i2it_op_conv2d_ex: GroupNorm needs gamma, beta, 16-bit out");
+  const int64_t wshape[4] = {d->Cout, d->Cin, k, k};
+  E.set_weight("__op.conv.weight", d->w, wshape, 4, I2IT_F32, true);
+  if (d->bias) { const int64_t bshape[1] = {d->Cout}; E.set_weight("__op.conv.bias", d->bias, bshape, 1, I2IT_F32, true); }
+  if (d->x2) {
+    I2IT_CHECK(d->w2 != nullptr, "i2it_op_conv2d_ex: x2 without w2");
+    const int64_t w2shape[4] = {d->Cout, d->C2, 1, 1};
+    E.set_weight("__op.conv2.weight", d->w2, w2shape, 4, I2IT_F32, true);
+  }
   E.finalize(1.f, 1.f, 1.f, -1.f);
   {
     Plan P;
-    PW pw = E.prep("__op.conv", {"__op.conv"}, act == TG_ACT_GEGLU);
-    ConvOpts o;
-    o.ksize = ksize; o.stride = stride; o.asym = asym_pad != 0; o.act = act; o.out_fp32 = out_fp32 != 0;
-    const int Ho = H / stride, Wo = W / stride;
-    Act xin = view(x, N, H, W, Cin, ldx);
-    Act res = view(residual, N, Ho, Wo, Cout, ldr);
-    if (residual) o.res = &res;
-    Act ov = view(out, N, Ho, Wo, (act == TG_ACT_GEGLU) ? Cout / 2 : Cout, ldo);
-    o.out = &ov;
-    E.conv(P, xin, pw, o);
-    run_plan(E, P, static_cast<cudaStream_t>(stream));
+    // Ho = ceil(H / stride): Engine::conv pads an odd map to even before a stride-2 conv
+    const int Ho = d->up2x ? 2 * d->H : (d->H + stride - 1) / stride, Wo = d->up2x ? 2 * d->W : (d->W + stride - 1) / stride;
+    Act xin = view(d->x, d->N, d->H, d->W, d->Cin, d->ldx);
+    Act res = view(d->residual, d->N, Ho, Wo, oc, d->ldr);
+    Act ov = view(d->out, d->N, Ho, Wo, oc, d->ldo);
+    Act x2 = view(d->x2, d->N, Ho, Wo, d->C2, d->ld2);
+    PW pw2;
+    if (d->x2) pw2 = E.prep("__op.conv2", {"__op.conv2"});
+    Act y;
+    if (d->up2x) {
+      const PW pw = E.prep_subpixel("__op.conv");
+      y = E.conv_up2x(P, xin, pw, d->x2 ? &x2 : nullptr, d->x2 ? &pw2 : nullptr, d->gn_y != nullptr);
+      E.copy_channels(P, y, ov);
+    } else {
+      const PW pw = E.prep("__op.conv", {"__op.conv"}, d->act == TG_ACT_GEGLU);
+      ConvOpts o;
+      o.ksize = k; o.stride = stride; o.asym = d->asym_pad != 0; o.act = d->act; o.out_fp32 = d->out_fp32 != 0;
+      o.gn_out = d->gn_y != nullptr;
+      if (d->tokens) {
+        o.gn_rows_per_image = 1ll * d->H * d->W;
+        xin = xin.as_rows(); res = res.as_rows(); ov = ov.as_rows(); x2 = x2.as_rows();
+      }
+      if (d->residual) o.res = &res;
+      if (d->x2) { o.x2 = &x2; o.w2 = &pw2; }
+      o.out = &ov;
+      y = E.conv(P, xin, pw, o);
+      y.N = d->N; y.H = Ho; y.W = Wo;
+    }
+    if (d->gn_y) {
+      NormW nw; nw.g = d->gn_gamma; nw.b = d->gn_beta; nw.C = oc;
+      const Act g = E.group_norm(P, y, nw, d->gn_eps, d->gn_silu != 0);
+      E.copy_channels(P, g, view(d->gn_y, d->N, Ho, Wo, oc, d->ldg));
+    }
+    run_plan(h, P, static_cast<cudaStream_t>(stream));
   }
+  API_END
+}
+
+int i2it_op_conv2d(i2it_handle* h, const void* x, int N, int H, int W, int Cin, int ldx, const float* w,
+                   const float* bias, int Cout, int ksize, int stride, int asym_pad, const void* residual, int ldr,
+                   int act, void* out, int ldo, int out_fp32, void* stream) {
+  i2it_conv_desc d;
+  std::memset(&d, 0, sizeof d);
+  d.x = x; d.N = N; d.H = H; d.W = W; d.Cin = Cin; d.ldx = ldx; d.w = w; d.bias = bias; d.Cout = Cout; d.ksize = ksize;
+  d.stride = stride; d.asym_pad = asym_pad; d.residual = residual; d.ldr = ldr; d.act = act; d.out = out; d.ldo = ldo;
+  d.out_fp32 = out_fp32;
+  return i2it_op_conv2d_ex(h, &d, stream);
+}
+
+int i2it_op_launches(i2it_handle* h, char* json, size_t cap) {
+  API_BEGIN(h)
+  I2IT_CHECK(json != nullptr && cap > 2, "i2it_op_launches: bad arguments");
+  std::string js = "[";
+  for (size_t i = 0; i < h->op_meta.size(); ++i)
+    js += std::string(i ? "," : "") + "{\"kind\":\"" + h->op_meta[i].kind + "\",\"shape\":\"" + h->op_meta[i].shape + "\"}";
+  js += "]";
+  I2IT_CHECK(js.size() + 1 <= cap, "i2it_op_launches: buffer too small");
+  std::memcpy(json, js.c_str(), js.size() + 1);
   API_END
 }
 
@@ -231,7 +290,7 @@ int i2it_op_group_norm(i2it_handle* h, const void* x, int N, int HW, int C, int 
     NormW nw; nw.g = gamma; nw.b = beta; nw.C = C;
     Act y = E.group_norm(P, view(x, N, 1, HW, C, ldx), nw, eps, silu != 0);
     E.copy_channels(P, y, view(out, N, 1, HW, C, ldo));
-    run_plan(E, P, static_cast<cudaStream_t>(stream));
+    run_plan(h, P, static_cast<cudaStream_t>(stream));
   }
   API_END
 }
@@ -245,21 +304,40 @@ int i2it_op_layer_norm(i2it_handle* h, const void* x, int rows, int C, int ldx, 
     NormW nw; nw.g = gamma; nw.b = beta; nw.C = C;
     Act y = E.layer_norm(P, view(x, 1, 1, rows, C, ldx), nw);
     E.copy_channels(P, y, view(out, 1, 1, rows, C, ldo));
-    run_plan(E, P, static_cast<cudaStream_t>(stream));
+    run_plan(h, P, static_cast<cudaStream_t>(stream));
   }
   API_END
 }
 
 int i2it_op_attention(i2it_handle* h, const void* q, int ldq, const void* k, int ldk, const void* vt, int ldv, int B,
-                      int Nq, int Nk, int heads, int d, int kv_batch, void* out, int ldo, void* stream) {
+                      int Nq, int Nk, int heads, int d, int kv_batch, int causal, void* out, int ldo, void* stream) {
   API_BEGIN(h)
+  I2IT_CHECK(!causal || (d == FA_D && E.use_flash), "i2it_op_attention: causal attention runs on the flash path (d = 64)");
   {
     Plan P;
     const int C = heads * d;
-    Act o = E.attention(P, view(q, B, 1, Nq, C, ldq), view(k, kv_batch, 1, Nk, C, ldk), view(vt, kv_batch, 1, C, ldv, ldv), B,
-                        Nq, Nk, heads, d, kv_batch);
+    const Act qa = view(q, B, 1, Nq, C, ldq), ka = view(k, kv_batch, 1, Nk, C, ldk), va = view(vt, kv_batch, 1, C, ldv, ldv);
+    Act o = causal ? E.flash_attention(P, qa, ka, va, B, Nq, Nk, heads, kv_batch, true)
+                   : E.attention(P, qa, ka, va, B, Nq, Nk, heads, d, kv_batch);
     E.copy_channels(P, o, view(out, B, 1, Nq, C, ldo));
-    run_plan(E, P, static_cast<cudaStream_t>(stream));
+    run_plan(h, P, static_cast<cudaStream_t>(stream));
+  }
+  API_END
+}
+
+int i2it_op_vt_proj(i2it_handle* h, const void* x, int B, int ntok, int Cin, int ldx, const float* w, const float* bias, int Cout,
+                    void* out, void* stream) {
+  API_BEGIN(h)
+  const int64_t wshape[2] = {Cout, Cin};
+  E.set_weight("__op.vt.weight", w, wshape, 2, I2IT_F32, true);
+  if (bias) { const int64_t bshape[1] = {Cout}; E.set_weight("__op.vt.bias", bias, bshape, 1, I2IT_F32, true); }
+  E.finalize(1.f, 1.f, 1.f, -1.f);
+  {
+    Plan P;
+    const PW pw = E.prep("__op.vt", {"__op.vt"});
+    const Act vt = E.vt_proj(P, view(x, 1, 1, B * ntok, Cin, ldx), B, ntok, pw);
+    E.copy_channels(P, vt, view(out, B, 1, Cout, vt.C, vt.C));
+    run_plan(h, P, static_cast<cudaStream_t>(stream));
   }
   API_END
 }
@@ -270,7 +348,18 @@ int i2it_op_upsample2x(i2it_handle* h, const void* x, int N, int H, int W, int C
     Plan P;
     Act y = E.upsample2x(P, view(x, N, H, W, C, C));
     E.copy_channels(P, y, view(out, N, 2 * H, 2 * W, C, C));
-    run_plan(E, P, static_cast<cudaStream_t>(stream));
+    run_plan(h, P, static_cast<cudaStream_t>(stream));
+  }
+  API_END
+}
+
+int i2it_op_upsample_to(i2it_handle* h, const void* x, int N, int H, int W, int C, int Ho, int Wo, void* out, void* stream) {
+  API_BEGIN(h)
+  {
+    Plan P;
+    Act y = E.upsample_to(P, view(x, N, H, W, C, C), Ho, Wo);
+    E.copy_channels(P, y, view(out, N, Ho, Wo, C, C));
+    run_plan(h, P, static_cast<cudaStream_t>(stream));
   }
   API_END
 }

@@ -1159,17 +1159,17 @@ Act Engine::attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B,
       add_op(P, [=](cudaStream_t st) {
         DISPATCH_T(dt, (launch_k(softmax_long_kernel<T>, dim3(static_cast<unsigned>(rows)), dim3(256), 0, st, 0, S, lds, reinterpret_cast<T*>(Pm),
                                                                                           lds, Nk, lds)));
-      }, "softmax", 0, 6.0 * rows * Nk);
+      }, "softmax", 0, 6.0 * rows * Nk, "long");
     } else if (Nk > 1024) {
       add_op(P, [=](cudaStream_t st) {
         DISPATCH_T(dt, (launch_k(softmax_kernel<T, 128>, dim3(static_cast<unsigned>(rows)), dim3(128), 0, st, 0, S, lds, reinterpret_cast<T*>(Pm), lds,
                                                                                           rows, Nk, lds)));
-      }, "softmax", 0, 6.0 * rows * Nk);
+      }, "softmax", 0, 6.0 * rows * Nk, "128");
     } else {
       add_op(P, [=](cudaStream_t st) {
         DISPATCH_T(dt, (launch_k(softmax_kernel<T, 32>, dim3(static_cast<unsigned>((rows + 3) / 4)), dim3(128), 0, st, 0,
                            S, lds, reinterpret_cast<T*>(Pm), lds, rows, Nk, lds)));
-      }, "softmax", 0, 6.0 * rows * Nk);
+      }, "softmax", 0, 6.0 * rows * Nk, "32");
     }
   }
   {  // O = P V   (V given transposed: [kvB][C][ldv])

@@ -18,7 +18,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libi2it.so")
 F16, BF16, F32 = 0, 1, 2
 PIX2PIX, CYCLEGAN = 0, 1
 A2B, B2A = 0, 1
-ACT_NONE, ACT_CLAMP1, ACT_GEGLU = 0, 1, 2
+ACT_NONE, ACT_CLAMP1, ACT_GEGLU, ACT_GELU, ACT_QUICKGELU = 0, 1, 2, 3, 4   # epilogue activations (tapgemm TgAct)
 IN_UNIT, IN_NORMALIZE, IN_SKETCH = 0, 1, 2      # uint8 input transforms of i2it_forward_u8
 
 _TORCH2DT = {torch.float16: F16, torch.bfloat16: BF16, torch.float32: F32}
@@ -29,8 +29,23 @@ SYMBOLS = [
     "i2it_default_config", "i2it_create", "i2it_destroy", "i2it_last_error", "i2it_set_weight",
     "i2it_set_adapter_scale", "i2it_finalize_weights", "i2it_workspace_bytes", "i2it_forward",
     "i2it_set_text", "i2it_encode_text", "i2it_forward_u8", "i2it_prep_launch_count", "i2it_debug_fast_div", "i2it_launch_count", "i2it_profile", "i2it_read_stage", "i2it_op_conv2d", "i2it_op_group_norm", "i2it_op_layer_norm",
-    "i2it_op_attention", "i2it_op_upsample2x",
+    "i2it_op_attention", "i2it_op_upsample2x", "i2it_op_conv2d_ex", "i2it_op_launches", "i2it_op_vt_proj",
+    "i2it_op_upsample_to",
 ]
+
+
+class ConvDesc(C.Structure):
+    """i2it_conv_desc (include/i2it.h)."""
+    _fields_ = [
+        ("x", C.c_void_p), ("N", C.c_int), ("H", C.c_int), ("W", C.c_int), ("Cin", C.c_int), ("ldx", C.c_int),
+        ("w", C.c_void_p), ("bias", C.c_void_p), ("Cout", C.c_int), ("ksize", C.c_int), ("stride", C.c_int),
+        ("asym_pad", C.c_int), ("residual", C.c_void_p), ("ldr", C.c_int), ("act", C.c_int),
+        ("out", C.c_void_p), ("ldo", C.c_int), ("out_fp32", C.c_int),
+        ("x2", C.c_void_p), ("C2", C.c_int), ("ld2", C.c_int), ("w2", C.c_void_p),
+        ("up2x", C.c_int), ("tokens", C.c_int),
+        ("gn_y", C.c_void_p), ("ldg", C.c_int), ("gn_silu", C.c_int), ("gn_eps", C.c_float), ("gn_gamma", C.c_void_p),
+        ("gn_beta", C.c_void_p),
+    ]
 
 
 class Config(C.Structure):
@@ -81,8 +96,12 @@ def load_library(path: Optional[str] = None):
     lib.i2it_op_conv2d.argtypes = [vp, vp, ci, ci, ci, ci, ci, vp, vp, ci, ci, ci, ci, vp, ci, ci, vp, ci, ci, vp]
     lib.i2it_op_group_norm.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, cf, ci, vp, ci, vp]
     lib.i2it_op_layer_norm.argtypes = [vp, vp, ci, ci, ci, vp, vp, cf, vp, ci, vp]
-    lib.i2it_op_attention.argtypes = [vp, vp, ci, vp, ci, vp, ci, ci, ci, ci, ci, ci, ci, vp, ci, vp]
+    lib.i2it_op_conv2d_ex.argtypes = [vp, C.POINTER(ConvDesc), vp]
+    lib.i2it_op_launches.argtypes = [vp, C.c_char_p, C.c_size_t]
+    lib.i2it_op_attention.argtypes = [vp, vp, ci, vp, ci, vp, ci, ci, ci, ci, ci, ci, ci, ci, vp, ci, vp]
+    lib.i2it_op_vt_proj.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, ci, vp, vp]
     lib.i2it_op_upsample2x.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp]
+    lib.i2it_op_upsample_to.argtypes = [vp, vp, ci, ci, ci, ci, ci, ci, vp, vp]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("i2it_destroy", "i2it_last_error"):
@@ -269,7 +288,9 @@ class Engine:
         N, H, W, Cin = x_nhwc.shape
         Cout, _, k, _ = w.shape
         oc = Cout // 2 if act == ACT_GEGLU else Cout
-        out = torch.empty(N, H // stride, W // stride, oc, device="cuda", dtype=torch.float32 if out_fp32 else self.dtype)
+        # ceil(H / stride): an odd map is padded to even before a stride-2 conv, as F.conv2d(stride=2, padding=1) sizes it
+        out = torch.empty(N, -(-H // stride), -(-W // stride), oc, device="cuda",
+                          dtype=torch.float32 if out_fp32 else self.dtype)
         w = w.float().contiguous()
         b = bias.float().contiguous() if bias is not None else None
         self._check(self.lib.i2it_op_conv2d(self._h, _ptr(x_nhwc), N, H, W, Cin, x_nhwc.stride(2), _ptr(w), _ptr(b), Cout, k,
@@ -277,6 +298,47 @@ class Engine:
                                             residual.stride(2) if residual is not None else 0, act, _ptr(out), oc,
                                             int(out_fp32), _stream()), "i2it_op_conv2d")
         return out
+
+    def op_conv2d_ex(self, x_nhwc, w, bias=None, *, stride=1, asym_pad=False, residual=None, act=ACT_NONE, out=None,
+                     out_fp32=False, x2=None, w2=None, up2x=False, tokens=False, gn=None, gn_out=None):
+        """Every conv variant of the engine (i2it_conv_desc).  NHWC views may be channel slices (pixel stride > C);
+        `out` / `gn_out` are optional preallocated views.  gn = (gamma, beta, eps, silu) adds the GroupNorm that consumes the
+        output.  Returns out, or (out, groupnorm output) when gn is given."""
+        N, H, W, Cin = x_nhwc.shape
+        Cout, _, k, _ = w.shape
+        oc = Cout // 2 if act == ACT_GEGLU else Cout
+        Ho, Wo = (2 * H, 2 * W) if up2x else (-(-H // stride), -(-W // stride))
+        dt = torch.float32 if out_fp32 else self.dtype
+        if out is None:
+            out = torch.empty(N, Ho, Wo, oc, device="cuda", dtype=dt)
+        assert out.shape == (N, Ho, Wo, oc) and out.dtype == dt and out.stride(3) == 1
+        keep = [w.float().contiguous(), bias.float().contiguous() if bias is not None else None,
+                w2.float().contiguous() if w2 is not None else None]
+        d = ConvDesc()
+        d.x, d.N, d.H, d.W, d.Cin, d.ldx = x_nhwc.data_ptr(), N, H, W, Cin, x_nhwc.stride(2)
+        d.w, d.bias, d.Cout, d.ksize, d.stride, d.asym_pad = _ptr(keep[0]), _ptr(keep[1]), Cout, k, stride, int(asym_pad)
+        d.residual, d.ldr = _ptr(residual), residual.stride(2) if residual is not None else 0
+        d.act, d.out, d.ldo, d.out_fp32 = act, out.data_ptr(), out.stride(2), int(out_fp32)
+        if x2 is not None:
+            d.x2, d.C2, d.ld2, d.w2 = x2.data_ptr(), x2.shape[3], x2.stride(2), _ptr(keep[2])
+        d.up2x, d.tokens = int(up2x), int(tokens)
+        g = None
+        if gn is not None:
+            gamma, beta, eps, silu = gn
+            g = gn_out if gn_out is not None else torch.empty(N, Ho, Wo, oc, device="cuda", dtype=self.dtype)
+            keep += [gamma.float().contiguous(), beta.float().contiguous()]
+            d.gn_y, d.ldg, d.gn_silu, d.gn_eps = g.data_ptr(), g.stride(2), int(silu), float(eps)
+            d.gn_gamma, d.gn_beta = _ptr(keep[3]), _ptr(keep[4])
+        self._check(self.lib.i2it_op_conv2d_ex(self._h, C.byref(d), _stream()), "i2it_op_conv2d_ex")
+        return (out, g) if gn is not None else out
+
+    def op_launches(self):
+        """Launch list of the last op call: [{"kind", "shape"}...]."""
+        import json
+        cap = 1 << 16
+        buf = C.create_string_buffer(cap)
+        self._check(self.lib.i2it_op_launches(self._h, buf, cap), "i2it_op_launches")
+        return json.loads(buf.value.decode())
 
     def op_group_norm(self, x_nhwc, gamma, beta, eps, silu):
         N, H, W, Cc = x_nhwc.shape
@@ -293,16 +355,35 @@ class Engine:
                                                 eps, _ptr(out), Cc, _stream()), "i2it_op_layer_norm")
         return out
 
-    def op_attention(self, q, k, vt, heads):
+    def op_attention(self, q, k, vt, heads, causal=False):
         B, Nq, Cc = q.shape
         kvb, Nk, _ = k.shape
         out = torch.empty_like(q)
         self._check(self.lib.i2it_op_attention(self._h, _ptr(q), q.stride(1), _ptr(k), k.stride(1), _ptr(vt), vt.stride(1), B, Nq,
-                                               Nk, heads, Cc // heads, kvb, _ptr(out), Cc, _stream()), "i2it_op_attention")
+                                               Nk, heads, Cc // heads, kvb, int(causal), _ptr(out), Cc, _stream()),
+                    "i2it_op_attention")
+        return out
+
+    def op_vt_proj(self, x, w, bias=None):
+        """x [B, ntok, Cin] -> (w @ x[b]^T + bias[:, None]) as [B, Cout, round_up(ntok, 8)] (columns past ntok are padding)."""
+        B, ntok, Cin = x.shape
+        Cout = w.shape[0]
+        out = torch.empty(B, Cout, (ntok + 7) // 8 * 8, device="cuda", dtype=self.dtype)
+        w = w.float().contiguous()
+        b = bias.float().contiguous() if bias is not None else None
+        self._check(self.lib.i2it_op_vt_proj(self._h, _ptr(x), B, ntok, Cin, x.stride(1), _ptr(w), _ptr(b), Cout, _ptr(out),
+                                             _stream()), "i2it_op_vt_proj")
         return out
 
     def op_upsample2x(self, x_nhwc):
         N, H, W, Cc = x_nhwc.shape
         out = torch.empty(N, 2 * H, 2 * W, Cc, device="cuda", dtype=self.dtype)
         self._check(self.lib.i2it_op_upsample2x(self._h, _ptr(x_nhwc), N, H, W, Cc, _ptr(out), _stream()), "i2it_op_upsample2x")
+        return out
+
+    def op_upsample_to(self, x_nhwc, Ho, Wo):
+        N, H, W, Cc = x_nhwc.shape
+        out = torch.empty(N, Ho, Wo, Cc, device="cuda", dtype=self.dtype)
+        self._check(self.lib.i2it_op_upsample_to(self._h, _ptr(x_nhwc), N, H, W, Cc, Ho, Wo, _ptr(out), _stream()),
+                    "i2it_op_upsample_to")
         return out

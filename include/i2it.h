@@ -155,17 +155,50 @@ int i2it_read_stage(i2it_handle* h, const char* name, float* dst, size_t dst_ele
 /* ---- diagnostic single-op entry points (used by tests/ to check each kernel against the oracle) ----
  * Activations NHWC with pixel stride ld (elements); weights fp32 device pointers in PyTorch layout.
  * All are synchronous on `stream`. */
+/* The output is [N, Ho, Wo, Cout] (Cout/2 for GEGLU) with Ho = ceil(H / stride): an odd map is zero-padded to even
+ * (as F.conv2d(stride=2, padding=1) does).  The asymmetric VAE padding needs even H and W. */
 int i2it_op_conv2d(i2it_handle* h, const void* x, int N, int H, int W, int Cin, int ldx, const float* w,
                    const float* bias, int Cout, int ksize, int stride, int asym_pad, const void* residual,
                    int ldr, int act, void* out, int ldo, int out_fp32, void* stream);
+/* act values of the conv ops (csrc/tapgemm.cuh TgAct) */
+enum { I2IT_ACT_NONE = 0, I2IT_ACT_CLAMP1 = 1, I2IT_ACT_GEGLU = 2, I2IT_ACT_GELU = 3, I2IT_ACT_QUICKGELU = 4 };
+/* Every variant of the GEMM-backed conv: i2it_op_conv2d's fields plus the ones below.  Zero-initialise unused fields.
+ * LoRA adapters of the op weight are registered as "__op.conv.lora_{A,B}.<adapter>.weight" (scale: i2it_set_adapter_scale). */
+typedef struct i2it_conv_desc {
+  const void* x; int N, H, W, Cin, ldx;
+  const float* w; const float* bias; int Cout, ksize, stride, asym_pad;
+  const void* residual; int ldr;
+  int act;
+  void* out; int ldo, out_fp32;
+  /* second source folded into the same accumulator: out += conv1x1(x2, w2); x2 [N, Ho, Wo, C2] (pixel stride ld2),
+   * w2 [Cout, C2, 1, 1] fp32 */
+  const void* x2; int C2, ld2; const float* w2;
+  int up2x;              /* nearest-2x upsample then the 3x3 conv (sub-pixel: four parity launches); x2 at output size */
+  int tokens;            /* 1x1 only: N images of H*W token rows each (GroupNorm statistics per 128-row tile) */
+  /* gn_y != NULL: GroupNorm(32 groups, gn_eps, gn_gamma/gn_beta, optional SiLU) of the output into gn_y (pixel stride ldg),
+   * with the statistics taken in the conv epilogue where the launch qualifies */
+  void* gn_y; int ldg, gn_silu; float gn_eps; const float* gn_gamma; const float* gn_beta;
+} i2it_conv_desc;
+int i2it_op_conv2d_ex(i2it_handle* h, const i2it_conv_desc* d, void* stream);
+/* Launch list of the last op call, as a JSON array [{"kind","shape"}...] (GEMM shape strings carry BN, tma/tma2, gn;
+ * softmax launches carry their variant 32 / 128 / long). */
+int i2it_op_launches(i2it_handle* h, char* json, size_t cap);
 int i2it_op_group_norm(i2it_handle* h, const void* x, int N, int HW, int C, int ldx, const float* gamma,
                        const float* beta, float eps, int silu, void* out, int ldo, void* stream);
 int i2it_op_layer_norm(i2it_handle* h, const void* x, int rows, int C, int ldx, const float* gamma,
                        const float* beta, float eps, void* out, int ldo, void* stream);
-/* q [B,Nq,heads*d] (ldq), k [B,Nk,heads*d] (ldk), vt [B, heads*d, ldv] (V transposed), out [B,Nq,heads*d] */
+/* q [B,Nq,heads*d] (ldq), k [B,Nk,heads*d] (ldk), vt [B, heads*d, ldv] (V transposed), out [B,Nq,heads*d];
+ * causal (flash path, d = 64 only): query i attends keys 0..i */
 int i2it_op_attention(i2it_handle* h, const void* q, int ldq, const void* k, int ldk, const void* vt, int ldv,
-                      int B, int Nq, int Nk, int heads, int d, int kv_batch, void* out, int ldo, void* stream);
+                      int B, int Nq, int Nk, int heads, int d, int kv_batch, int causal, void* out, int ldo,
+                      void* stream);
+/* V^T projection: x [B*ntok, Cin] (ldx), w [Cout, Cin] fp32, bias [Cout] (nullable) -> out [B][Cout][round_up(ntok, 8)] */
+int i2it_op_vt_proj(i2it_handle* h, const void* x, int B, int ntok, int Cin, int ldx, const float* w, const float* bias,
+                    int Cout, void* out, void* stream);
 int i2it_op_upsample2x(i2it_handle* h, const void* x, int N, int H, int W, int C, void* out, void* stream);
+/* F.interpolate(size=(Ho, Wo), mode="nearest") */
+int i2it_op_upsample_to(i2it_handle* h, const void* x, int N, int H, int W, int C, int Ho, int Wo, void* out,
+                        void* stream);
 
 #ifdef __cplusplus
 }
