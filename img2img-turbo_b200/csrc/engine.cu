@@ -118,7 +118,9 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CUDA(cudaFuncSetAttribute(tapgemm_kernel<__nv_bfloat16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
-  use_flash = std::getenv("I2IT_NO_FLASH") == nullptr;
+  I2IT_CUDA(cudaFuncSetAttribute(flash_attn512_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA5_SMEM));
+  I2IT_CUDA(cudaFuncSetAttribute(flash_attn512_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA5_SMEM));
+  use_flash = std::getenv("I2IT_NO_FLASH") == nullptr;     // both flash kernels (d = 64, and d = 512 above 8192 keys)
   use_pdl = std::getenv("I2IT_PDL") != nullptr;     // programmatic dependent launch: measured neutral (1 CTA/SM kernels cannot co-reside), opt-in
 #ifdef I2IT_TRACE_BUILD
   trace_on = std::getenv("I2IT_TRACE") != nullptr;
@@ -1107,6 +1109,10 @@ Act Engine::vt_proj(Plan& P, const Act& x, int B, int ntok, const PW& wv) {
 Act Engine::attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B, int Nq, int Nk, int heads, int d,
                       int kv_batch) {
   if (d == FA_D && use_flash) return flash_attention(P, q, k, vt, B, Nq, Nk, heads, kv_batch);
+  // The VAE attention (one head of 512) goes fused only where the unfused S + P buffers grow large (N*N*6 bytes per image:
+  // 0.4 GB at Nk = 8192, 100 GB at 4K).  The rule reads the per-image shape only, so every image of a batch takes the same
+  // path as its batch-1 call.  At and below 8192 keys (every 512^2 forward) the unfused path is kept as it was.
+  if (d == FA5_D && heads == 1 && Nk > 8192 && use_flash) return flash_attention512(P, q, k, vt, B, Nq, Nk, kv_batch);
   I2IT_CHECK(d % 64 == 0 && (d <= 256 || d % 256 == 0), "attention: head dim must be a multiple of 64");
 
   I2IT_CHECK(kv_batch == B || kv_batch == 1, "attention: kv batch must be 1 or B");
@@ -1248,6 +1254,49 @@ Act Engine::flash_attention(Plan& P, const Act& q, const Act& k, const Act& vt, 
   add_op(P, [=](cudaStream_t st) {
     DISPATCH_T(dt, (launch_k(flash_attn_kernel<T>, dim3(grid), dim3(FA_THREADS), FA_SMEM, st, 0, tq, tk, tv, fp)));
   }, "flash_attn", 4.0 * B * heads * Nq * Nk * d, 2.0 * (2.0 * B * Nq * C + 2.0 * kv_batch * Nk * C), shp);
+  return out;
+}
+
+Act Engine::flash_attention512(Plan& P, const Act& q, const Act& k, const Act& vt, int B, int Nq, int Nk, int kv_batch) {
+  I2IT_CHECK(kv_batch == B || kv_batch == 1, "attention: kv batch must be 1 or B");
+  const int d = FA5_D;
+  Act out = alloc_act(P, B, 1, Nq, d);
+  TmapSpec sq, sk, sv;
+  sq.base = q.p;
+  sq.dim[0] = d; sq.dim[1] = Nq; sq.dim[2] = B;
+  sq.stride[0] = q.ld * 2ull; sq.stride[1] = 2ull * Nq * q.ld;
+  sq.box[0] = 64; sq.box[1] = FA5_BM;
+  fill_strides(sq);
+  sk.base = k.p;
+  sk.dim[0] = d; sk.dim[1] = Nk; sk.dim[2] = kv_batch;
+  sk.stride[0] = k.ld * 2ull; sk.stride[1] = 2ull * Nk * k.ld;
+  sk.box[0] = 64; sk.box[1] = FA5_BN;
+  fill_strides(sk);
+  const int ldv = vt.ld;
+  sv.base = vt.p;
+  sv.dim[0] = Nk; sv.dim[1] = d; sv.dim[2] = kv_batch;
+  sv.stride[0] = ldv * 2ull; sv.stride[1] = 2ull * d * ldv;
+  sv.box[0] = FA5_BN; sv.box[1] = 64;
+  fill_strides(sv);
+  FlashParams fp;
+  std::memset(&fp, 0, sizeof fp);
+  fp.Nq = Nq; fp.Nk = Nk; fp.heads = 1; fp.B = B;
+  fp.q_tiles = ceil_div(Nq, FA5_BM);
+  fp.kv_bmul = (kv_batch == B) ? 1 : 0;
+  fp.scale_log2e = (1.0f / sqrtf(static_cast<float>(d))) * 1.4426950408889634f;
+  fp.out = out.p;
+  fp.ldo = out.ld;
+  fp.err = d_err;
+  const CUtensorMap tq = encode_tmap(sq, dtype), tk = encode_tmap(sk, dtype), tv = encode_tmap(sv, dtype);
+  const long long grid = 2ll * fp.q_tiles * B;
+  I2IT_CHECK(grid < (1ll << 31), "attention: too many query tiles");
+  const int dt = dtype;
+  char shp[96];
+  snprintf(shp, sizeof shp, "B=%d h=1 Nq=%d Nk=%d d=%d", B, Nq, Nk, d);
+  add_op(P, [=](cudaStream_t st) {
+    DISPATCH_T(dt, (launch_k(flash_attn512_kernel<T>, dim3(static_cast<unsigned>(grid)), dim3(FA5_THREADS), FA5_SMEM, st, 0,
+                             tq, tk, tv, fp)));
+  }, "flash_attn512", 4.0 * B * Nq * Nk * d, 2.0 * (2.0 * B * Nq * d + 2.0 * kv_batch * Nk * d), shp);
   return out;
 }
 

@@ -202,6 +202,7 @@ class Engine {
                 int kv_batch);
   Act flash_attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B, int Nq, int Nk, int heads, int kv_batch,
                       bool causal = false);
+  Act flash_attention512(Plan& P, const Act& q, const Act& k, const Act& vt, int B, int Nq, int Nk, int kv_batch);
   bool use_flash = true;
 
   // ---- weights ----

@@ -193,4 +193,188 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   }
 }
 
+// flash_attn512_kernel: fused softmax(Q K^T / sqrt(512)) V for ONE head of 512 (the VAE mid-block attention), used where
+// the unfused path's fp32 logits (B * N * N * 6 bytes for S and P) would not fit: a 4K frame needs 100 GB of them.
+//
+// A 64-row x 512 fp32 O tile is 256 registers per thread, so each CTA owns one 64-row Q tile and one HALF (256 columns) of
+// d_v; grid = 2 x q_tiles x B, the two halves of a Q tile adjacent in launch order so K / V^T come from L2 the second time.
+// S is recomputed by both halves (1.5x the minimal MMA work) to keep the d = 64 kernel's structure: S and O in registers,
+// P fed back as the register A operand.  One consumer warpgroup per CTA: O (128) + S (32) + P (16) registers per thread
+// need more than the 168 a 9-warp CTA can have (three warps share an SM sub-partition's 16K registers; ptxas did not honour
+// setmaxnreg for a second warpgroup), while 5 warps get up to 255.  160 threads, 1 CTA per SM:
+//   warp 4      : TMA producer  Q once (8 boxes of 64 rows x 64 d, 64 KB, resident); per KV tile j twelve 64 x 64
+//                 128B-swizzled boxes, K_j's 8 d-chunks then V^T_j's 4 column blocks of this half, through a 20-slot ring
+//   warps 0..3  : S_j = Q K_j^T    8 chunks x 4 wgmma m64n64k16 (smem x smem); the K slots are released when S is complete
+//                 online softmax exactly as flash_attn_kernel (fp32 logits, ex2.approx, row sum over the ROUNDED P)
+//                 O[:, 64c..] += P_j V_j   4 column blocks x 4 wgmma m64n64k16, P as the register A operand
+// Shared memory: Q 64 KB + ring 20 x 8 KB = 224 KB: the producer runs up to 1.6 KV tiles ahead.  Numerics per element do not
+// depend on B or on the tile's position: image i of a batch is bit for bit its batch-1 result.
+constexpr int FA5_BM = 64, FA5_BN = 64, FA5_D = 512, FA5_DV = 256;    // FA5_DV: the d_v half one CTA produces
+constexpr int FA5_KCH = FA5_D / 64, FA5_VCH = FA5_DV / 64;            // 8 K boxes + 4 V^T boxes per KV tile
+constexpr int FA5_SLOTS = 20;
+constexpr int FA5_BOX = 64 * 64 * 2;                                   // 8 KiB; a Q box (64 rows x 64 d) is the same size
+constexpr int FA5_Q_BYTES = FA5_KCH * FA5_BOX;                         // 64 KiB
+constexpr int FA5_SMEM = FA5_Q_BYTES + FA5_SLOTS * FA5_BOX + 512 + 1024;
+constexpr int FA5_THREADS = 160;
+
+template <typename T>
+__global__ void __launch_bounds__(FA5_THREADS, 1)
+flash_attn512_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                     const __grid_constant__ CUtensorMap tmVt, const __grid_constant__ FlashParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sQ = base;
+  const uint32_t sR = base + FA5_Q_BYTES;
+  const uint32_t bars = sR + FA5_SLOTS * FA5_BOX;
+  const uint32_t q_full = bars;
+  auto full = [&](int i) { return bars + 8u * (1 + i); };
+  auto empty = [&](int i) { return bars + 8u * (1 + FA5_SLOTS + i); };
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int half = blockIdx.x & 1;
+  const int qt = (blockIdx.x >> 1) % p.q_tiles;
+  const int b = (blockIdx.x >> 1) / p.q_tiles;
+  const int nkv = (p.Nk + FA5_BN - 1) / FA5_BN;
+
+  if (warp == 4 && lane == 0) {
+    mbar_init(q_full, 1);
+    for (int i = 0; i < FA5_SLOTS; ++i) { mbar_init(full(i), 1); mbar_init(empty(i), 4); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmQ)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmK)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmVt)) : "memory");
+  }
+  __syncthreads();
+  pdl_sync();
+
+  if (warp == 4) {
+    if (elect_one()) {
+      mbar_expect_tx(q_full, FA5_Q_BYTES);
+      for (int c = 0; c < FA5_KCH; ++c) tma_load_5d(sQ + c * FA5_BOX, &tmQ, q_full, 64 * c, qt * FA5_BM, b, 0, 0);
+    }
+    __syncwarp();
+    const int kb = b * p.kv_bmul;
+    int slot = 0, ph = 0;
+    for (int j = 0; j < nkv; ++j) {
+      for (int i = 0; i < FA5_KCH + FA5_VCH; ++i) {
+        mbar_wait(empty(slot), ph ^ 1, p.err, 21);
+        if (elect_one()) {
+          const uint32_t dst = sR + slot * FA5_BOX;
+          mbar_expect_tx(full(slot), FA5_BOX);
+          if (i < FA5_KCH) tma_load_5d(dst, &tmK, full(slot), 64 * i, j * FA5_BN, kb, 0, 0);
+          else tma_load_5d(dst, &tmVt, full(slot), j * FA5_BN, half * FA5_DV + 64 * (i - FA5_KCH), kb, 0, 0);
+        }
+        __syncwarp();
+        if (++slot == FA5_SLOTS) { slot = 0; ph ^= 1; }
+      }
+    }
+  } else {
+    // thread (warp w, lane l) holds rows r and r + 8, r = 16 w + l / 4
+    const int q0 = qt * FA5_BM + warp * 16 + (lane >> 2), q1 = q0 + 8;
+    const float sc = p.scale_log2e;
+    const int ccol = 2 * (lane & 3);
+    float o[FA5_VCH][32];
+#pragma unroll
+    for (int c = 0; c < FA5_VCH; ++c)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    mbar_wait(q_full, 0, p.err, 22);
+    int slot = 0, ph = 0;       // ring position of the tile's first box
+    for (int j = 0; j < nkv; ++j) {
+      int sl[FA5_KCH + FA5_VCH], pp[FA5_KCH + FA5_VCH];
+#pragma unroll
+      for (int i = 0; i < FA5_KCH + FA5_VCH; ++i) {
+        sl[i] = slot; pp[i] = ph;
+        if (++slot == FA5_SLOTS) { slot = 0; ph ^= 1; }
+      }
+      float sacc[32];
+      // every wait precedes the MMA chain: a (divergent) spin between two wgmmas makes ptxas serialise them
+      for (int c = 0; c < FA5_KCH; ++c) mbar_wait(full(sl[c]), pp[c], p.err, 23);
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < FA5_KCH; ++c) {
+        const uint64_t qd = wgmma_desc_sw128(sQ + c * FA5_BOX), kd = wgmma_desc_sw128(sR + sl[c] * FA5_BOX);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_ss<64, T>(sacc, qd + 2 * k, kd + 2 * k, (c | k) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0)
+        for (int c = 0; c < FA5_KCH; ++c) mbar_arrive(empty(sl[c]));
+      const int kbase = j * FA5_BN;
+      if (kbase + FA5_BN > p.Nk) {
+#pragma unroll
+        for (int g = 0; g < 8; ++g)
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            if (kbase + 8 * g + ccol + (e & 1) >= p.Nk) sacc[4 * g + e] = -INFINITY;
+      }
+      float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        mx0 = fmaxf(mx0, fmaxf(sacc[4 * g], sacc[4 * g + 1]));
+        mx1 = fmaxf(mx1, fmaxf(sacc[4 * g + 2], sacc[4 * g + 3]));
+      }
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+      const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+      const float f0 = (mn0 == -INFINITY) ? 1.f : fast_exp2((m0 - mn0) * sc);
+      const float f1 = (mn1 == -INFINITY) ? 1.f : fast_exp2((m1 - mn1) * sc);
+      const float ng0 = (mn0 == -INFINITY) ? 0.f : -mn0 * sc, ng1 = (mn1 == -INFINITY) ? 0.f : -mn1 * sc;
+      m0 = mn0; m1 = mn1;
+      uint32_t pk[16];
+      float ls0 = 0.f, ls1 = 0.f;
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        pk[2 * g] = Elem<T>::pack(fast_exp2(fmaf(sacc[4 * g], sc, ng0)), fast_exp2(fmaf(sacc[4 * g + 1], sc, ng0)));
+        pk[2 * g + 1] = Elem<T>::pack(fast_exp2(fmaf(sacc[4 * g + 2], sc, ng1)), fast_exp2(fmaf(sacc[4 * g + 3], sc, ng1)));
+        const float2 a = Elem<T>::unpack(pk[2 * g]), c = Elem<T>::unpack(pk[2 * g + 1]);
+        ls0 += a.x + a.y;
+        ls1 += c.x + c.y;
+      }
+      ls0 += __shfl_xor_sync(0xffffffffu, ls0, 1); ls0 += __shfl_xor_sync(0xffffffffu, ls0, 2);
+      ls1 += __shfl_xor_sync(0xffffffffu, ls1, 1); ls1 += __shfl_xor_sync(0xffffffffu, ls1, 2);
+      l0 = l0 * f0 + ls0;
+      l1 = l1 * f1 + ls1;
+#pragma unroll
+      for (int c = 0; c < FA5_VCH; ++c)
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+          o[c][4 * g] *= f0; o[c][4 * g + 1] *= f0;
+          o[c][4 * g + 2] *= f1; o[c][4 * g + 3] *= f1;
+        }
+      for (int c = 0; c < FA5_VCH; ++c) mbar_wait(full(sl[FA5_KCH + c]), pp[FA5_KCH + c], p.err, 24);
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < FA5_VCH; ++c) {
+        const uint64_t vd = wgmma_desc_sw128(sR + sl[FA5_KCH + c] * FA5_BOX);
+#pragma unroll
+        for (int kk = 0; kk < FA5_BN / 16; ++kk) {
+          const uint32_t a[4] = {pk[4 * kk], pk[4 * kk + 1], pk[4 * kk + 2], pk[4 * kk + 3]};
+          wgmma_rs64<T>(o[c], a, vd + 2 * kk);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0)
+        for (int c = 0; c < FA5_VCH; ++c) mbar_arrive(empty(sl[FA5_KCH + c]));
+    }
+    const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+    T* const obase = reinterpret_cast<T*>(p.out) + static_cast<long long>(b) * p.Nq * p.ldo + half * FA5_DV + ccol;
+#pragma unroll
+    for (int c = 0; c < FA5_VCH; ++c)
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        if (q0 < p.Nq)
+          *reinterpret_cast<uint32_t*>(obase + q0 * p.ldo + 64 * c + 8 * g) = Elem<T>::pack(o[c][4 * g] * inv0, o[c][4 * g + 1] * inv0);
+        if (q1 < p.Nq)
+          *reinterpret_cast<uint32_t*>(obase + q1 * p.ldo + 64 * c + 8 * g) =
+              Elem<T>::pack(o[c][4 * g + 2] * inv1, o[c][4 * g + 3] * inv1);
+      }
+  }
+}
+
 }  // namespace i2it
