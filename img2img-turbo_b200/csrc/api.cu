@@ -183,6 +183,31 @@ int i2it_read_stage(i2it_handle* h, const char* name, float* dst, size_t dst_ele
   API_END
 }
 
+static void copy_json(const std::string& js, char* json, size_t cap, const char* what) {
+  I2IT_CHECK(json != nullptr && cap > 2, std::string(what) + ": bad arguments");
+  I2IT_CHECK(js.size() + 1 <= cap, std::string(what) + ": buffer too small (" + std::to_string(js.size() + 1) + " bytes needed)");
+  std::memcpy(json, js.c_str(), js.size() + 1);
+}
+
+int i2it_stage_names(i2it_handle* h, char* json, size_t cap) {
+  API_BEGIN(h)
+  copy_json(E.stage_names_json(), json, cap, "i2it_stage_names");
+  API_END
+}
+
+int i2it_prepared_keys(i2it_handle* h, char* json, size_t cap) {
+  API_BEGIN(h)
+  copy_json(E.prepared_keys_json(), json, cap, "i2it_prepared_keys");
+  API_END
+}
+
+int i2it_read_prepared(i2it_handle* h, const char* key, void* w, size_t w_elems, float* bias, size_t b_elems, int dims[4]) {
+  API_BEGIN(h)
+  I2IT_CHECK(key != nullptr && dims != nullptr, "i2it_read_prepared: null argument");
+  E.read_prepared(key, w, w_elems, bias, b_elems, dims);
+  API_END
+}
+
 // ------------------------------------------------------------------------------------------------
 // diagnostic single-op entry points
 // ------------------------------------------------------------------------------------------------

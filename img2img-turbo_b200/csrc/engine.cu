@@ -1536,4 +1536,42 @@ void Engine::read_stage(const std::string& name_in, float* dst, size_t dst_elems
   I2IT_CUDA(cudaDeviceSynchronize());
 }
 
+std::string Engine::stage_names_json() const {
+  I2IT_CHECK(last_plan_ != nullptr, "no forward has run yet");
+  std::string js = "[";
+  for (size_t i = 0; i < last_plan_->stage_order.size(); ++i) {
+    const std::string& n = last_plan_->stage_order[i];
+    const Act& a = last_plan_->stages.at(n);
+    js += std::string(i ? "," : "") + "{\"name\":\"" + n + "\",\"dims\":[" + std::to_string(a.N) + "," + std::to_string(a.C) + "," +
+          std::to_string(a.H) + "," + std::to_string(a.W) + "]}";
+  }
+  return js + "]";
+}
+
+std::string Engine::prepared_keys_json() const {
+  std::vector<std::string> keys;
+  for (const auto& kv : prepared_) keys.push_back(kv.first);
+  std::sort(keys.begin(), keys.end());
+  std::string js = "[";
+  for (size_t i = 0; i < keys.size(); ++i) js += std::string(i ? "," : "") + "\"" + keys[i] + "\"";
+  return js + "]";
+}
+
+void Engine::read_prepared(const std::string& key, void* w, size_t w_elems, float* bias, size_t b_elems, int dims[4]) {
+  auto it = prepared_.find(key);
+  I2IT_CHECK(it != prepared_.end(), "unknown prepared weight '" + key + "'");
+  const PW& pw = it->second;
+  dims[0] = pw.taps; dims[1] = pw.rows; dims[2] = pw.cin_pad; dims[3] = pw.bias ? 1 : 0;
+  const size_t n = static_cast<size_t>(pw.taps) * pw.rows * pw.cin_pad;
+  I2IT_CUDA(cudaDeviceSynchronize());                     // preparation runs on the default stream
+  if (w) {
+    I2IT_CHECK(n <= w_elems, "read_prepared: weight destination too small");
+    I2IT_CUDA(cudaMemcpy(w, pw.w, n * 2, cudaMemcpyDefault));
+  }
+  if (bias && pw.bias) {
+    I2IT_CHECK(static_cast<size_t>(pw.rows) <= b_elems, "read_prepared: bias destination too small");
+    I2IT_CUDA(cudaMemcpy(bias, pw.bias, pw.rows * sizeof(float), cudaMemcpyDefault));
+  }
+}
+
 }  // namespace i2it

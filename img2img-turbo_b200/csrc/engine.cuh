@@ -114,6 +114,7 @@ struct Plan {
   std::vector<std::function<void(cudaStream_t)>> ops;  // one kernel launch each
   std::vector<OpMeta> meta;                            // parallel to ops
   std::map<std::string, Act> stages;
+  std::vector<std::string> stage_order;                // stage names in build order (i2it_stage_names)
   struct Trace { unsigned long long* buf; int grid; std::string what; };
   std::vector<Trace> traces;                           // I2IT_TRACE=1 only
   std::vector<std::shared_ptr<void>> keep;
@@ -181,6 +182,10 @@ class Engine {
   bool has_text_encoder() const { return has("text_encoder.text_model.embeddings.token_embedding.weight"); }
   Plan* last_plan() const { return last_plan_; }
   void read_stage(const std::string& name, float* dst, size_t dst_elems, int dims[4]);
+  std::string stage_names_json() const;                              // last forward's stages, build order, with dims
+  std::string prepared_keys_json() const;                            // every prepared-weight cache key, sorted
+  // a prepared weight exactly as the kernels read it: [taps][rows][cin_pad] 16-bit + fp32 bias; dims = taps, rows, cin_pad, has_bias
+  void read_prepared(const std::string& key, void* w, size_t w_elems, float* bias, size_t b_elems, int dims[4]);
 
   // ---- op builders (append launches to a plan) ----
   Act alloc_act(Plan& P, int N, int H, int W, int C, int ld = 0, bool zero_persistent = false);
@@ -234,7 +239,14 @@ class Engine {
   Act unet_resnet(Plan& P, const std::string& p, const Act& x, bool gn_next = false, const Act* out = nullptr);
   Act unet_xformer(Plan& P, const std::string& p, const Act& x, int heads, int text_batch, bool gn_next = false,
                    const Act* out = nullptr);
-  void mark(Plan& P, const std::string& name, const Act& a) { if (cfg.keep_stages) P.stages[name] = a; }
+  // keep_stages >= 1: the named checkpoints (skip0, latent, model_pred, ...); keep_stages >= 2 also every layer output under its
+  // state-dict prefix (mark_layer), for the per-layer audit of tests/layer_audit.py.  Marks hold tensors; they add no launches.
+  void mark(Plan& P, const std::string& name, const Act& a) { if (cfg.keep_stages) keep_stage(P, name, a); }
+  void mark_layer(Plan& P, const std::string& name, const Act& a) { if (cfg.keep_stages >= 2) keep_stage(P, name, a); }
+  void keep_stage(Plan& P, const std::string& name, const Act& a) {
+    if (!P.stages.count(name)) P.stage_order.push_back(name);
+    P.stages[name] = a;
+  }
 
   template <typename F> void add_op(Plan& P, F&& f, const char* kind = "misc", double flops = 0, double bytes = 0,
                                     const std::string& shape = "") {

@@ -22,9 +22,12 @@ static inline int ceil_div_i(long long a, long long b) { return static_cast<int>
 // ------------------------------------------------------------------------------------------ VAE
 Act Engine::vae_resnet(Plan& P, const std::string& p, const Act& x, const Act* skip, const PW* skip_w, bool gn_next) {
   Act h = group_norm(P, x, norm(p + ".norm1"), 1e-6f, true);
+  mark_layer(P, p + ".norm1", h);
   ConvOpts o1; o1.gn_out = true;                     // conv1 feeds norm2: its epilogue takes the GroupNorm statistics
   h = conv(P, h, prep(p + ".conv1", {p + ".conv1"}), o1);
+  mark_layer(P, p + ".conv1", h);
   h = group_norm(P, h, norm(p + ".norm2"), 1e-6f, true);
+  mark_layer(P, p + ".norm2", h);
   ConvOpts o;
   o.gn_out = gn_next;                                // the block's output feeds another GroupNorm (norm1 / attention / conv_norm_out)
   if (has(p + ".conv_shortcut.weight")) {
@@ -34,22 +37,32 @@ Act Engine::vae_resnet(Plan& P, const std::string& p, const Act& x, const Act* s
     PW wsc = prep(p + ".conv_shortcut", {p + ".conv_shortcut"});
     PW w2 = prep(p + ".conv2+sc", {p + ".conv2"}, false, 1.f, raw(p + ".conv_shortcut", "bias").d);
     o.x2 = &x; o.w2 = &wsc;
-    return conv(P, h, w2, o);
+    Act y = conv(P, h, w2, o);
+    mark_layer(P, p + ".conv2", y);
+    return y;
   }
   o.res = &x;
   if (skip) { o.x2 = skip; o.w2 = skip_w; }        // decoder: the next block's  + skip_conv(skip*gamma)  folded in here
-  return conv(P, h, prep(p + ".conv2", {p + ".conv2"}), o);
+  Act y = conv(P, h, prep(p + ".conv2", {p + ".conv2"}), o);
+  mark_layer(P, p + ".conv2", y);
+  return y;
 }
 
 Act Engine::vae_attn(Plan& P, const std::string& p, const Act& x) {
   // diffusers Attention (1 head, d = C) with residual; tokens are the NHWC pixels
   const int C = x.C, B = x.N, N = x.H * x.W;
   Act t = group_norm(P, x, norm(p + ".group_norm"), 1e-6f, false);
+  mark_layer(P, p + ".group_norm", t);
   Act qk = linear(P, t, prep(p + ".qk", {p + ".to_q", p + ".to_k"}));
+  mark_layer(P, p + ".qk", qk);
   Act vt = vt_proj(P, t, B, N, prep(p + ".to_v", {p + ".to_v"}));
+  mark_layer(P, p + ".to_v", vt);
   Act a = attention(P, qk.slice(0, C), qk.slice(C, C), vt, B, N, N, 1, C, B);
   a.N = x.N; a.H = x.H; a.W = x.W;
-  return linear(P, a, prep(p + ".to_out.0", {p + ".to_out.0"}), &x, TG_ACT_NONE, true);   // -> mid_block.resnets.1.norm1
+  mark_layer(P, p, a);
+  Act y = linear(P, a, prep(p + ".to_out.0", {p + ".to_out.0"}), &x, TG_ACT_NONE, true);   // -> mid_block.resnets.1.norm1
+  mark_layer(P, p + ".to_out.0", y);
+  return y;
 }
 
 Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int W, std::vector<Act>& skips, bool u8_in) {
@@ -74,8 +87,10 @@ Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int 
       }, "pack_im2col", 0, 2.0 * total * (3 + 32));
     }
   }
+  mark_layer(P, e + ".conv_in.im2col", xcol);
   ConvOpts oin; oin.ksize = 1; oin.gn_out = true;
   Act s = conv(P, xcol, prep_im2col3(e + ".conv_in"), oin);
+  mark_layer(P, e + ".conv_in", s);
   xcol = Act();
   for (int i = 0; i < 4; ++i) {
     skips.push_back(s);                                   // model.py:18-20: the INPUT of each down block
@@ -87,6 +102,7 @@ Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int 
       ConvOpts o; o.stride = 2; o.asym = true; o.gn_out = true;
       const std::string d = e + ".down_blocks." + std::to_string(i) + ".downsamplers.0.conv";
       s = conv(P, s, prep(d, {d}), o);
+      mark_layer(P, d, s);
     }
   }
   s = vae_resnet(P, e + ".mid_block.resnets.0", s);
@@ -94,7 +110,9 @@ Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int 
   s = vae_resnet(P, e + ".mid_block.resnets.1", s);
   mark(P, "enc_mid", s);
   s = group_norm(P, s, norm(e + ".conv_norm_out"), 1e-6f, true);
+  mark_layer(P, e + ".conv_norm_out", s);
   s = conv(P, s, prep(e + ".conv_out", {e + ".conv_out"}), ConvOpts());
+  mark_layer(P, e + ".conv_out", s);
   ConvOpts o1; o1.ksize = 1;
   Act mom = conv(P, s, prep(vp + "quant_conv", {vp + "quant_conv"}), o1);
   mark(P, "moments", mom);
@@ -121,7 +139,9 @@ void Engine::build_vae_decoder(Plan& P, const std::string& vp, const Act& dec_in
   const std::string d = vp + "decoder";
   ConvOpts o1; o1.ksize = 1;
   Act s = conv(P, dec_in, prep(vp + "post_quant_conv", {vp + "post_quant_conv"}), o1);
+  mark_layer(P, vp + "post_quant_conv", s);
   { ConvOpts oc; oc.gn_out = true; s = conv(P, s, prep(d + ".conv_in", {d + ".conv_in"}), oc); }
+  mark_layer(P, d + ".conv_in", s);
   // `sample = sample + skip_conv_i(skip_i * gamma)` (src/model.py:40-42) is folded into whichever conv PRODUCES `sample`
   // for up-block i: mid_block.resnets.1.conv2 for i = 0, the previous block's upsampler conv for i >= 1.  gamma is folded
   // into the bias-free 1x1 weights.
@@ -144,11 +164,13 @@ void Engine::build_vae_decoder(Plan& P, const std::string& vp, const Act& dec_in
       const std::string u = d + ".up_blocks." + std::to_string(i) + ".upsamplers.0.conv";
       PW wn = skip_w(i + 1);
       s = conv_up2x(P, s, prep_subpixel(u), &skips[2 - i], &wn, true);
+      mark_layer(P, u, s);
       skips[2 - i] = Act();
     }
     mark(P, "dec_up" + std::to_string(i), s);
   }
   s = group_norm(P, s, norm(d + ".conv_norm_out"), 1e-6f, true);
+  mark_layer(P, d + ".conv_norm_out", s);
   if (cfg.keep_stages) {   // tests compare the PRE-clamp image (BASELINE.md section 5): one extra launch, test mode only
     Act pre = conv(P, s, prep(d + ".conv_out", {d + ".conv_out"}), ConvOpts());
     mark(P, "pre_clamp", pre);
@@ -160,10 +182,13 @@ void Engine::build_vae_decoder(Plan& P, const std::string& vp, const Act& dec_in
 // ------------------------------------------------------------------------------------------ UNet
 Act Engine::unet_resnet(Plan& P, const std::string& p, const Act& x, bool gn_next, const Act* out) {
   Act h = group_norm(P, x, norm(p + ".norm1"), 1e-5f, true);
+  mark_layer(P, p + ".norm1", h);
   // t == 999 always: time_emb_proj(silu(emb)) is a per-channel constant -> part of conv1's bias
   ConvOpts o1; o1.gn_out = true;
   h = conv(P, h, prep(p + ".conv1", {p + ".conv1"}, false, 1.f, temb_bias(p)), o1);
+  mark_layer(P, p + ".conv1", h);
   h = group_norm(P, h, norm(p + ".norm2"), 1e-5f, true);
+  mark_layer(P, p + ".norm2", h);
   ConvOpts o;
   o.gn_out = gn_next;
   o.out = out;
@@ -171,28 +196,41 @@ Act Engine::unet_resnet(Plan& P, const std::string& p, const Act& x, bool gn_nex
     PW wsc = prep(p + ".conv_shortcut", {p + ".conv_shortcut"});
     PW w2 = prep(p + ".conv2+sc", {p + ".conv2"}, false, 1.f, raw(p + ".conv_shortcut", "bias").d);
     o.x2 = &x; o.w2 = &wsc;
-    return conv(P, h, w2, o);
+    Act y = conv(P, h, w2, o);
+    mark_layer(P, p + ".conv2", y);
+    return y;
   }
   o.res = &x;
-  return conv(P, h, prep(p + ".conv2", {p + ".conv2"}), o);
+  Act y = conv(P, h, prep(p + ".conv2", {p + ".conv2"}), o);
+  mark_layer(P, p + ".conv2", y);
+  return y;
 }
 
 Act Engine::unet_xformer(Plan& P, const std::string& p, const Act& x, int heads, int text_batch, bool gn_next, const Act* out) {
   const int C = x.C, B = x.N, N = x.H * x.W, d = C / heads;
   const std::string b = p + ".transformer_blocks.0";
   Act t = group_norm(P, x, norm(p + ".norm"), 1e-6f, false);
+  mark_layer(P, p + ".norm", t);
   t = linear(P, t, prep(p + ".proj_in", {p + ".proj_in"}));
+  mark_layer(P, p + ".proj_in", t);
   {  // self-attention
     Act n = layer_norm(P, t, norm(b + ".norm1"));
+    mark_layer(P, b + ".norm1", n);
     Act qk = linear(P, n, prep(b + ".attn1.qk", {b + ".attn1.to_q", b + ".attn1.to_k"}));
+    mark_layer(P, b + ".attn1.qk", qk);
     Act vt = vt_proj(P, n, B, N, prep(b + ".attn1.to_v", {b + ".attn1.to_v"}));
+    mark_layer(P, b + ".attn1.to_v", vt);
     Act a = attention(P, qk.slice(0, C), qk.slice(C, C), vt, B, N, N, heads, d, B);
     a.N = x.N; a.H = x.H; a.W = x.W;
+    mark_layer(P, b + ".attn1", a);
     t = linear(P, a, prep(b + ".attn1.to_out.0", {b + ".attn1.to_out.0"}), &t);
+    mark_layer(P, b + ".attn1.to_out.0", t);
   }
   {  // cross-attention over the 77 text tokens
     Act n = layer_norm(P, t, norm(b + ".norm2"));
+    mark_layer(P, b + ".norm2", n);
     Act q = linear(P, n, prep(b + ".attn2.to_q", {b + ".attn2.to_q"}));
+    mark_layer(P, b + ".attn2.to_q", q);
     Act k2, v2t;
     if (text_kv_) {                                   // computed once per prompt by i2it_set_text
       auto it = text_kv_->kv.find(b);
@@ -202,16 +240,25 @@ Act Engine::unet_xformer(Plan& P, const std::string& p, const Act& x, int heads,
       k2 = linear(P, text_, prep(b + ".attn2.to_k", {b + ".attn2.to_k"}));
       v2t = vt_proj(P, text_, text_batch, 77, prep(b + ".attn2.to_v", {b + ".attn2.to_v"}));
     }
+    mark_layer(P, b + ".attn2.to_k", k2);            // inline or cached: the audit checks both against this block's weights
+    mark_layer(P, b + ".attn2.to_v", v2t);
     Act a = attention(P, q, k2, v2t, B, N, 77, heads, d, text_batch);
     a.N = x.N; a.H = x.H; a.W = x.W;
+    mark_layer(P, b + ".attn2", a);
     t = linear(P, a, prep(b + ".attn2.to_out.0", {b + ".attn2.to_out.0"}), &t);
+    mark_layer(P, b + ".attn2.to_out.0", t);
   }
   {  // GEGLU feed-forward: h * gelu(g) fused into the first projection's epilogue (weight rows interleaved)
     Act n = layer_norm(P, t, norm(b + ".norm3"));
+    mark_layer(P, b + ".norm3", n);
     Act g = linear(P, n, prep(b + ".ff.net.0.proj", {b + ".ff.net.0.proj"}, true), nullptr, TG_ACT_GEGLU);
+    mark_layer(P, b + ".ff.net.0.proj", g);
     t = linear(P, g, prep(b + ".ff.net.2", {b + ".ff.net.2"}), &t);
+    mark_layer(P, b + ".ff.net.2", t);
   }
-  return linear(P, t, prep(p + ".proj_out", {p + ".proj_out"}), &x, TG_ACT_NONE, gn_next, out);
+  Act y = linear(P, t, prep(p + ".proj_out", {p + ".proj_out"}), &x, TG_ACT_NONE, gn_next, out);
+  mark_layer(P, p + ".proj_out", y);
+  return y;
 }
 
 // every transformer block of the UNet, in execution-independent fixed order (the cross-attention K/V^T cache is keyed by it)
@@ -298,6 +345,7 @@ Act Engine::build_unet(Plan& P, const Act& z, int text_batch, bool text_cached) 
       s = conv(P, z, prep_twin(u + ".conv_in.conv_in_pretrained", u + ".conv_in.conv_in_curr", twin_r_), oc);
     else
       s = conv(P, z, prep(u + ".conv_in", {u + ".conv_in"}), oc);
+    mark_layer(P, u + ".conv_in", s);
     push(t, s);
   }
   for (int i = 0; i < 4; ++i) {
@@ -316,6 +364,7 @@ Act Engine::build_unet(Plan& P, const Act& z, int text_batch, bool text_cached) 
       ConvOpts o; o.stride = 2; o.gn_out = true;
       if (fuse) o.out = &t.skip;
       s = conv(P, s, prep(blk + ".downsamplers.0.conv", {blk + ".downsamplers.0.conv"}), o);
+      mark_layer(P, blk + ".downsamplers.0.conv", s);
       push(t, s);
     }
   }
@@ -344,6 +393,7 @@ Act Engine::build_unet(Plan& P, const Act& z, int text_batch, bool text_cached) 
         copy_channels(P, t.skip, cat.slice(s.C, t.skip.C));
       }
       t = SkipSlot();
+      mark_layer(P, blk + ".resnets." + std::to_string(j) + ".concat", cat);   // torch.cat([h, skip], dim=1)
       const bool last = (i == 3 && j == 2);                            // the very last block feeds conv_norm_out directly
       // the block's output is the next concat's `h` unless an upsampler (j == 2, i < 3) or conv_norm_out (last) follows
       Act tgt;
@@ -358,15 +408,18 @@ Act Engine::build_unet(Plan& P, const Act& z, int text_batch, bool text_cached) 
       // — nearest to the spatial size of the next skip connection (e.g. 14 -> 27 columns for a 560x840 image)
       const SkipSlot& nxt = res.back();
       s = upsample_to(P, s, nxt.skip.H, nxt.skip.W);
+      mark_layer(P, blk + ".upsamplers.0.nearest", s);
       Act tgt;
       ConvOpts oc;
       if (fuse) { tgt = h_target(); oc.out = &tgt; }
       s = conv(P, s, prep(blk + ".upsamplers.0.conv", {blk + ".upsamplers.0.conv"}), oc);
+      mark_layer(P, blk + ".upsamplers.0.conv", s);
     }
   }
   I2IT_CHECK(res.empty(), "unet: residual stack not consumed");
   (void)ch;
   s = group_norm(P, s, norm(u + ".conv_norm_out"), 1e-5f, true);
+  mark_layer(P, u + ".conv_norm_out", s);
   s = conv(P, s, prep(u + ".conv_out", {u + ".conv_out"}), ConvOpts());
   text_ = Act();
   text_kv_ = nullptr;

@@ -30,7 +30,7 @@ SYMBOLS = [
     "i2it_set_adapter_scale", "i2it_finalize_weights", "i2it_workspace_bytes", "i2it_forward",
     "i2it_set_text", "i2it_encode_text", "i2it_forward_u8", "i2it_prep_launch_count", "i2it_debug_fast_div", "i2it_launch_count", "i2it_profile", "i2it_read_stage", "i2it_op_conv2d", "i2it_op_group_norm", "i2it_op_layer_norm",
     "i2it_op_attention", "i2it_op_upsample2x", "i2it_op_conv2d_ex", "i2it_op_launches", "i2it_op_vt_proj",
-    "i2it_op_upsample_to",
+    "i2it_op_upsample_to", "i2it_stage_names", "i2it_prepared_keys", "i2it_read_prepared",
 ]
 
 
@@ -102,6 +102,9 @@ def load_library(path: Optional[str] = None):
     lib.i2it_op_vt_proj.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, ci, vp, vp]
     lib.i2it_op_upsample2x.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp]
     lib.i2it_op_upsample_to.argtypes = [vp, vp, ci, ci, ci, ci, ci, ci, vp, vp]
+    lib.i2it_stage_names.argtypes = [vp, C.c_char_p, C.c_size_t]
+    lib.i2it_prepared_keys.argtypes = [vp, C.c_char_p, C.c_size_t]
+    lib.i2it_read_prepared.argtypes = [vp, C.c_char_p, vp, C.c_size_t, vp, C.c_size_t, C.POINTER(ci)]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("i2it_destroy", "i2it_last_error"):
@@ -122,7 +125,7 @@ class Engine:
     """One engine per (device, stream).  Thin, typed wrapper over the C handle."""
 
     def __init__(self, dtype: torch.dtype = torch.bfloat16, model_kind: int = PIX2PIX, cfg: Optional[dict] = None,
-                 device: Optional[int] = None, keep_stages: bool = False, use_cuda_graph: bool = True,
+                 device: Optional[int] = None, keep_stages: int = 0, use_cuda_graph: bool = True,
                  text_heads: int = 0, text_act: str = "gelu"):
         if not torch.cuda.is_available():
             raise RuntimeError("libi2it needs a CUDA device (H100 / sm_90a); no CPU fallback exists")
@@ -133,7 +136,7 @@ class Engine:
         c.dtype = _TORCH2DT[dtype]
         c.model_kind = model_kind
         c.device = torch.cuda.current_device() if device is None else device
-        c.keep_stages = int(keep_stages)
+        c.keep_stages = int(keep_stages)                     # 1: named checkpoints, 2: every layer output
         c.use_cuda_graph = int(use_cuda_graph)
         c.text_heads = int(text_heads)                       # 0: hidden / 64
         c.text_act = 1 if text_act == "quick_gelu" else 0
@@ -282,6 +285,31 @@ class Engine:
         self._check(self.lib.i2it_read_stage(self._h, name.encode(), _ptr(buf), max_elems, dims), f"i2it_read_stage({name})")
         n, c, h, w = list(dims)
         return buf[: n * c * h * w].view(n, c, h, w).clone()
+
+    def _json(self, fn, what, cap=1 << 22):
+        import json
+        buf = C.create_string_buffer(cap)
+        self._check(fn(self._h, buf, cap), what)
+        return json.loads(buf.value.decode())
+
+    def stage_names(self):
+        """[(name, (N, C, H, W))] of every stage the last forward kept, in build order."""
+        return [(s["name"], tuple(s["dims"])) for s in self._json(self.lib.i2it_stage_names, "i2it_stage_names")]
+
+    def prepared_keys(self):
+        """Cache keys of every prepared weight (plain layer names, "+sc", ".qk", "|twin", "|im2col", "|subpixel", "identity|n")."""
+        return self._json(self.lib.i2it_prepared_keys, "i2it_prepared_keys")
+
+    def read_prepared(self, key: str):
+        """A prepared weight as the kernels read it: ([taps, rows, cin_pad] in the engine dtype, fp32 bias [rows] or None)."""
+        dims = (C.c_int * 4)()
+        self._check(self.lib.i2it_read_prepared(self._h, key.encode(), None, 0, None, 0, dims), f"i2it_read_prepared({key})")
+        taps, rows, cin_pad, has_bias = list(dims)
+        w = torch.empty(taps, rows, cin_pad, device="cuda", dtype=self.dtype)
+        b = torch.empty(rows, device="cuda", dtype=torch.float32) if has_bias else None
+        self._check(self.lib.i2it_read_prepared(self._h, key.encode(), _ptr(w), w.numel(), _ptr(b), rows if has_bias else 0, dims),
+                    f"i2it_read_prepared({key})")
+        return w, b
 
     # ---- diagnostic single ops (NHWC tensors in the engine dtype; weights fp32 CUDA) -----------------
     def op_conv2d(self, x_nhwc, w, bias=None, stride=1, asym_pad=False, residual=None, act=ACT_NONE, out_fp32=False):

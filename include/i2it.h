@@ -50,7 +50,8 @@ typedef struct i2it_config {
   int temb_dim;              /* 1280                                                                       */
   int vae_channels[4];       /* 128, 256, 512, 512                                                         */
   float scaling_factor;      /* 0.18215                                                                    */
-  int keep_stages;           /* 1: keep named intermediate tensors readable via i2it_read_stage (tests)    */
+  int keep_stages;           /* 1: keep named intermediate tensors readable via i2it_read_stage (tests);   */
+                             /* 2: also every layer output (per-layer audit; needs memory for all of them) */
   int use_cuda_graph;        /* 1: replay the forward as one CUDA graph when shapes and pointers repeat    */
   int text_heads;            /* CLIP text tower: attention heads (16; head_dim must be 64); 0 = hidden/64  */
   int text_act;              /* CLIP text tower MLP activation: 0 = gelu (SD-Turbo), 1 = quick_gelu        */
@@ -154,6 +155,19 @@ int i2it_profile(i2it_handle* h, int reps, char* json, size_t cap, void* stream)
  * into dst (device pointer) and reports its dims.  Synchronous.  Names: "skip0".."skip3", "moments",
  * "latent", "model_pred", "dec_in", "pre_out"... (see DESIGN.md). */
 int i2it_read_stage(i2it_handle* h, const char* name, float* dst, size_t dst_elems, int dims[4]);
+
+/* Every stage of the LAST forward in build order, as JSON [{"name","dims":[N,C,H,W]}...].  With cfg.keep_stages = 2
+ * the forward also keeps every layer output under its state-dict prefix ("unet.down_blocks.0.resnets.0.conv1", ...;
+ * DESIGN.md section 6 lists the names); the output image is bit-identical to keep_stages = 0.  Synchronous. */
+int i2it_stage_names(i2it_handle* h, char* json, size_t cap);
+
+/* Cache keys of every prepared (folded, re-laid-out) weight, as a sorted JSON array of strings.  Synchronous. */
+int i2it_prepared_keys(i2it_handle* h, char* json, size_t cap);
+
+/* Copies the prepared weight `key` exactly as the kernels read it: w = [taps][rows][cin_pad] 16-bit elements of the
+ * handle dtype, bias = [rows] fp32 (when the weight has one).  dims = {taps, rows, cin_pad, has_bias}.  w / bias may be
+ * NULL to query dims only; host or device pointers.  Synchronous. */
+int i2it_read_prepared(i2it_handle* h, const char* key, void* w, size_t w_elems, float* bias, size_t b_elems, int dims[4]);
 
 /* ---- diagnostic single-op entry points (used by tests/ to check each kernel against the oracle) ----
  * Activations NHWC with pixel stride ld (elements); weights fp32 device pointers in PyTorch layout.
