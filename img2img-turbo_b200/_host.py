@@ -240,16 +240,20 @@ class TurboBase(torch.nn.Module):
     # ---- text ----------------------------------------------------------------------------------------
     def _text_encoder_spec(self):
         """{"heads", "act", "hidden"} if the text encoder is a CLIP text tower libi2it can run (64-wide heads, gelu / quick_gelu,
-        width <= 1280), else None (the stock transformers module is called instead)."""
+        width <= 1280, 77 positions, LayerNorm eps 1e-5 as the engine's layernorm launches use), else None (the stock
+        transformers module is called instead)."""
         enc = self.text_encoder
         c = getattr(enc, "config", None)
         if enc is None or c is None or os.environ.get("I2IT_TORCH_TEXT"):
             return None
         try:
             hidden, heads, act = int(c.hidden_size), int(c.num_attention_heads), str(c.hidden_act)
+            ln_eps = float(c.layer_norm_eps)
         except Exception:
             return None
         if heads * 64 != hidden or hidden > 1280 or act not in ("gelu", "quick_gelu") or int(c.max_position_embeddings) != 77:
+            return None
+        if ln_eps != 1e-5:
             return None
         return {"heads": heads, "act": act, "hidden": hidden}
 

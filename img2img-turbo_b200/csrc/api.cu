@@ -195,6 +195,12 @@ int i2it_stage_names(i2it_handle* h, char* json, size_t cap) {
   API_END
 }
 
+int i2it_text_stage_names(i2it_handle* h, char* json, size_t cap) {
+  API_BEGIN(h)
+  copy_json(E.stage_names_json(/*text=*/true), json, cap, "i2it_text_stage_names");
+  API_END
+}
+
 int i2it_prepared_keys(i2it_handle* h, char* json, size_t cap) {
   API_BEGIN(h)
   copy_json(E.prepared_keys_json(), json, cap, "i2it_prepared_keys");

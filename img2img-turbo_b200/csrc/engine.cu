@@ -232,6 +232,7 @@ void Engine::finalize(float lw_unet, float lw_vae, float skip_gamma, float twin_
   textkv_.clear();                 // cached cross-attention operands were projected with the old (LoRA-scaled) weights
   textenc_.clear();
   last_plan_ = nullptr;
+  last_text_plan_ = nullptr;
   free_prepared();
   finalized_ = true;
 }
@@ -1359,17 +1360,27 @@ void Engine::encode_text(const int* tokens, int batch, void* out, cudaStream_t s
                            reinterpret_cast<const int*>(plan->io.x), tp, pp, reinterpret_cast<T*>(xp), C, ntok, vocab, total)));
       }, "clip_embed", 0, 2.0 * total * 8 * 3);
     }
+    // keep_stages >= 2: every layer output under its transformers state-dict prefix (tests/text_audit.py); no launches added
+    mark_layer(P, te + ".embeddings", x);
     for (int l = 0; l < layers; ++l) {
       const std::string L = te + ".encoder.layers." + std::to_string(l);
       Act n = layer_norm(P, x, norm(L + ".layer_norm1"));
+      mark_layer(P, L + ".layer_norm1", n);
       Act qk = linear(P, n, prep(L + ".qk", {L + ".self_attn.q_proj", L + ".self_attn.k_proj"}));
+      mark_layer(P, L + ".self_attn.qk", qk);
       Act vt = vt_proj(P, n, batch, ntok, prep(L + ".self_attn.v_proj", {L + ".self_attn.v_proj"}));
+      mark_layer(P, L + ".self_attn.v_proj", vt);
       Act a = flash_attention(P, qk.slice(0, C), qk.slice(C, C), vt, batch, ntok, ntok, heads, batch, /*causal=*/true);
       a.N = batch; a.H = 1; a.W = ntok;
+      mark_layer(P, L + ".self_attn", a);
       x = linear(P, a, prep(L + ".self_attn.out_proj", {L + ".self_attn.out_proj"}), &x);
+      mark_layer(P, L + ".self_attn.out_proj", x);
       Act m = layer_norm(P, x, norm(L + ".layer_norm2"));
+      mark_layer(P, L + ".layer_norm2", m);
       Act h = linear(P, m, prep(L + ".mlp.fc1", {L + ".mlp.fc1"}), nullptr, act);
+      mark_layer(P, L + ".mlp.fc1", h);
       x = linear(P, h, prep(L + ".mlp.fc2", {L + ".mlp.fc2"}), &x);
+      mark_layer(P, L + ".mlp.fc2", x);
     }
     layer_norm(P, x, norm(te + ".final_layer_norm"), /*to_io_out=*/true);
     P.keep.push_back(x.hold);
@@ -1379,6 +1390,7 @@ void Engine::encode_text(const int* tokens, int batch, void* out, cudaStream_t s
   Plan& P = *slot;
   P.io.x = tokens;
   P.io.out = out;
+  last_text_plan_ = &P;
   nvtxRangePushA("i2it:clip_text_encoder");
   g_pdl.enabled = false; g_pdl.prev_is_kernel = false;
   for (auto& op : P.ops) op(st);
@@ -1516,14 +1528,17 @@ __global__ void stage_to_nchw_f32_kernel(const uint16_t* x, int ld, int C, long 
 }
 
 void Engine::read_stage(const std::string& name_in, float* dst, size_t dst_elems, int dims[4]) {
-  I2IT_CHECK(last_plan_ != nullptr, "no forward has run yet");
+  // "text_encoder.*" names are stages of the last encode_text, every other name one of the last forward
+  const bool text = name_in.rfind("text_encoder.", 0) == 0;
+  const Plan* plan = text ? last_text_plan_ : last_plan_;
+  I2IT_CHECK(plan != nullptr, text ? "no encode_text has run yet" : "no forward has run yet");
   // "name@i" selects image i of the stage (large-batch stages do not fit a test's scratch buffer)
   std::string name = name_in;
   int pick = -1;
   const size_t at = name.find('@');
   if (at != std::string::npos) { pick = atoi(name.c_str() + at + 1); name = name.substr(0, at); }
-  auto it = last_plan_->stages.find(name);
-  I2IT_CHECK(it != last_plan_->stages.end(), "unknown stage '" + name + "' (was keep_stages set?)");
+  auto it = plan->stages.find(name);
+  I2IT_CHECK(it != plan->stages.end(), "unknown stage '" + name + "' (was keep_stages set?)");
   const Act& a = it->second;
   I2IT_CHECK(pick < a.N, "read_stage: image index out of range");
   const int n = pick >= 0 ? 1 : a.N;
@@ -1536,12 +1551,13 @@ void Engine::read_stage(const std::string& name_in, float* dst, size_t dst_elems
   I2IT_CUDA(cudaDeviceSynchronize());
 }
 
-std::string Engine::stage_names_json() const {
-  I2IT_CHECK(last_plan_ != nullptr, "no forward has run yet");
+std::string Engine::stage_names_json(bool text) const {
+  const Plan* plan = text ? last_text_plan_ : last_plan_;
+  I2IT_CHECK(plan != nullptr, text ? "no encode_text has run yet" : "no forward has run yet");
   std::string js = "[";
-  for (size_t i = 0; i < last_plan_->stage_order.size(); ++i) {
-    const std::string& n = last_plan_->stage_order[i];
-    const Act& a = last_plan_->stages.at(n);
+  for (size_t i = 0; i < plan->stage_order.size(); ++i) {
+    const std::string& n = plan->stage_order[i];
+    const Act& a = plan->stages.at(n);
     js += std::string(i ? "," : "") + "{\"name\":\"" + n + "\",\"dims\":[" + std::to_string(a.N) + "," + std::to_string(a.C) + "," +
           std::to_string(a.H) + "," + std::to_string(a.W) + "]}";
   }

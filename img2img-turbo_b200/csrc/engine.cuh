@@ -182,7 +182,7 @@ class Engine {
   bool has_text_encoder() const { return has("text_encoder.text_model.embeddings.token_embedding.weight"); }
   Plan* last_plan() const { return last_plan_; }
   void read_stage(const std::string& name, float* dst, size_t dst_elems, int dims[4]);
-  std::string stage_names_json() const;                              // last forward's stages, build order, with dims
+  std::string stage_names_json(bool text = false) const;             // last forward's (text: last encode_text's) stages
   std::string prepared_keys_json() const;                            // every prepared-weight cache key, sorted
   // a prepared weight exactly as the kernels read it: [taps][rows][cin_pad] 16-bit + fp32 bias; dims = taps, rows, cin_pad, has_bias
   void read_prepared(const std::string& key, void* w, size_t w_elems, float* bias, size_t b_elems, int dims[4]);
@@ -289,6 +289,7 @@ class Engine {
   std::map<int, std::unique_ptr<Plan>> textenc_;            // CLIP text tower plans, by batch
   std::map<std::vector<int>, std::unique_ptr<Plan>> plans_;
   Plan* last_plan_ = nullptr;
+  Plan* last_text_plan_ = nullptr;   // the plan of the last encode_text (its stages: i2it_text_stage_names)
   Act text_;                     // staged text embedding while a UNet plan is being built
   TextKV* text_kv_ = nullptr;    // ... or the cached cross-attention operands (text_emb == NULL forwards)
 

@@ -30,8 +30,22 @@ SYMBOLS = [
     "i2it_set_adapter_scale", "i2it_finalize_weights", "i2it_workspace_bytes", "i2it_forward",
     "i2it_set_text", "i2it_encode_text", "i2it_forward_u8", "i2it_prep_launch_count", "i2it_debug_fast_div", "i2it_launch_count", "i2it_profile", "i2it_read_stage", "i2it_op_conv2d", "i2it_op_group_norm", "i2it_op_layer_norm",
     "i2it_op_attention", "i2it_op_upsample2x", "i2it_op_conv2d_ex", "i2it_op_launches", "i2it_op_vt_proj",
-    "i2it_op_upsample_to", "i2it_stage_names", "i2it_prepared_keys", "i2it_read_prepared",
+    "i2it_op_upsample_to", "i2it_stage_names", "i2it_prepared_keys", "i2it_read_prepared", "i2it_text_stage_names",
 ]
+TEXT_TOKEN_EMB = "text_encoder.text_model.embeddings.token_embedding.weight"
+TEXT_POS_EMB = "text_encoder.text_model.embeddings.position_embedding.weight"
+
+
+def check_tokens(tokens: torch.Tensor, vocab: int, ntok: int):
+    """Raise ValueError unless `tokens` is [B, ntok] with every id in [0, vocab).  The text tower reads B * ntok ids and
+    writes B * ntok rows whatever the tensor's shape, and its embedding kernel clamps ids: both checks must come first."""
+    if tokens.dim() != 2 or tokens.shape[0] < 1 or tokens.shape[1] != ntok:
+        raise ValueError(f"text tokens must be [B, {ntok}] (the position table's length), got {list(tokens.shape)}")
+    if tokens.dtype.is_floating_point or tokens.dtype.is_complex or tokens.dtype == torch.bool:
+        raise ValueError(f"text tokens must be integer ids, got {tokens.dtype}")
+    lo, hi = int(tokens.min()), int(tokens.max())
+    if lo < 0 or hi >= vocab:
+        raise ValueError(f"token ids must lie in [0, {vocab}), got ids from {lo} to {hi}")
 
 
 class ConvDesc(C.Structure):
@@ -103,6 +117,7 @@ def load_library(path: Optional[str] = None):
     lib.i2it_op_upsample2x.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp]
     lib.i2it_op_upsample_to.argtypes = [vp, vp, ci, ci, ci, ci, ci, ci, vp, vp]
     lib.i2it_stage_names.argtypes = [vp, C.c_char_p, C.c_size_t]
+    lib.i2it_text_stage_names.argtypes = [vp, C.c_char_p, C.c_size_t]
     lib.i2it_prepared_keys.argtypes = [vp, C.c_char_p, C.c_size_t]
     lib.i2it_read_prepared.argtypes = [vp, C.c_char_p, vp, C.c_size_t, vp, C.c_size_t, C.POINTER(ci)]
     for name in SYMBOLS:
@@ -180,6 +195,10 @@ class Engine:
             shape = (C.c_int64 * t.dim())(*t.shape)
             self._check(self.lib.i2it_set_weight(self._h, k.encode(), _ptr(t), shape, t.dim(), _TORCH2DT[t.dtype],
                                                  int(t.is_cuda)), f"i2it_set_weight({k})")
+            if k == TEXT_TOKEN_EMB:              # encode_text checks token ids and the output width against these
+                self._text_vocab, self._text_hidden = int(t.shape[0]), int(t.shape[1])
+            elif k == TEXT_POS_EMB:
+                self._text_ntok = int(t.shape[0])
 
     def set_adapter_scale(self, adapter: str, alpha_over_r: float):
         self._check(self.lib.i2it_set_adapter_scale(self._h, adapter.encode(), alpha_over_r), "i2it_set_adapter_scale")
@@ -202,7 +221,14 @@ class Engine:
 
     def encode_text(self, tokens: torch.Tensor, hidden: int) -> torch.Tensor:
         """CLIP text tower on the engine: tokens [B,77] (any integer dtype) -> last_hidden_state [B,77,hidden] in the engine dtype.
-        Needs the `text_encoder.*` tensors in the loaded state dict."""
+        Needs the `text_encoder.*` tensors in the loaded state dict.  Raises ValueError, before any launch, unless tokens is
+        [B, position-table length] with ids in [0, vocab) and `hidden` is the tower's width."""
+        vocab, ntok = getattr(self, "_text_vocab", None), getattr(self, "_text_ntok", None)
+        if vocab is None or ntok is None:
+            raise ValueError("encode_text needs the text_encoder.* tensors (load_state_dict) first")
+        check_tokens(tokens, vocab, ntok)
+        if hidden != self._text_hidden:
+            raise ValueError(f"hidden must be the text tower's width {self._text_hidden}, got {hidden}")
         ids = tokens.to(device="cuda", dtype=torch.int32).contiguous()
         out = torch.empty(ids.shape[0], ids.shape[1], hidden, device="cuda", dtype=self.dtype)
         self._check(self.lib.i2it_encode_text(self._h, _ptr(ids), ids.shape[0], _ptr(out), _stream()), "i2it_encode_text")
@@ -295,6 +321,10 @@ class Engine:
     def stage_names(self):
         """[(name, (N, C, H, W))] of every stage the last forward kept, in build order."""
         return [(s["name"], tuple(s["dims"])) for s in self._json(self.lib.i2it_stage_names, "i2it_stage_names")]
+
+    def text_stage_names(self):
+        """[(name, (N, C, H, W))] of every stage the last encode_text kept, in build order (read them with read_stage)."""
+        return [(s["name"], tuple(s["dims"])) for s in self._json(self.lib.i2it_text_stage_names, "i2it_text_stage_names")]
 
     def prepared_keys(self):
         """Cache keys of every prepared weight (plain layer names, "+sc", ".qk", "|twin", "|im2col", "|subpixel", "identity|n")."""

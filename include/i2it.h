@@ -122,7 +122,9 @@ int i2it_set_text(i2it_handle* h, const void* text_emb, int text_batch, void* st
 /* The CLIP text tower on the engine (SURVEY.md section 8f #1): tokens [batch, 77] int32 (device) -> last_hidden_state
  * [batch, 77, hidden] (device, handle dtype), i.e. `self.text_encoder(tokens)[0]` of src/pix2pix_turbo.py:190-196
  * and cyclegan_turbo.py:251-253.  Needs the "text_encoder.<transformers CLIPTextModel key>" tensors registered with
- * i2it_set_weight.  Enqueued on `stream` (no CUDA graph: a prompt is encoded once and cached by the caller). */
+ * i2it_set_weight.  Enqueued on `stream` (no CUDA graph: a prompt is encoded once and cached by the caller).
+ * The kernels read batch * 77 ids and write batch * 77 rows: the caller owns both sizes, and every id must lie in
+ * [0, vocab) (the Python binding checks both before the launch). */
 int i2it_encode_text(i2it_handle* h, const int32_t* tokens, int batch, void* out, void* stream);
 
 /* i2it_forward with a uint8 HWC boundary: x_u8_hwc [batch, H, W, 3] and out_u8_hwc [batch, H, W, 3] are device pointers.
@@ -160,6 +162,12 @@ int i2it_read_stage(i2it_handle* h, const char* name, float* dst, size_t dst_ele
  * the forward also keeps every layer output under its state-dict prefix ("unet.down_blocks.0.resnets.0.conv1", ...;
  * DESIGN.md section 6 lists the names); the output image is bit-identical to keep_stages = 0.  Synchronous. */
 int i2it_stage_names(i2it_handle* h, char* json, size_t cap);
+
+/* Every stage of the LAST i2it_encode_text, in the format of i2it_stage_names.  With cfg.keep_stages = 2 the text tower
+ * keeps every layer output under its transformers state-dict prefix ("text_encoder.text_model.embeddings",
+ * "text_encoder.text_model.encoder.layers.0.self_attn.qk", ...; DESIGN.md section 6); i2it_read_stage reads a
+ * "text_encoder."-prefixed name from this plan.  The encoded output is bit-identical to keep_stages = 0.  Synchronous. */
+int i2it_text_stage_names(i2it_handle* h, char* json, size_t cap);
 
 /* Cache keys of every prepared (folded, re-laid-out) weight, as a sorted JSON array of strings.  Synchronous. */
 int i2it_prepared_keys(i2it_handle* h, char* json, size_t cap);

@@ -17,8 +17,8 @@ import math
 import torch
 import torch.nn.functional as F
 
-_MANT = {torch.bfloat16: 7, torch.float16: 10, torch.float32: 23}
-_EMIN = {torch.bfloat16: -126, torch.float16: -14, torch.float32: -126}
+_MANT = {torch.bfloat16: 7, torch.float16: 10, torch.float32: 23, torch.float64: 52}      # float64: rounding switched off
+_EMIN = {torch.bfloat16: -126, torch.float16: -14, torch.float32: -126, torch.float64: -1022}
 EPS24 = 2.0 ** -24                       # fp32 unit roundoff
 MEAN_ULP_MAX = 0.30
 # Norm statistics: sums of x and x^2 run in fp32 chains before the double finalisation, so var = E[x^2] - mean^2 carries

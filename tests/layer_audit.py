@@ -116,7 +116,7 @@ class Audit:
             v = ref_nchw if exact else kref.round16(ref_nchw, self.dt)
             if self.stage_hook:
                 v = self.stage_hook(name, v, self)
-            self.src.stages[name] = v.float()
+            self.src.stages[name] = v if self.dt == torch.float64 else v.float()     # float64: no rounding anywhere
             self.src.order.append(name)
             return
         got = self.src.read_stage(name).to(self.dev).double()
@@ -167,8 +167,8 @@ class Audit:
         ref, bound = ref.permute(0, 3, 1, 2), bound.permute(0, 3, 1, 2)
         self.emit("groupnorm", name, ref, lambda got: kref.check_norm(name, got, ref, bound, self.dt))
 
-    def layer_norm(self, name, x, norm):
-        ref, bound = kref.layer_norm64(x, self.P(norm + ".weight"), self.P(norm + ".bias"), 1e-5, self.dt)
+    def layer_norm(self, name, x, norm, eps=1e-5):
+        ref, bound = kref.layer_norm64(x, self.P(norm + ".weight"), self.P(norm + ".bias"), eps, self.dt)
         ref, bound = ref.permute(0, 3, 1, 2), bound.permute(0, 3, 1, 2)
         self.emit("layernorm", name, ref, lambda got: kref.check_norm(name, got, ref, bound, self.dt))
 
@@ -184,9 +184,9 @@ class Audit:
     def read_v(self, name, ntok):
         return self.S(name)[:, 0, :, :ntok].transpose(1, 2)            # NHWC [B, 1, C, ldv] -> V [B, ntok, C]
 
-    def attention(self, name, q, k, v, heads, H, W):
+    def attention(self, name, q, k, v, heads, H, W, causal=False):
         """q [B, Nq, C], k / v [kvB, Nk, C] (the engine's own operands) -> stage [B, C, H, W]."""
-        o, pav, e_s = kref.attention64(q, k, v, heads)
+        o, pav, e_s = kref.attention64(q, k, v, heads, causal=causal)
         B, C = q.shape[0], q.shape[2]
         sp = lambda t: t.reshape(B, H, W, C).permute(0, 3, 1, 2)
         ref, pav, e_s = sp(o), sp(pav), sp(e_s)
@@ -580,9 +580,13 @@ class Audit:
         return c
 
     # ------------------------------------------------------------------------------------------------ driver
+    def audited_keys(self, keys):
+        """The prepared keys this audit owns: the forward's (the CLIP text tower's are tests/text_audit.py's)."""
+        return [k for k in keys if not k.startswith("text_encoder.")]
+
     def run(self, require_complete=True):
         self.walk()
-        keys = sorted(self.used_keys) if self.emulate else self.src.prepared_keys()
+        keys = sorted(self.used_keys) if self.emulate else self.audited_keys(self.src.prepared_keys())
         for k in keys:
             self.keys_seen.append(k)
             if not self.emulate:
