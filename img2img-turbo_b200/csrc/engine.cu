@@ -104,6 +104,23 @@ __global__ void cvt16_to_f32_kernel(const uint16_t* s, float* d, long long n, in
 
 thread_local PdlState g_pdl;
 
+// tapgemm instantiations: the MMA of a k16 step is one wgmma of the tile's full width, so BN is a template parameter.  The
+// LEAN variant only runs TMA-store launches (whole 64-column rounds); the full variant takes every BN pick_bn can choose.
+// Callers that set BN themselves must use one of these widths: attn_pv's BN = min(head dim, 256) covers head dims 16, 32, ..., 160,
+// 192, 224 and >= 256 (the model's are 64 and 512); 176, 208 and 240 are refused at plan time.
+#define TG_BN_LEAN(X) X(64) X(128) X(192) X(256)
+#define TG_BN_FULL(X) X(16) X(32) X(48) X(64) X(80) X(96) X(112) X(128) X(160) X(192) X(224) X(256)
+template <typename T> using TgKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TapGemmParams);
+template <typename T> static TgKernel<T> tapgemm_for(bool lean, int bn) {   // nullptr: no such instantiation
+#define TG_CASE_LEAN(n) if (lean && bn == n) return tapgemm_kernel<T, true, n>;
+#define TG_CASE_FULL(n) if (!lean && bn == n) return tapgemm_kernel<T, false, n>;
+  TG_BN_LEAN(TG_CASE_LEAN)
+  TG_BN_FULL(TG_CASE_FULL)
+#undef TG_CASE_LEAN
+#undef TG_CASE_FULL
+  return nullptr;
+}
+
 Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CHECK(c.dtype == DT_F16 || c.dtype == DT_BF16, "dtype must be I2IT_F16 or I2IT_BF16");
   I2IT_CUDA(cudaSetDevice(c.device));
@@ -112,10 +129,12 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CHECK(prop.major == 9 && prop.minor == 0, "libi2it is built for sm_90a (H100) only; found compute capability " +
                                                   std::to_string(prop.major) + "." + std::to_string(prop.minor));
   num_sms = prop.multiProcessorCount;
-  I2IT_CUDA(cudaFuncSetAttribute(tapgemm_kernel<__half, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
-  I2IT_CUDA(cudaFuncSetAttribute(tapgemm_kernel<__half, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
-  I2IT_CUDA(cudaFuncSetAttribute(tapgemm_kernel<__nv_bfloat16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
-  I2IT_CUDA(cudaFuncSetAttribute(tapgemm_kernel<__nv_bfloat16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
+  for (int lean = 0; lean < 2; ++lean)
+    for (int bn = 16; bn <= 256; bn += 16) {
+      if (auto k = tapgemm_for<__half>(lean, bn)) I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
+      if (auto k = tapgemm_for<__nv_bfloat16>(lean, bn))
+        I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
+    }
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn512_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA5_SMEM));
@@ -531,7 +550,7 @@ Act Engine::alloc_act(Plan& P, int N, int H, int W, int C, int ld, bool zero_per
 
 int Engine::pick_bn(long long m_tiles, int N, int step) const {
   if (N <= 16) return 16;
-  static const int cand_any[] = {256, 224, 192, 160, 128, 112, 96, 80, 64, 48, 32, 16};
+  static const int cand_any[] = {256, 224, 192, 160, 128, 112, 96, 80, 64, 48, 32, 16};   // = TG_BN_FULL
   static const int cand_64[] = {256, 192, 128, 64};
   static const int cand_128[] = {256, 128};
   const int* cand = step == 128 ? cand_128 : (step == 64 ? cand_64 : cand_any);
@@ -639,11 +658,11 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
     while ((1 << p.gn_shift) < p.gn_red) ++p.gn_shift;
   }
   const bool lean = use_lean && p.tma_out && p.act == TG_ACT_NONE;      // the epilogue variant without activation / direct-store code
+  I2IT_CHECK(tapgemm_for<__half>(lean, p.BN) != nullptr, "tapgemm: no kernel instantiated for BN=" + std::to_string(p.BN));
   add_op(P, [ta, tb, ta2, tb2, to, p, grid, dt, out_from_io, plan, lean](cudaStream_t st) {
     TapGemmParams q = p;
     if (out_from_io) q.out = plan->io.out;
-    if (lean) { DISPATCH_T(dt, (launch_k(tapgemm_kernel<T, true>, dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q))); }
-    else { DISPATCH_T(dt, (launch_k(tapgemm_kernel<T, false>, dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q))); }
+    DISPATCH_T(dt, (launch_k(tapgemm_for<T>(lean, q.BN), dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q)));
   }, kind, 2.0 * m_valid * p.N * k_valid, bytes, shp);
 }
 

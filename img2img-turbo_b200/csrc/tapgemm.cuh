@@ -10,15 +10,18 @@
 // sm_90a structure (one persistent CTA per SM, 384 threads):
 //   warp 8        : TMA producer   cp.async.bulk.tensor.5d -> 128B-swizzled smem ring (4 stages at BN = 256)
 //   warps 0..7    : two consumer warpgroups; warpgroup g owns tile rows [64g, 64g+64):
-//                   mainloop  wgmma.mma_async m64nNk16 (N = 64 blocks, or 16 blocks when BN is not a multiple of 64),
-//                             fp32 accumulators in registers
-//                   epilogue  accumulators -> fp32 staging tile in smem (aliases the operand ring) -> one accumulator ROW per
-//                             thread -> bias/residual/GEGLU/clamp -> TMA store boxes or direct stores
-//   mbarriers     : full/empty per smem stage; epi_done holds the producer off the ring while it is the staging tile
+//                   mainloop  one wgmma.mma_async m64nBNk16 per k16 step (BN is a template parameter, so the chain has
+//                             no run-time predicates), fp32 accumulators in registers, defined anew by each tile's first MMA
+//                   epilogue  TMA-store launches: from the wgmma fragments -> bias/residual/GEGLU/clamp -> swizzled store boxes
+//                             -> TMA stores (the ring is not touched, so the producer loads the next tile meanwhile);
+//                             direct-store launches: fp32 staging tile in smem (aliases the operand ring) -> one accumulator ROW
+//                             per thread -> per-thread stores
+//   mbarriers     : full/empty per smem stage; epi_done holds the producer off the ring while it is a staging tile
 //
 // Replaces every nn.Conv2d / nn.Linear / SDPA matmul under vae.encode / unet(...) / vae.decode of the reference
 // pipeline, which dispatch to cuDNN implicit GEMM, cuBLAS and flash/mem-efficient SDPA in the reference stack.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 
 namespace i2it {
@@ -35,11 +38,11 @@ constexpr int TG_EPI_GROUPS = TG_EPI_WARPS / 4;  // warps per 32-row quarter: th
 constexpr int TG_EPI_RPW = 8 / TG_EPI_GROUPS;    // rounds per warp at BN = 256
 constexpr int TG_BAR_BYTES = 512;
 constexpr int TG_BIAS_BYTES = 2 * 256 * 4;       // per-tile bias slice, double-buffered across tiles
-// Epilogue store staging: each epilogue warp owns ONE TMA box = 32 rows x 64 output columns (128-byte rows, SWIZZLE_128B: the
-// 16-byte chunk c of row r lives at r*128 + ((c ^ (r & 7)) << 4)).  A thread holds one accumulator ROW, so direct stores touch 32
-// different lines per instruction.  Through the box the thread writes its row with conflict-free st.shared.v4 and ONE elected
-// lane hands the 4 KB box to the TMA unit, which writes full lines and clips ragged edges.  The residual takes the same road in
-// reverse: coalesced 16-byte global loads (4 rows x 128 B per instruction), transposed through the box, added in place.
+// Epilogue store boxes: each epilogue warp owns ONE TMA box = 32 rows x 64 output columns (128-byte rows, SWIZZLE_128B: the
+// 16-byte chunk c of row r lives at r*128 + ((c ^ (r & 7)) << 4)).  The two warps that hold a 32-row quarter's fragments write
+// their column pairs into it with conflict-free 32-bit st.shared and ONE lane hands the 4 KB box to the TMA unit, which writes
+// full lines and clips ragged edges.  The residual takes the same road in reverse: coalesced 16-byte global loads (4 rows x
+// 128 B per instruction) into the box, added in place.
 constexpr int TG_OSTG_WARP = 32 * 128;
 constexpr int TG_OSTG_BYTES = TG_EPI_WARPS * TG_OSTG_WARP;
 // manual 1024-byte alignment slack of the dynamic smem base: 512 B are budgeted (a full 1 KB would put the CTA over the
@@ -47,7 +50,9 @@ constexpr int TG_OSTG_BYTES = TG_EPI_WARPS * TG_OSTG_WARP;
 constexpr int TG_ALIGN_PAD = 512;
 constexpr int TG_SMEM = TG_STAGES * (TG_A_STAGE + TG_B_STAGE) + TG_BAR_BYTES + TG_BIAS_BYTES + TG_OSTG_BYTES + TG_ALIGN_PAD;
 // + one producer warpgroup (warp 8 issues the TMA loads, warps 9..11 idle).  Registers are allocated per warpgroup, so the
-// producer warpgroup gives its registers to the consumers (setmaxnreg): 128 x 40 + 256 x 232 <= 64 K.
+// producer warpgroup gives its registers to the consumers (setmaxnreg): 128 x 40 + 256 x 232 <= 64 K.  ptxas honours the
+// two setmaxnreg with each inside its own role's branch (see the role split in tapgemm_kernel).  The kernel is still register-
+// allocated within the launch's 168 per thread: ptxas needs the launch bound to honour setmaxnreg (without it: C7508).
 constexpr int TG_THREADS = (TG_EPI_WARPS + 4) * 32;
 constexpr int TG_REGS_PRODUCER = 40, TG_REGS_CONSUMER = 232;
 // fp32 accumulator staging: 128 rows x (BN + 4) floats.  BN is a multiple of 16, so the row pitch is 4 mod 8 words and eight
@@ -188,37 +193,89 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
-// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in 128B-swizzled smem; acc == 0 overwrites D.
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T for the tile's whole width N (BN) in one instruction, both operands K-major in
+// 128B-swizzled smem.  ACC = false is the first k16 step of a tile: scale-d = 0 and output-only operands, so D is overwritten
+// (an exact -0 sum stays -0) and the accumulators carry nothing from the previous tile.
 // Fragment of D: register 4*g + e of thread (warp w, lane l) is row 16w + l/4 + 8*(e >> 1), column 8g + 2*(l % 4) + (e & 1).
-template <int N, typename T> __device__ __forceinline__ void wgmma_ss(float* d, uint64_t a, uint64_t b, uint32_t acc);
-template <> __device__ __forceinline__ void wgmma_ss<64, __half>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b), "r"(acc));
+#define TG_D4(C, i) C(d[i]), C(d[i + 1]), C(d[i + 2]), C(d[i + 3])
+#define TG_D8(C, i) TG_D4(C, i), TG_D4(C, i + 4)
+#define TG_D32(C, i) TG_D8(C, i), TG_D8(C, i + 8), TG_D8(C, i + 16), TG_D8(C, i + 24)
+#define TG_WGMMA_N16(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n16k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D8(C, 0) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N32(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D8(C, 0), TG_D8(C, 8) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N48(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n48k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D8(C, 0), TG_D8(C, 8), TG_D8(C, 16) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N64(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D32(C, 0) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N80(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n80k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, %40, %41, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D32(C, 0), TG_D8(C, 32) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N96(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n96k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, %48, %49, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D32(C, 0), TG_D8(C, 32), TG_D8(C, 40) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N112(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n112k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55}, %56, %57, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D32(C, 0), TG_D8(C, 32), TG_D8(C, 40), TG_D8(C, 48) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N128(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D32(C, 0), TG_D32(C, 32) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N160(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n160k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79}, %80, %81, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D32(C, 0), TG_D32(C, 32), TG_D8(C, 64), TG_D8(C, 72) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N192(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n192k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95}, %96, %97, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D32(C, 0), TG_D32(C, 32), TG_D32(C, 64) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N224(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %114, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n224k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111}, %112, %113, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D32(C, 0), TG_D32(C, 32), TG_D32(C, 64), TG_D8(C, 96), TG_D8(C, 104) : "l"(a), "l"(b), "r"(scale_d))
+#define TG_WGMMA_N256(TY, C) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t" \
+    "wgmma.mma_async.sync.aligned.m64n256k16.f32." TY "." TY " {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, 0, 0;\n\t}" \
+    : TG_D32(C, 0), TG_D32(C, 32), TG_D32(C, 64), TG_D32(C, 96) : "l"(a), "l"(b), "r"(scale_d))
+
+#define TG_WGMMA_CASE(n, C)                                                                \
+  else if constexpr (N == n) { if constexpr (F16) TG_WGMMA_N##n("f16", C); else TG_WGMMA_N##n("bf16", C); }
+#define TG_WGMMA_SWITCH(C)                                                                                          \
+  if constexpr (N == 0) {}                                                                                          \
+  TG_WGMMA_CASE(16, C) TG_WGMMA_CASE(32, C) TG_WGMMA_CASE(48, C) TG_WGMMA_CASE(64, C) TG_WGMMA_CASE(80, C)          \
+  TG_WGMMA_CASE(96, C) TG_WGMMA_CASE(112, C) TG_WGMMA_CASE(128, C) TG_WGMMA_CASE(160, C) TG_WGMMA_CASE(192, C)     \
+  TG_WGMMA_CASE(224, C) TG_WGMMA_CASE(256, C)                                                                       \
+  else static_assert(N == 0, "no wgmma wrapper for this N");
+// scale_d == 0 overwrites D (the flash kernels' form, with a run-time flag)
+template <int N, typename T> __device__ __forceinline__ void wgmma_ss(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+  constexpr bool F16 = std::is_same<T, __half>::value;
+  TG_WGMMA_SWITCH("+f")
 }
-template <> __device__ __forceinline__ void wgmma_ss<64, __nv_bfloat16>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b), "r"(acc));
+template <int N, bool ACC, typename T> __device__ __forceinline__ void wgmma_ss(float* d, uint64_t a, uint64_t b) {
+  if constexpr (ACC) {
+    wgmma_ss<N, T>(d, a, b, 1u);
+  } else {
+    constexpr bool F16 = std::is_same<T, __half>::value;
+    const uint32_t scale_d = 0u;
+    TG_WGMMA_SWITCH("=f")
+  }
 }
-template <> __device__ __forceinline__ void wgmma_ss<16, __half>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma_ss<16, __nv_bfloat16>(float* d, uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a), "l"(b), "r"(acc));
-}
+#undef TG_WGMMA_SWITCH
+#undef TG_WGMMA_CASE
+#undef TG_WGMMA_N16
+#undef TG_WGMMA_N32
+#undef TG_WGMMA_N48
+#undef TG_WGMMA_N64
+#undef TG_WGMMA_N80
+#undef TG_WGMMA_N96
+#undef TG_WGMMA_N112
+#undef TG_WGMMA_N128
+#undef TG_WGMMA_N160
+#undef TG_WGMMA_N192
+#undef TG_WGMMA_N224
+#undef TG_WGMMA_N256
+#undef TG_D32
+#undef TG_D8
+#undef TG_D4
 // K-major, 128B-swizzled operand tile for wgmma: rows of 128 B, 8-row groups 1024 B apart (SBO), start address advanced by
 // 32 B (+2 in the descriptor) per K = 16 step inside the swizzle atom.
 __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
@@ -362,40 +419,209 @@ __device__ __forceinline__ void epilogue_chunk(const TapGemmParams& p, const uin
   }
 }
 
-// The whole epilogue of one output tile for one thread (= one accumulator row, read from the fp32 staging tile at `arow`).
-// Two paths, chosen per launch on the host:
-//   * tma_out: 64-column rounds -> this warp's swizzled 4 KB box in smem -> one TMA store per round (see TG_OSTG_WARP);
-//     the residual is fetched with coalesced loads and added from the box; optional GroupNorm
-//     statistics of the rounded output come from the box as well;
-//   * direct: each thread stores its own row (fp32 logits, NCHW image, row-bias V^T, channel counts that are not multiples of 64).
-// LEAN (compile time): the launch takes the TMA-store path with no activation (every conv / linear of the path except the GEGLU,
-// GELU and clamp epilogues) -> the activation branches, the GEGLU rounds and the whole direct path are not compiled in; half the
-// code, fewer instruction-cache misses (17 % of the r02g stall samples were no_inst).
-template <typename T, bool LEAN>
-__device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUtensorMap* tmO, const TileCoord& c, int m_tile,
-                                              int row, int warp, int j1, int j2, int j3, int j4, int acc, uint32_t arow,
-                                              float* s_bias, uint32_t ostg_base, uint32_t ostg2_base, int& box_sel,
-                                              bool stage_bias, bool stamp = false) {
-  const int lane = threadIdx.x & 31;
-  // this warp's store box(es), 1024-byte aligned; with two boxes the warp alternates per round (box_sel persists across tiles)
-  const uint32_t ostg_w0 = ostg_base + warp * TG_OSTG_WARP, ostg_w1 = p.ostg2 ? ostg2_base + warp * TG_OSTG_WARP : ostg_w0;
-  const int grp = warp >> 2;                     // which of the two warps sharing this 32-row quarter
-  const int g1 = c.t[0] * p.box[0] + j1, g2 = c.t[1] * p.box[1] + j2, g3 = c.t[2] * p.box[2] + j3,
-            g4 = c.t[3] * p.box[3] + j4;
-  const bool row_ok = (g1 < p.ext[0]) && (g2 < p.ext[1]) && (g3 < p.ext[2]) && (g4 < p.ext[3]);
-  const long long rbase = p.res ? g1 * p.rstride[0] + g2 * p.rstride[1] + g3 * p.rstride[2] + g4 * p.rstride[3] : 0;
-  const int n0 = c.nt * p.BN;
+// Row coordinates of tile row (j1..j4) in tile c: g1..g4, whether the row lies inside the tensor, and its residual offset.
+struct RowCoord {
+  int g1, g2, g3, g4, ok;
+  long long rbase;
+};
+__device__ __forceinline__ RowCoord row_coord(const TapGemmParams& p, const TileCoord& c, int j1, int j2, int j3, int j4) {
+  RowCoord r;
+  r.g1 = c.t[0] * p.box[0] + j1; r.g2 = c.t[1] * p.box[1] + j2; r.g3 = c.t[2] * p.box[2] + j3; r.g4 = c.t[3] * p.box[3] + j4;
+  r.ok = (r.g1 < p.ext[0]) && (r.g2 < p.ext[1]) && (r.g3 < p.ext[2]) && (r.g4 < p.ext[3]);
+  r.rbase = p.res ? r.g1 * p.rstride[0] + r.g2 * p.rstride[1] + r.g3 * p.rstride[2] + r.g4 * p.rstride[3] : 0;
+  return r;
+}
 
-  // stage this tile's bias slice in smem once (a per-chunk global load here stalled the whole epilogue: r01 ncu)
-  // (a launch with a single n-tile stages its one slice into both buffers during the first two tiles and then skips this and the
-  // barrier: 110 tiles per CTA in the 512x512 convs)
-  float* sb = s_bias + acc * 256;
-  if (stage_bias) {      // no column bias: zeros, so the rounds add unconditionally (one FFMA: alpha * acc + bias)
-    for (int cc = warp * 32 + (threadIdx.x & 31); cc < p.BN; cc += TG_EPI_WARPS * 32)
-      sb[cc] = (p.bias_mode == TG_BIAS_COL && n0 + cc < p.N) ? p.bias[n0 + cc] : 0.f;
-    asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");   // the epilogue warps only
+// Stage this tile's column-bias slice in smem (zeros where there is none, so the epilogue adds unconditionally); all 256
+// epilogue threads take part.  The slice is double-buffered across tiles (acc = iter & 1).
+__device__ __forceinline__ void stage_bias(const TapGemmParams& p, float* sb, int n0, int warp) {
+  for (int cc = warp * 32 + (threadIdx.x & 31); cc < p.BN; cc += TG_EPI_WARPS * 32)
+    sb[cc] = (p.bias_mode == TG_BIAS_COL && n0 + cc < p.N) ? p.bias[n0 + cc] : 0.f;
+  asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");   // the epilogue warps only
+}
+
+// TMA-store epilogue, straight from the wgmma fragments (every tma_out launch: no staging tile, so the operand ring stays with
+// the producer, which loads the next tile while this runs).  Rounds of 64 OUTPUT columns (128 accumulator columns for GEGLU)
+// go through swizzled 32 x 64 store boxes (see TG_OSTG_WARP).  The tile's 32-row quarter q = warp >> 1 comes from the two
+// warps 2q, 2q+1 of one warpgroup (fragment rows 16 (warp & 1) + [0, 16) each); they share the boxes of warps 2q and 2q+1
+// (and the second set with ostg2) and meet at named barrier 2 + q (64 threads).  Box slot s = rsel & (ostg2 ? 3 : 1) of a
+// round belongs to warp 2q + (s & 1): its lane 0 issues the TMA store and it takes the GroupNorm statistics from the box.
+// Lane L of both warps describes tile row 32q + L (rc).  The arithmetic per element is that of every other epilogue:
+// fmaf(acc, alpha, bias), activation, residual, clamp, one rounding.
+template <typename T, bool LEAN, int BN>
+__device__ __forceinline__ void epilogue_frag(const TapGemmParams& p, const CUtensorMap* tmO, const TileCoord& c, int m_tile,
+                                              const float (&accum)[BN / 2], int warp, const RowCoord& rc, const float* sb,
+                                              uint32_t ostg, uint32_t ostg2, int& rsel, bool stamp) {
+  const int lane = threadIdx.x & 31, q = warp >> 1, half = warp & 1;
+  const int n0 = c.nt * BN;
+  const bool geglu = !LEAN && p.act == TG_ACT_GEGLU;
+  const bool res_on = p.res != nullptr && !geglu;
+  const int lrow = lane >> 3, lch = lane & 7;
+  const int fr0 = 16 * half + (lane >> 2);                    // this thread's fragment rows in the quarter: fr0, fr0 + 8
+  const int sw = lane >> 2;                                   // == fr0 & 7 == (fr0 + 8) & 7
+  const int ok0 = __shfl_sync(0xffffffffu, rc.ok, fr0), ok1 = __shfl_sync(0xffffffffu, rc.ok, fr0 + 8);
+  const int cq = 2 * (lane & 3);                              // column pair inside an 8-column fragment group
+  // Residual: this warp's 16 rows of the box, 4 rows x 128 B per instruction; one round ahead of the math.
+  uint4 rq[4];
+  auto load_res = [&](int r) {
+    const int colg = n0 + 64 * r;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int src_row = 16 * half + 4 * i + lrow;
+      const long long rb = __shfl_sync(0xffffffffu, rc.rbase, src_row);
+      const int ok = __shfl_sync(0xffffffffu, rc.ok, src_row);
+      rq[i] = make_uint4(0u, 0u, 0u, 0u);
+      if (ok && colg < p.N) rq[i] = ld_nc16(reinterpret_cast<const T*>(p.res) + rb + colg + lch * 8);
+    }
+  };
+  if (res_on) load_res(0);
+  if (stamp) tg_stamp(p, 8);
+
+  // one round: take a free box, (residual in), the caller's fragment writes, TMA store + statistics by the box's owner
+  auto round = [&](int r, int c0, auto&& write_box) {
+    const int s = rsel & (p.ostg2 ? 3 : 1);
+    ++rsel;
+    const bool owner = (s & 1) == half;                       // warp-uniform
+    const uint32_t box = (s >= 2 ? ostg2 : ostg) + (2 * q + (s & 1)) * TG_OSTG_WARP;
+    // the owner's previous TMA store out of this box must have finished READING it (two box sets: the store before that)
+    if (owner && lane == 0) { if (p.ostg2) bulk_wait_read1(); else bulk_wait_read0(); }
+    asm volatile("bar.sync %0, 64;" ::"r"(2 + q) : "memory");
+    if (res_on) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int rr = 16 * half + 4 * i + lrow;
+        sts16(box + rr * 128 + ((lch ^ (rr & 7)) << 4), rq[i]);
+      }
+      __syncwarp();                                           // a thread reads back only rows of its own warp
+      if (r + 1 < BN / 64) load_res(r + 1);
+    }
+    write_box(box);
+    fence_async_smem();                                       // generic-proxy writes -> visible to the TMA unit
+    asm volatile("bar.sync %0, 64;" ::"r"(2 + q) : "memory");
+    if (!owner) return;
+    const int ocol0 = geglu ? ((n0 + c0) >> 1) : (n0 + c0);
+    if (lane == 0) {                                          // lane 0 describes row 32q, the box origin
+      tma_store_5d(tmO, box, ocol0, rc.g1, rc.g2, rc.g3, rc.g4);
+      bulk_commit();
+    }
+    if (p.gn_part) {
+      // GroupNorm statistics of the tensor just produced, from the ROUNDED values in the box (what the next layer's GroupNorm
+      // sees; rows outside the tensor were written as zeros).  Lane (rg, ch) = (lane >> 3, lane & 7) reads the 16-byte chunk
+      // ch (8 output columns) of rows rg, rg+4, ..., rg+28: eight independent conflict-free ld.shared.v4 (a quarter warp
+      // covers one 128-byte row), per-column-pair sums in registers, then the four row groups are combined by two shuffle
+      // steps and lanes 0..7 write one (sum, sum of squares) entry per gn_red columns.  Fixed order, no atomics.
+      const int rg = lane >> 3, ch = lane & 7;
+      uint4 w[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int rr = 4 * i + rg;
+        w[i] = lds16(box + rr * 128 + ((ch ^ (rr & 7)) << 4));
+      }
+      float s2[4] = {0.f, 0.f, 0.f, 0.f}, q2[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const uint32_t ww[4] = {w[i].x, w[i].y, w[i].z, w[i].w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 f = Elem<T>::unpack(ww[j]);
+          s2[j] += f.x + f.y;
+          q2[j] = fmaf(f.x, f.x, fmaf(f.y, f.y, q2[j]));
+        }
+      }
+      const int red = p.gn_red;                              // 2, 4, 8 or 16 columns per entry (warp-uniform)
+      if (red >= 4) { s2[0] += s2[1]; q2[0] += q2[1]; s2[2] += s2[3]; q2[2] += q2[3]; }
+      if (red >= 8) { s2[0] += s2[2]; q2[0] += q2[2]; }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if ((red >= 4 && (j & 1)) || (red >= 8 && j)) continue;   // folded above
+        s2[j] += __shfl_xor_sync(0xffffffffu, s2[j], 8);  q2[j] += __shfl_xor_sync(0xffffffffu, q2[j], 8);
+        s2[j] += __shfl_xor_sync(0xffffffffu, s2[j], 16); q2[j] += __shfl_xor_sync(0xffffffffu, q2[j], 16);
+      }
+      if (red == 16) { s2[0] += __shfl_xor_sync(0xffffffffu, s2[0], 1); q2[0] += __shfl_xor_sync(0xffffffffu, q2[0], 1); }
+      if (rg == 0 && m_tile < p.gn_mtiles) {                 // slots without a valid row still get their zeros
+        const int per_row = p.N >> p.gn_shift;
+        const long long slot = p.gn_slot0 + static_cast<long long>(m_tile) * 4 + q;
+        float2* dst = reinterpret_cast<float2*>(p.gn_part) + slot * per_row + ((ocol0 + 8 * ch) >> p.gn_shift);
+        if (red == 2) {
+          reinterpret_cast<float4*>(dst)[0] = make_float4(s2[0], q2[0], s2[1], q2[1]);
+          reinterpret_cast<float4*>(dst)[1] = make_float4(s2[2], q2[2], s2[3], q2[3]);
+        } else if (red == 4) {
+          *reinterpret_cast<float4*>(dst) = make_float4(s2[0], q2[0], s2[2], q2[2]);
+        } else if (red == 8 || (ch & 1) == 0) {
+          *dst = make_float2(s2[0], q2[0]);
+        }
+      }
+    }
+  };
+
+  if (geglu) {
+    // interleaved accumulator columns (2j, 2j+1) = (h_j, gate_j) sit in one thread -> output column j = h * gelu(gate)
+#pragma unroll
+    for (int r = 0; r < BN / 128; ++r) {
+      const int c0 = 128 * r;
+      if (n0 + c0 >= p.N) break;                               // whole round beyond N (last n-tile): nothing to store
+      round(r, c0, [&](uint32_t box) {
+#pragma unroll
+        for (int gg = 0; gg < 16; ++gg) {                     // accumulator columns c0 + 8 gg + cq, +1 -> output column 4 gg + cq / 2
+          const int G = 16 * r + gg, col = c0 + 8 * gg + cq;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float hv = accum[4 * G + 2 * e] * p.alpha + sb[col];
+            const float gv = accum[4 * G + 2 * e + 1] * p.alpha + sb[col + 1];
+            const uint32_t u = Elem<T>::pack(hv * gelu_erf_f(gv), 0.f);
+            const uint32_t a = box + (fr0 + 8 * e) * 128 + (((gg >> 1) ^ sw) << 4) + 8 * (gg & 1) + cq;
+            asm volatile("st.shared.b16 [%0], %1;" ::"r"(a), "h"(static_cast<unsigned short>(u & 0xffffu)) : "memory");
+          }
+        }
+      });
+    }
+    return;
   }
-  if (stamp) tg_stamp(p, 7);
+#pragma unroll
+  for (int r = 0; r < BN / 64; ++r) {
+    const int c0 = 64 * r;
+    if (n0 + c0 >= p.N) break;                                 // whole round beyond N (last n-tile): nothing to store
+    round(r, c0, [&](uint32_t box) {
+#pragma unroll
+      for (int gg = 0; gg < 8; ++gg) {                        // accumulator / output columns c0 + 8 gg + cq, +1
+        const int G = 8 * r + gg, col = c0 + 8 * gg + cq;
+        const float2 bq = *reinterpret_cast<const float2*>(sb + col);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float v0 = fmaf(accum[4 * G + 2 * e], p.alpha, bq.x), v1 = fmaf(accum[4 * G + 2 * e + 1], p.alpha, bq.y);
+          if (!LEAN) {
+            if (p.act == TG_ACT_GELU) { v0 = gelu_erf_f(v0); v1 = gelu_erf_f(v1); }
+            else if (p.act == TG_ACT_QUICKGELU) { v0 = quick_gelu_f(v0); v1 = quick_gelu_f(v1); }
+          }
+          const uint32_t a = box + (fr0 + 8 * e) * 128 + ((gg ^ sw) << 4) + 2 * cq;
+          if (res_on) {
+            uint32_t ru;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ru) : "r"(a) : "memory");
+            const float2 f = Elem<T>::unpack(ru);
+            v0 += f.x; v1 += f.y;
+          }
+          if (!LEAN && p.act == TG_ACT_CLAMP1) { v0 = fminf(fmaxf(v0, -1.0f), 1.0f); v1 = fminf(fmaxf(v1, -1.0f), 1.0f); }
+          uint32_t u = Elem<T>::pack(v0, v1);
+          if (p.gn_part && !(e ? ok1 : ok0)) u = 0u;          // clipped by the TMA store; keeps the statistics clean
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(u) : "memory");
+        }
+      }
+    });
+  }
+}
+
+// Direct-store epilogue of one output tile for one thread (= one accumulator row, read from the fp32 staging tile at `arow`):
+// the launches whose output does not fit whole TMA-store rounds (fp32 logits, NCHW image, row-bias V^T, split-K partials,
+// channel counts that are not multiples of 64).  The row's warp pair takes the 32-column rounds in turn (grp = warp & 1).
+template <typename T>
+__device__ __forceinline__ void epilogue_direct(const TapGemmParams& p, const TileCoord& c, const RowCoord& rc, int warp,
+                                                uint32_t arow, const float* sb, bool stamp) {
+  const int g1 = rc.g1, g2 = rc.g2, g3 = rc.g3, g4 = rc.g4;
+  const bool row_ok = rc.ok;
+  const long long rbase = rc.rbase;
+  const int grp = warp & 1;
+  const int n0 = c.nt * p.BN;
+  const bool geglu = p.act == TG_ACT_GEGLU;
   auto acc_ld16 = [&](int col, uint32_t (&r)[16]) {          // accumulator columns [col, col+16) of this thread's row
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -403,194 +629,6 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
       r[4 * i] = u.x; r[4 * i + 1] = u.y; r[4 * i + 2] = u.z; r[4 * i + 3] = u.w;
     }
   };
-  const bool geglu = !LEAN && p.act == TG_ACT_GEGLU;
-
-  if (LEAN || p.tma_out) {
-    // ================= TMA-store path: rounds of 64 OUTPUT columns (64 accumulator columns, 128 for GEGLU) =================
-    const int acols = geglu ? 128 : 64;                       // accumulator columns per round
-    const int nrounds = p.BN >> (geglu ? 7 : 6);              // host guarantees BN % acols == 0 and N % acols == 0
-    const bool res_on = p.res != nullptr && !geglu;
-    // Residual prefetch: one round ahead, so its latency overlaps the previous round's math.  Instruction i loads rows 4i..4i+3 of the warp's 32 (8 lanes x 16 B = one full 128-byte row
-    // segment each) -> 4 fully used lines per instruction instead of 32 half-used sectors.
-    uint4 rq[8];
-    const int lrow = lane >> 3, lch = lane & 7;
-    auto load_res = [&](int r) {                             // this warp's residual box of round r -> registers
-      const int colg = n0 + 64 * r;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int src_row = 4 * i + lrow;
-        const long long rb = __shfl_sync(0xffffffffu, rbase, src_row);
-        const int ok = __shfl_sync(0xffffffffu, static_cast<int>(row_ok), src_row);
-        rq[i] = make_uint4(0u, 0u, 0u, 0u);
-        if (ok && r < nrounds && colg < p.N)
-          rq[i] = ld_nc16(reinterpret_cast<const T*>(p.res) + rb + colg + lch * 8);
-      }
-    };
-    if (res_on) load_res(grp);
-    if (stamp) tg_stamp(p, 8);
-    const int sw = lane & 7;
-#pragma unroll
-    for (int k = 0; k < TG_EPI_RPW / 2; ++k) {
-      const int r = grp + TG_EPI_GROUPS * k;
-      if (r >= nrounds) break;                               // warp-uniform
-      const int c0 = acols * r;                              // accumulator column of this round inside the tile
-      if (n0 + c0 >= p.N) break;                             // whole round beyond N (last n-tile): nothing to store
-      // the previous TMA store out of this box must have finished READING it (two boxes: the store before the previous one)
-      const uint32_t ostg_warp = box_sel ? ostg_w1 : ostg_w0;
-      const uint32_t my_row = ostg_warp + lane * 128;
-      if (lane == 0) { if (p.ostg2) bulk_wait_read1(); else bulk_wait_read0(); }
-      __syncwarp();
-      box_sel ^= p.ostg2;
-      if (res_on) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int rr = 4 * i + lrow;
-          sts16(ostg_warp + rr * 128 + ((lch ^ (rr & 7)) << 4), rq[i]);
-        }
-        __syncwarp();
-        if (r + TG_EPI_GROUPS < nrounds) load_res(r + TG_EPI_GROUPS);   // next round's residual: in flight during this round's math
-      }
-      const int nq = geglu ? 4 : 2;
-      // 32 accumulator columns per step, in two register buffers
-      uint32_t xa0[16], xa1[16], xb0[16], xb1[16];       // two 32-column register buffers
-      auto step = [&](int q, const uint32_t (&raw0)[16], const uint32_t (&raw1)[16]) {
-        const uint32_t sbq_s = smem_u32(sb + c0 + 32 * q);      // 16-byte aligned: the bias slice comes in as ld.shared.v4
-        const float* sbq = sb + c0 + 32 * q;
-        if (geglu) {
-          // interleaved accumulator columns (2j, 2j+1) = (h_j, gate_j) -> output column j = h * gelu(gate): 32 -> 16 columns
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t* raw = h ? raw1 : raw0;
-            float o[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float hv = __uint_as_float(raw[2 * i]) * p.alpha + sbq[16 * h + 2 * i];
-              const float gv = __uint_as_float(raw[2 * i + 1]) * p.alpha + sbq[16 * h + 2 * i + 1];
-              o[i] = hv * gelu_erf_f(gv);
-            }
-            uint4 u;
-            u.x = Elem<T>::pack(o[0], o[1]); u.y = Elem<T>::pack(o[2], o[3]);
-            u.z = Elem<T>::pack(o[4], o[5]); u.w = Elem<T>::pack(o[6], o[7]);
-            sts16(my_row + (((2 * q + h) ^ sw) << 4), u);
-          }
-        } else {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t* raw = h ? raw1 : raw0;
-            float v[16];
-#pragma unroll
-            for (int i4 = 0; i4 < 4; ++i4) {               // v = alpha * acc + bias (zeros staged when there is no column bias)
-              const uint4 bq = lds16(sbq_s + (16 * h + 4 * i4) * 4);
-              v[4 * i4] = fmaf(__uint_as_float(raw[4 * i4]), p.alpha, __uint_as_float(bq.x));
-              v[4 * i4 + 1] = fmaf(__uint_as_float(raw[4 * i4 + 1]), p.alpha, __uint_as_float(bq.y));
-              v[4 * i4 + 2] = fmaf(__uint_as_float(raw[4 * i4 + 2]), p.alpha, __uint_as_float(bq.z));
-              v[4 * i4 + 3] = fmaf(__uint_as_float(raw[4 * i4 + 3]), p.alpha, __uint_as_float(bq.w));
-            }
-            if (!LEAN) {
-              if (p.act == TG_ACT_GELU) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) v[i] = gelu_erf_f(v[i]);
-              } else if (p.act == TG_ACT_QUICKGELU) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) v[i] = quick_gelu_f(v[i]);
-              }
-            }
-            const uint32_t a0 = my_row + (((4 * q + 2 * h) ^ sw) << 4), a1 = my_row + (((4 * q + 2 * h + 1) ^ sw) << 4);
-            if (res_on) {
-              const uint4 r0 = lds16(a0), r1 = lds16(a1);
-              const uint32_t ru[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float2 f = Elem<T>::unpack(ru[i]);
-                v[2 * i] += f.x; v[2 * i + 1] += f.y;
-              }
-            }
-            if (!LEAN && p.act == TG_ACT_CLAMP1) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] = fminf(fmaxf(v[i], -1.0f), 1.0f);
-            }
-            uint4 u0, u1;
-            u0.x = Elem<T>::pack(v[0], v[1]);   u0.y = Elem<T>::pack(v[2], v[3]);
-            u0.z = Elem<T>::pack(v[4], v[5]);   u0.w = Elem<T>::pack(v[6], v[7]);
-            u1.x = Elem<T>::pack(v[8], v[9]);   u1.y = Elem<T>::pack(v[10], v[11]);
-            u1.z = Elem<T>::pack(v[12], v[13]); u1.w = Elem<T>::pack(v[14], v[15]);
-            if (p.gn_part && !row_ok) u0 = u1 = make_uint4(0u, 0u, 0u, 0u);   // clipped by the TMA store; keeps the statistics clean
-            sts16(a0, u0);
-            sts16(a1, u1);
-          }
-        }
-      };
-      acc_ld16(c0, xa0); acc_ld16(c0 + 16, xa1);
-      acc_ld16(c0 + 32, xb0); acc_ld16(c0 + 48, xb1);
-      step(0, xa0, xa1);
-      if (!LEAN && nq > 2) { acc_ld16(c0 + 64, xa0); acc_ld16(c0 + 80, xa1); }   // warp-uniform (GEGLU rounds)
-      step(1, xb0, xb1);
-      if (!LEAN && nq > 2) {
-        acc_ld16(c0 + 96, xb0); acc_ld16(c0 + 112, xb1);
-        step(2, xa0, xa1);
-        step(3, xb0, xb1);
-      }
-      fence_async_smem();                                    // generic-proxy writes -> visible to the TMA unit
-      __syncwarp();
-      const int ocol0 = geglu ? ((n0 + c0) >> 1) : (n0 + c0);
-      if (lane == 0) {                                       // lane 0 holds the box origin: its own row coordinates
-        tma_store_5d(tmO, ostg_warp, ocol0, g1, g2, g3, g4);
-        bulk_commit();
-      }
-      if (p.gn_part) {
-        // GroupNorm statistics of the tensor just produced, from the ROUNDED values in the box (what the next layer's GroupNorm
-        // sees; rows outside the tensor were written as zeros).  Lane (rg, ch) = (lane >> 3, lane & 7) reads the 16-byte chunk
-        // ch (8 output columns) of rows rg, rg+4, ..., rg+28: eight independent conflict-free ld.shared.v4 (a quarter warp
-        // covers one 128-byte row), per-column-pair sums in registers, then the four row groups are combined by two shuffle
-        // steps and lanes 0..7 write one (sum, sum of squares) entry per gn_red columns.  Fixed order, no atomics.
-        const int rg = lane >> 3, ch = lane & 7;
-        uint4 w[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int rr = 4 * i + rg;
-          w[i] = lds16(ostg_warp + rr * 128 + ((ch ^ (rr & 7)) << 4));
-        }
-        float s2[4] = {0.f, 0.f, 0.f, 0.f}, q2[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const uint32_t ww[4] = {w[i].x, w[i].y, w[i].z, w[i].w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float2 f = Elem<T>::unpack(ww[j]);
-            s2[j] += f.x + f.y;
-            q2[j] = fmaf(f.x, f.x, fmaf(f.y, f.y, q2[j]));
-          }
-        }
-        const int red = p.gn_red;                            // 2, 4, 8 or 16 columns per entry (warp-uniform)
-        if (red >= 4) { s2[0] += s2[1]; q2[0] += q2[1]; s2[2] += s2[3]; q2[2] += q2[3]; }
-        if (red >= 8) { s2[0] += s2[2]; q2[0] += q2[2]; }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if ((red >= 4 && (j & 1)) || (red >= 8 && j)) continue;   // folded above
-          s2[j] += __shfl_xor_sync(0xffffffffu, s2[j], 8);  q2[j] += __shfl_xor_sync(0xffffffffu, q2[j], 8);
-          s2[j] += __shfl_xor_sync(0xffffffffu, s2[j], 16); q2[j] += __shfl_xor_sync(0xffffffffu, q2[j], 16);
-        }
-        if (red == 16) { s2[0] += __shfl_xor_sync(0xffffffffu, s2[0], 1); q2[0] += __shfl_xor_sync(0xffffffffu, q2[0], 1); }
-        if (rg == 0 && m_tile < p.gn_mtiles) {               // slots without a valid row still get their zeros
-          const int per_row = p.N >> p.gn_shift;
-          const long long slot = p.gn_slot0 + static_cast<long long>(m_tile) * 4 + (warp & 3);
-          float2* dst = reinterpret_cast<float2*>(p.gn_part) + slot * per_row + ((ocol0 + 8 * ch) >> p.gn_shift);
-          if (red == 2) {
-            reinterpret_cast<float4*>(dst)[0] = make_float4(s2[0], q2[0], s2[1], q2[1]);
-            reinterpret_cast<float4*>(dst)[1] = make_float4(s2[2], q2[2], s2[3], q2[3]);
-          } else if (red == 4) {
-            *reinterpret_cast<float4*>(dst) = make_float4(s2[0], q2[0], s2[2], q2[2]);
-          } else if (red == 8 || (ch & 1) == 0) {
-            *dst = make_float2(s2[0], q2[0]);
-          }
-        }
-      }
-    }
-    return;
-  }
-
-  if constexpr (LEAN) return;
-  // ================= direct path =================
   const long long obase = g1 * p.ostride[0] + g2 * p.ostride[1] + g3 * p.ostride[2] + g4 * p.ostride[3] + c.split * p.split_ostride;
   const float rbias = (p.bias_mode == TG_BIAS_ROW && row_ok) ? p.bias[g1] : 0.0f;
   // This thread's WHOLE residual slice (its row x the 32-column rounds r = grp, grp+2, ...; <= 256 B) is requested up front,
@@ -635,7 +673,8 @@ __device__ __forceinline__ void epilogue_tile(const TapGemmParams& p, const CUte
   }
 }
 
-template <typename T, bool LEAN>
+
+template <typename T, bool LEAN, int BN>
 __global__ void __launch_bounds__(TG_THREADS, 1)
 tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -680,59 +719,70 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   pdl_sync();   // prologue (barriers, descriptor prefetch) overlaps the previous kernel's tail; no global access before here
   if (threadIdx.x == 0) tg_stamp(p, 1);
 
-  if (warp >= TG_EPI_WARPS) reg_dec<TG_REGS_PRODUCER>(); else reg_inc<TG_REGS_CONSUMER>();
-  if (warp == TG_EPI_WARPS) {
-    // ================================ TMA producer (whole warp runs the loop, one elected lane issues) ==========
-    int stage = 0, phase = 0, iter = 0;
-    const uint32_t tx_bytes = TG_A_STAGE + static_cast<uint32_t>(p.BN) * (TG_BK * 2);
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-      const TileCoord c = decode_tile(p, tile);
-      const int a1 = c.t[0] * p.a_mul[0], a2 = c.t[1] * p.a_mul[1], a3 = c.t[2] * p.a_mul[2],
-                a4 = c.t[3] * p.a_mul[3];
-      const int b2 = c.t[1] * p.b_mul[0], b3 = c.t[2] * p.b_mul[1], b4 = c.t[3] * p.b_mul[2];
-      const int n0 = c.nt * p.BN;
-      // the ring doubles as the previous tile's accumulator staging tile until its epilogue has read it
-      if (iter > 0) mbar_wait(epi_done, (iter - 1) & 1, p.err, 2);
-      auto load_step = [&](int t, int kc) {
-        const CUtensorMap* ta = p.tap_src[t] ? &tmA2 : &tmA;
-        const CUtensorMap* tb = p.tap_src[t] ? &tmB2 : &tmB;
-        mbar_wait(empty_bar(stage), phase ^ 1, p.err, 1);
-        if (elect_one()) {
-          mbar_expect_tx(full_bar(stage), tx_bytes);
-          tma_load_5d(sA + stage * TG_A_STAGE, ta, full_bar(stage), kc * TG_BK + p.tap_a[t][0],
-                      a1 + p.tap_a[t][1], a2 + p.tap_a[t][2], a3 + p.tap_a[t][3], a4 + p.tap_a[t][4]);
-          tma_load_5d(sB + stage * BST, tb, full_bar(stage), kc * TG_BK + p.tap_b[t][0], n0,
-                      b2 + p.tap_b[t][1], b3 + p.tap_b[t][2], b4 + p.tap_b[t][3]);
-        }
-        __syncwarp();
-        if (++stage == NS) { stage = 0; phase ^= 1; }
-      };
-      const int kc0 = nsplit > 1 ? c.split * p.kc_per : 0, kc1 = nsplit > 1 ? min(p.kchunks, kc0 + p.kc_per) : p.kchunks;
-      for (int kc = kc0; kc < kc1; ++kc)
-        for (int t = 0; t < p.nprim; ++t) load_step(t, kc);
-      if (c.split == 0)
-        for (int t = p.nprim; t < p.num_taps; ++t)
-          for (int kc = 0; kc < p.tap_kc[t]; ++kc) load_step(t, kc);
-      if (tile == static_cast<int>(blockIdx.x) && lane == 0) tg_stamp(p, 2);   // first tile's loads all issued
+  // setmaxnreg inside each role's branch: issued by all warps before the role branches, both were ignored (C7507)
+  if (warp >= TG_EPI_WARPS) {
+    reg_dec<TG_REGS_PRODUCER>();
+    if (warp == TG_EPI_WARPS) {             // warps 9..11 only hand their registers to the consumers
+      // ================================ TMA producer (whole warp runs the loop, one elected lane issues) ==========
+      int stage = 0, phase = 0, iter = 0;
+      const uint32_t tx_bytes = TG_A_STAGE + static_cast<uint32_t>(p.BN) * (TG_BK * 2);
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
+        const TileCoord c = decode_tile(p, tile);
+        const int a1 = c.t[0] * p.a_mul[0], a2 = c.t[1] * p.a_mul[1], a3 = c.t[2] * p.a_mul[2],
+                  a4 = c.t[3] * p.a_mul[3];
+        const int b2 = c.t[1] * p.b_mul[0], b3 = c.t[2] * p.b_mul[1], b4 = c.t[3] * p.b_mul[2];
+        const int n0 = c.nt * p.BN;
+        // direct-store launches: the ring doubles as the previous tile's accumulator staging tile until its epilogue has read it
+        if (iter > 0 && !p.tma_out) mbar_wait(epi_done, (iter - 1) & 1, p.err, 2);
+        auto load_step = [&](int t, int kc) {
+          const CUtensorMap* ta = p.tap_src[t] ? &tmA2 : &tmA;
+          const CUtensorMap* tb = p.tap_src[t] ? &tmB2 : &tmB;
+          mbar_wait(empty_bar(stage), phase ^ 1, p.err, 1);
+          if (elect_one()) {
+            mbar_expect_tx(full_bar(stage), tx_bytes);
+            tma_load_5d(sA + stage * TG_A_STAGE, ta, full_bar(stage), kc * TG_BK + p.tap_a[t][0],
+                        a1 + p.tap_a[t][1], a2 + p.tap_a[t][2], a3 + p.tap_a[t][3], a4 + p.tap_a[t][4]);
+            tma_load_5d(sB + stage * BST, tb, full_bar(stage), kc * TG_BK + p.tap_b[t][0], n0,
+                        b2 + p.tap_b[t][1], b3 + p.tap_b[t][2], b4 + p.tap_b[t][3]);
+          }
+          __syncwarp();
+          if (++stage == NS) { stage = 0; phase ^= 1; }
+        };
+        const int kc0 = nsplit > 1 ? c.split * p.kc_per : 0, kc1 = nsplit > 1 ? min(p.kchunks, kc0 + p.kc_per) : p.kchunks;
+        for (int kc = kc0; kc < kc1; ++kc)
+          for (int t = 0; t < p.nprim; ++t) load_step(t, kc);
+        if (c.split == 0)
+          for (int t = p.nprim; t < p.num_taps; ++t)
+            for (int kc = 0; kc < p.tap_kc[t]; ++kc) load_step(t, kc);
+        if (tile == static_cast<int>(blockIdx.x) && lane == 0) tg_stamp(p, 2);   // first tile's loads all issued
+      }
+      if (lane == 0) tg_stamp(p, 3);
     }
-    if (lane == 0) tg_stamp(p, 3);
-  } else if (warp < TG_EPI_WARPS) {
+  } else {
+    reg_inc<TG_REGS_CONSUMER>();
     // ============================ consumers: wgmma mainloop + epilogue (warps 0..7) ============================
     const int wg = warp >> 2;                    // warpgroup: tile rows [64 wg, 64 wg + 64) in the mainloop
-    const int row = (warp & 3) * 32 + lane;      // epilogue: this thread's accumulator row
+    const int row = 32 * (warp >> 1) + lane;     // epilogue: tile row described by this lane (quarter warp >> 1)
     int rr = row;
     const int j1 = rr % p.box[0]; rr /= p.box[0];
     const int j2 = rr % p.box[1]; rr /= p.box[1];
     const int j3 = rr % p.box[2];
     const int j4 = rr / p.box[2];
-    const bool n64 = (p.BN & 63) == 0;           // N = 64 MMA blocks; otherwise N = 16 blocks (BN is a multiple of 16)
-    const int nblk = n64 ? (p.BN >> 6) : (p.BN >> 4);
-    const int spitch = p.BN + 4;                 // staging row pitch in floats
+    constexpr int spitch = BN + 4;               // staging row pitch in floats
     const uint32_t arow = base + static_cast<uint32_t>(row * spitch * 4);
-    float accum[128];
+    // one k-step (one ring stage): four k16 MMAs of the tile's full width; the first of a tile overwrites the accumulators
+    auto mma_stage = [&](float (&accum)[BN / 2], int stage, auto first) {
+      wgmma_fence();
+      const uint32_t a0 = sA + stage * TG_A_STAGE + wg * (64 * 128), b0 = sB + stage * BST;
 #pragma unroll
-    for (int i = 0; i < 128; ++i) accum[i] = 0.f;
-    int stage = 0, phase = 0, iter = 0, box_sel = 0;
+      for (int k = 0; k < TG_BK / 16; ++k) {
+        const uint64_t adesc = wgmma_desc_sw128(a0) + 2 * k, bdesc = wgmma_desc_sw128(b0) + 2 * k;
+        if (decltype(first)::value && k == 0) wgmma_ss<BN, false, T>(accum, adesc, bdesc);
+        else wgmma_ss<BN, true, T>(accum, adesc, bdesc);
+      }
+      wgmma_commit();
+    };
+    int stage = 0, phase = 0, iter = 0, rsel = 0;   // rsel: store-box rounds so far (epilogue_frag)
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
       int tsteps = steps;
       if (nsplit > 1) {                                                         // this tile's share of the K loop
@@ -740,29 +790,17 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int kc0 = split * p.kc_per, kc1 = min(p.kchunks, kc0 + p.kc_per);
         tsteps = (kc1 - kc0) * p.nprim + (split == 0 ? sec_steps : 0);
       }
-      int prev = -1;
-      for (int s = 0; s < tsteps; ++s) {
+      float accum[BN / 2];                         // live from the tile's first MMA to the staging store only
+      mbar_wait(full_bar(stage), phase, p.err, 3);
+      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 4);                         // first operands landed
+      mma_stage(accum, stage, std::true_type());
+      int prev = stage;
+      if (++stage == NS) { stage = 0; phase ^= 1; }
+      for (int s = 1; s < tsteps; ++s) {
         mbar_wait(full_bar(stage), phase, p.err, 3);
-        if (iter == 0 && s == 0 && threadIdx.x == 0) tg_stamp(p, 4);             // first operands landed
-        wgmma_fence();
-        const uint32_t a0 = sA + stage * TG_A_STAGE + wg * (64 * 128), b0 = sB + stage * BST;
-#pragma unroll
-        for (int k = 0; k < TG_BK / 16; ++k) {
-          const uint64_t adesc = wgmma_desc_sw128(a0) + 2 * k;
-          const uint32_t on = (s > 0 || k > 0) ? 1u : 0u;
-          if (n64) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              if (j < nblk) wgmma_ss<64, T>(&accum[32 * j], adesc, wgmma_desc_sw128(b0 + j * (64 * 128)) + 2 * k, on);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (j < nblk) wgmma_ss<16, T>(&accum[8 * j], adesc, wgmma_desc_sw128(b0 + j * (16 * 128)) + 2 * k, on);
-          }
-        }
-        wgmma_commit();
+        mma_stage(accum, stage, std::false_type());
         wgmma_wait<1>();                                   // the previous step's MMAs have read their stage
-        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+        if (lane == 0) mbar_arrive(empty_bar(prev));
         prev = stage;
         if (++stage == NS) { stage = 0; phase ^= 1; }
       }
@@ -770,29 +808,37 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if (lane == 0) mbar_arrive(empty_bar(prev));
       if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 5);                        // first tile's MMAs complete
 
-      // accumulators -> fp32 staging tile (the producer is parked on epi_done, so no load writes the ring meanwhile); the
-      // barrier first: the other warpgroup's last MMAs may still be reading the ring stages the staging tile overlays
-      asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
-      {
-        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+      const TileCoord c = decode_tile(p, tile);
+      const RowCoord rc = row_coord(p, c, j1, j2, j3, j4);
+      float* const sb = s_bias + (iter & 1) * 256;
+      // a launch with a single n-tile stages its one slice into both buffers during the first two tiles and then skips this and
+      // its barrier (110 tiles per CTA in the 512x512 convs)
+      if (p.n_tiles > 1 || iter < 2) stage_bias(p, sb, c.nt * BN, warp);
+      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 7);
+      if (LEAN || p.tma_out) {
+        epilogue_frag<T, LEAN, BN>(p, &tmO, c, fast_div(tile, p.n_tiles, p.magic[0]), accum, warp, rc, sb, ostg, ostg2, rsel,
+                                   iter == 0 && threadIdx.x == 0);
+      } else if constexpr (!LEAN) {
+        // accumulators -> fp32 staging tile (the producer is parked on epi_done, so no load writes the ring meanwhile); the
+        // barrier first: the other warpgroup's last MMAs may still be reading the ring stages the staging tile overlays
+        asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
+        {
+          const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-        for (int g = 0; g < 32; ++g) {
-          if (8 * g < p.BN) {
+          for (int g = 0; g < BN / 8; ++g) {
             const uint32_t a = base + static_cast<uint32_t>((r0 * spitch + 8 * g + c0) * 4);
             asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(accum[4 * g]), "f"(accum[4 * g + 1]) : "memory");
             asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a + 8 * spitch * 4), "f"(accum[4 * g + 2]),
                          "f"(accum[4 * g + 3]) : "memory");
           }
         }
+        asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
+        epilogue_direct<T>(p, c, rc, warp, arow, sb, iter == 0 && threadIdx.x == 0);
+        // staging tile consumed: the ring goes back to the producer (generic reads ordered before the TMA's async writes)
+        fence_async_smem();
+        asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
+        if (threadIdx.x == 0) mbar_arrive(epi_done);
       }
-      asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
-      const TileCoord c = decode_tile(p, tile);
-      epilogue_tile<T, LEAN>(p, &tmO, c, fast_div(tile, p.n_tiles, p.magic[0]), row, warp, j1, j2, j3, j4, iter & 1, arow,
-                             s_bias, ostg, ostg2, box_sel, p.n_tiles > 1 || iter < 2, iter == 0 && threadIdx.x == 0);
-      // staging tile consumed: the ring goes back to the producer (generic reads ordered before the TMA's async writes)
-      fence_async_smem();
-      asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
-      if (threadIdx.x == 0) mbar_arrive(epi_done);
       if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 9);                        // first tile stored
     }
     if (p.tma_out && lane == 0) bulk_wait_all();      // the store boxes live in this CTA's shared memory
