@@ -95,6 +95,34 @@ def build_text_stack(cross_dim: int = 1024, seed: int = 1234):
 
 
 # ------------------------------------------------------------------------------------------------
+# resize geometry of the CLIs' host pre-processing (src/my_utils/training_utils.py build_transform)
+# ------------------------------------------------------------------------------------------------
+def image_prep_geometry(image_prep: str, H: int, W: int):
+    """(resize, crop) of forward_u8 that equals build_transform(image_prep) on an H x W PIL image: resize (H, W) of the
+    LANCZOS Resize, crop (top, left, height, width) of the CenterCrop or None.  Sizes follow torchvision: Resize(512) gives
+    the short side 512 and the long side int(512 * long / short); CenterCrop puts the window at int(round((h - 512) / 2)).
+    Raises ValueError for the random-crop training transforms and unknown names."""
+    if image_prep in ("resize_512x512", "resize_512"):
+        return (512, 512), None
+    if image_prep in ("resize_256x256", "resize_256"):
+        return (256, 256), None
+    if image_prep == "no_resize":
+        return (H, W), None
+    if image_prep == "resized_crop_512":
+        if W <= H:
+            rs = (int(512 * H / W), 512)
+        else:
+            rs = (512, int(512 * W / H))
+        return rs, (int(round((rs[0] - 512) / 2.0)), int(round((rs[1] - 512) / 2.0)), 512, 512)
+    raise ValueError(f"image_prep {image_prep!r} has no deterministic resize geometry (random crops are training-only)")
+
+
+def paired_geometry(H: int, W: int):
+    """resize (H, W) of src/inference_paired.py:38-41: LANCZOS to the multiple of 8 below each side."""
+    return H - H % 8, W - W % 8
+
+
+# ------------------------------------------------------------------------------------------------
 # light-weight stand-ins for the diffusers module objects the reference exposes as .unet / .vae
 # ------------------------------------------------------------------------------------------------
 class NetHandle:
@@ -295,16 +323,27 @@ class TurboBase(torch.nn.Module):
             self.__dict__["_text_bound"] = key
             self.__dict__["_text_ref"] = text      # keep it alive: id() must not be recycled while the key is cached
 
-    def _staged_forward(self, eng, x, text, eps, noise=None, r=1.0, direction=i2it.A2B, u8_mode=None):
+    @staticmethod
+    def _u8_geometry(shape, resize, crop, out_size):
+        """(H, W, geometry) of a uint8 forward on [B, H, W, 3] images: the network size and the forward_u8 keywords (None
+        without a resize, crop or output size)."""
+        if resize is None and crop is None and out_size is None:
+            return shape[1], shape[2], None
+        rs, cr, out = i2it.resize_geometry((shape[1], shape[2]), resize, crop, out_size)
+        return cr[2], cr[3], {"resize": rs, "crop": cr, "out_size": out}
+
+    def _staged_forward(self, eng, x, text, eps, noise=None, r=1.0, direction=i2it.A2B, u8_mode=None, geometry=None):
         """Run the engine through persistent device staging buffers (per shape/dtype): the captured CUDA graph bakes the IO
         pointers in, so stable addresses mean every call replays the same graph.  Costs two small device-to-device copies;
         the result is returned in a fresh tensor (never aliased across calls).  The text embedding is not an input of the
-        graph: its projections are cached on the engine (_bind_text)."""
+        graph: its projections are cached on the engine (_bind_text).  `geometry`: forward_u8 resize keywords."""
         self._bind_text(eng, text)
-        key = (tuple(x.shape), x.dtype, eps.dtype, noise is not None, _cur_dev())
+        gkey = tuple(sorted(geometry.items())) if geometry else None
+        key = (tuple(x.shape), x.dtype, eps.dtype, noise is not None, _cur_dev(), gkey)
         st = self.__dict__.setdefault("_stage", {}).get(key)
         if st is None:
-            st = {"x": torch.empty_like(x), "eps": torch.empty_like(eps), "out": torch.empty_like(x),
+            out = torch.empty_like(x) if geometry is None else x.new_empty((x.shape[0],) + geometry["out_size"] + (3,))
+            st = {"x": torch.empty_like(x), "eps": torch.empty_like(eps), "out": out,
                   "noise": torch.empty_like(eps) if noise is not None else None}
             if len(self._stage) > 8:
                 self._stage.clear()
@@ -316,7 +355,8 @@ class TurboBase(torch.nn.Module):
         if u8_mode is None:
             eng.forward(st["x"], None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction, out=st["out"])
         else:
-            eng.forward_u8(st["x"], u8_mode, None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction, out=st["out"])
+            eng.forward_u8(st["x"], u8_mode, None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction, out=st["out"],
+                           **(geometry or {}))
         return st["out"].clone()
 
     @staticmethod

@@ -144,6 +144,33 @@ int i2it_forward_u8(i2it_handle* h, const void* x_u8_hwc, int in_mode, const voi
   API_END
 }
 
+int i2it_forward_u8_resize(i2it_handle* h, const void* x_u8_hwc, int in_mode, const i2it_resize_desc* g, const void* text_emb,
+                           int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc, void* out_latent,
+                           int batch, int H, int W, int direction, void* stream) {
+  API_BEGIN(h)
+  I2IT_CHECK(in_mode >= 0 && in_mode <= 2, "i2it_forward_u8_resize: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
+  I2IT_CHECK(x_u8_hwc && out_u8_hwc && g, "i2it_forward_u8_resize: null image pointer or geometry");
+  IO io;
+  std::memset(&io, 0, sizeof io);
+  io.x_u8 = x_u8_hwc; io.in_mode = in_mode; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r;
+  io.out_u8 = out_u8_hwc; io.out_latent = out_latent;
+  E.check_device_error();
+  E.forward(io, batch, H, W, direction, text_batch, static_cast<cudaStream_t>(stream), g);
+  API_END
+}
+
+int i2it_debug_resample_coeffs(int in_size, int out_size, int* bounds, int* coeffs, int cap) {
+  try {
+    const i2it::ResampleTable t = i2it::lanczos_table(in_size, out_size);   // the host function the plans upload from
+    if (coeffs && static_cast<size_t>(cap) < t.coeffs.size()) return -1;
+    if (bounds) std::memcpy(bounds, t.bounds.data(), t.bounds.size() * sizeof(int));
+    if (coeffs) std::memcpy(coeffs, t.coeffs.data(), t.coeffs.size() * sizeof(int));
+    return t.ksize;
+  } catch (...) {
+    return -1;
+  }
+}
+
 long long i2it_debug_fast_div(long long max_dividend, int d, int x) {
   const uint32_t m = i2it::make_magic(max_dividend, d);              // the host function launch_gemm uses
   if (m == 0) return -1;
@@ -395,6 +422,27 @@ int i2it_op_upsample_to(i2it_handle* h, const void* x, int N, int H, int W, int 
     Act y = E.upsample_to(P, view(x, N, H, W, C, C), Ho, Wo);
     E.copy_channels(P, y, view(out, N, Ho, Wo, C, C));
     run_plan(h, P, static_cast<cudaStream_t>(stream));
+  }
+  API_END
+}
+
+int i2it_op_resize_u8(i2it_handle* h, const void* x, int B, int H, int W, void* out, int H2, int W2, void* stream) {
+  API_BEGIN(h)
+  I2IT_CHECK(B > 0 && H > 0 && W > 0 && H2 > 0 && W2 > 0, "i2it_op_resize_u8: sizes must be positive");
+  I2IT_CHECK(x && out, "i2it_op_resize_u8: null image pointer");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (H == H2 && W == W2) {   // PIL returns a copy
+    h->op_meta.clear();
+    I2IT_CUDA(cudaMemcpyAsync(out, x, static_cast<size_t>(B) * H * W * 3, cudaMemcpyDeviceToDevice, st));
+    I2IT_CUDA(cudaStreamSynchronize(st));
+  } else {
+    Plan P;
+    P.io.x_u8 = x; P.io.out_u8 = out;
+    U8View s, d;
+    s.slot = &P.io.x_u8; s.img = 3ll * H * W; s.w = W;
+    d.slot = &P.io.out_u8; d.img = 3ll * H2 * W2; d.w = W2;
+    E.resample_u8(P, s, B, H, W, H2, W2, 0, 0, H2, W2, d);
+    run_plan(h, P, st);
   }
   API_END
 }

@@ -1417,7 +1417,8 @@ void Engine::encode_text(const int* tokens, int batch, void* out, cudaStream_t s
   I2IT_CUDA(cudaGetLastError());
 }
 
-void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int text_batch, cudaStream_t st) {
+void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
+                     const i2it_resize_desc* g) {
   I2IT_CHECK(H % 8 == 0 && W % 8 == 0 && H > 0 && W > 0, "H and W must be positive multiples of 8 (as the reference CLIs crop them)");
   I2IT_CHECK(B > 0 && (text_batch == 1 || text_batch == B), "text_batch must be 1 or batch");
   IO io = io_in;
@@ -1429,7 +1430,16 @@ void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int te
     I2IT_CHECK(it != textkv_.end() && it->second->filled,
                "text_emb == NULL: call i2it_set_text first (and again after every i2it_finalize_weights)");
   }
-  Plan* P = plan_for(B, H, W, direction, text_batch, text_cached, io_mode);
+  if (g) {
+    I2IT_CHECK(io.x_u8 && io.out_u8, "a resize geometry needs the uint8 boundary");
+    I2IT_CHECK(g->in_H > 0 && g->in_W > 0 && g->resize_H > 0 && g->resize_W > 0 && g->out_H > 0 && g->out_W > 0,
+               "resize geometry: sizes must be positive");
+    I2IT_CHECK(g->crop_y >= 0 && g->crop_x >= 0 && g->crop_y + H <= g->resize_H && g->crop_x + W <= g->resize_W,
+               "resize geometry: the H x W crop window lies outside the resized image");
+    // nothing to resize or crop: the plan (and its key) of the plain uint8 forward
+    if (g->in_H == H && g->in_W == W && g->resize_H == H && g->resize_W == W && g->out_H == H && g->out_W == W) g = nullptr;
+  }
+  Plan* P = plan_for(B, H, W, direction, text_batch, text_cached, io_mode, g);
   if (io_mode & IO_U8_OUT) io.out = P->u8_out_tmp;
   P->io = io;
   last_plan_ = P;

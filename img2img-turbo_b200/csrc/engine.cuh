@@ -14,6 +14,7 @@
 #include "prep.cuh"
 #include "tapgemm.cuh"
 #include "flash.cuh"
+#include "resample.cuh"
 
 namespace i2it {
 
@@ -103,6 +104,16 @@ struct IO {
 };
 enum IoMode : int { IO_U8_IN = 1, IO_U8_OUT = 2 };
 
+// uint8 HWC images [B][img bytes][w pixels per row][3] an op reads or writes: a caller pointer read from the plan's IO at
+// launch time (slot), or a plan-internal buffer (p); off selects a window's first pixel
+struct U8View {
+  const void* const* slot = nullptr;
+  uint8_t* p = nullptr;
+  long long off = 0, img = 0;
+  int w = 0;
+  uint8_t* get() const { return (slot ? static_cast<uint8_t*>(const_cast<void*>(*slot)) : p) + off; }
+};
+
 struct OpMeta {                  // bookkeeping for i2it_profile / bench roofline accounting
   std::string kind;              // "tapgemm:conv3x3", "gn_apply", ...
   double flops = 0, bytes = 0;   // ALGORITHMIC work of the launch (2*M*N*K; unique bytes in + out + weights)
@@ -118,7 +129,7 @@ struct Plan {
   struct Trace { unsigned long long* buf; int grid; std::string what; };
   std::vector<Trace> traces;                           // I2IT_TRACE=1 only
   std::vector<std::shared_ptr<void>> keep;
-  std::vector<int> key;                                // (B, H, W, direction, text_batch, text_cached, io_mode)
+  std::vector<int> key;                                // (B, H, W, direction, text_batch, text_cached, io_mode[, resize geometry])
   void* u8_out_tmp = nullptr;                          // NCHW image the last conv writes when the caller wants uint8 HWC
   int* gn_counter = nullptr;                           // per-image tickets of the GroupNorm last-block reductions (zero between launches)
   std::vector<std::pair<size_t, const char*>> ranges;  // (first op index, name): NVTX stage ranges of the eager path
@@ -173,8 +184,11 @@ class Engine {
   void set_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dt, bool is_dev);
   void set_adapter_scale(const std::string& a, float s) { adapter_scale_[a] = s; }
   void finalize(float lw_unet, float lw_vae, float skip_gamma, float twin_r);
-  Plan* plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached = false, int io_mode = 0);
-  void forward(const IO& io, int B, int H, int W, int direction, int text_batch, cudaStream_t st);
+  // g: LANCZOS resize geometry of a uint8 forward (i2it_forward_u8_resize); part of the plan key
+  Plan* plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached = false, int io_mode = 0,
+                 const i2it_resize_desc* g = nullptr);
+  void forward(const IO& io, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
+               const i2it_resize_desc* g = nullptr);
   // cross-attention K / V^T of the prompt, computed once per prompt (i2it_set_text) instead of once per forward
   void set_text(const void* text, int text_batch, cudaStream_t st);
   // CLIP text tower (SURVEY 8f #1): tokens [batch, 77] int32 -> last_hidden_state [batch, 77, hidden] in the handle dtype
@@ -199,6 +213,10 @@ class Engine {
   Act upsample2x(Plan& P, const Act& x) { return upsample_to(P, x, 2 * x.H, 2 * x.W); }
   Act upsample_to(Plan& P, const Act& x, int Ho, int Wo);          // F.interpolate(size=(Ho,Wo), mode="nearest")
   Act pad_even(Plan& P, const Act& x);                               // zero-padded copy with even H and W
+  // PIL LANCZOS resize of src [B, inH, inW, 3] to rsH x rsW, window [y0, y0+H) x [x0, x0+W) written densely to dst
+  // [B, H, W, 3]: the horizontal pass if the width changes, then the vertical pass if the height changes (at least one must)
+  void resample_u8(Plan& P, const U8View& src, int B, int inH, int inW, int rsH, int rsW, int y0, int x0, int H, int W,
+                   const U8View& dst);
   void copy_channels(Plan& P, const Act& src, const Act& dst_slice);
   // V^T[b] = Wv X[b]^T (+ row bias): returns [B][C][ldv] as an Act with N=B,H=1,W=C,ld=ldv (C field = Ntok)
   Act vt_proj(Plan& P, const Act& x_tokens, int B, int ntok, const PW& wv);
@@ -227,7 +245,8 @@ class Engine {
   int prep_launches_ = 0;
 
   // ---- model graph ----
-  Act build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int W, std::vector<Act>& skips, bool u8_in = false);
+  Act build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int W, std::vector<Act>& skips,
+                        const U8View* u8_in = nullptr);
   Act build_unet(Plan& P, const Act& z, int text_batch, bool text_cached);
   void build_text_kv(struct TextKV& T);
   std::vector<std::string> xformer_prefixes() const;

@@ -443,8 +443,8 @@ __device__ __forceinline__ float u8_to_input(uint8_t q, int mode) {
   return v;
 }
 template <typename T>
-__global__ void pack_input_im2col_u8_kernel(const uint8_t* __restrict__ x /*[B,H,W,3]*/, T* __restrict__ y, int H, int W,
-                                            long long total, int mode) {
+__global__ void pack_input_im2col_u8_kernel(const uint8_t* __restrict__ x /*[B][x_img bytes][x_w][3]*/, long long x_img, int x_w,
+                                            T* __restrict__ y, int H, int W, long long total, int mode) {
   pdl_sync();
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;   // over B*H*W pixels
   if (i >= total) return;
@@ -460,7 +460,7 @@ __global__ void pack_input_im2col_u8_kernel(const uint8_t* __restrict__ x /*[B,H
     for (int kx = 0; kx < 3; ++kx) {
       const int yy = py + ky - 1, xx = px + kx - 1;
       if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
-        const uint8_t* q = x + ((n * H + yy) * W + xx) * 3;
+        const uint8_t* q = x + n * x_img + (static_cast<long long>(yy) * x_w + xx) * 3;   // H x W window of the image
 #pragma unroll
         for (int c = 0; c < 3; ++c) v[(ky * 3 + kx) * 3 + c] = Elem<T>::to_f(Elem<T>::from_f(u8_to_input(q[c], mode)));
       }

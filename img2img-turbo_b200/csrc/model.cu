@@ -65,7 +65,8 @@ Act Engine::vae_attn(Plan& P, const std::string& p, const Act& x) {
   return y;
 }
 
-Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int W, std::vector<Act>& skips, bool u8_in) {
+Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int W, std::vector<Act>& skips,
+                              const U8View* u8_in) {
   const std::string e = vp + "encoder";
   // conv_in (3 -> C0, 3x3): the NCHW boundary tensor is packed straight into im2col rows [B,H,W,32] (27 taps*channels + 5
   // zeros), so the conv is ONE K=32 GEMM tap with 64-byte TMA rows instead of nine taps of 16-byte rows
@@ -76,9 +77,10 @@ Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int 
     Plan* plan = &P;
     const int dt = dtype, hh = H, ww = W;
     if (u8_in) {
+      const U8View src = *u8_in;
       add_op(P, [=](cudaStream_t st) {
         DISPATCH_T(dt, (launch_k(pack_input_im2col_u8_kernel<T>, dim3(ceil_div_i(total, 128)), dim3(128), 0, st, 0,
-                           reinterpret_cast<const uint8_t*>(plan->io.x_u8), reinterpret_cast<T*>(yp), hh, ww, total, plan->io.in_mode)));
+                           src.get(), src.img, src.w, reinterpret_cast<T*>(yp), hh, ww, total, plan->io.in_mode)));
       }, "pack_im2col_u8", 0, 1.0 * total * (3 + 64));
     } else {
       add_op(P, [=](cudaStream_t st) {
@@ -427,8 +429,70 @@ Act Engine::build_unet(Plan& P, const Act& z, int text_batch, bool text_cached) 
 }
 
 // ------------------------------------------------------------------------------------------ whole path
-Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached, int io_mode) {
-  const std::vector<int> key{B, H, W, direction, text_batch, text_cached ? 1 : 0, io_mode};
+void Engine::resample_u8(Plan& P, const U8View& src, int B, int inH, int inW, int rsH, int rsW, int y0, int x0, int H, int W,
+                         const U8View& dst) {
+  const bool need_h = inW != rsW, need_v = inH != rsH;
+  I2IT_CHECK(need_h || need_v, "resample_u8: the size does not change");
+  I2IT_CHECK(y0 >= 0 && x0 >= 0 && y0 + H <= rsH && x0 + W <= rsW, "resample_u8: window outside the resized image");
+  // [bounds | coefficients] on the device, written once here: a fresh block, never recycled by later ops of the plan
+  auto upload = [&P](const ResampleTable& t) {
+    int* d = static_cast<int*>(P.pool.get_fresh((t.bounds.size() + t.coeffs.size()) * sizeof(int)));
+    I2IT_CUDA(cudaMemcpy(d, t.bounds.data(), t.bounds.size() * sizeof(int), cudaMemcpyHostToDevice));
+    I2IT_CUDA(cudaMemcpy(d + t.bounds.size(), t.coeffs.data(), t.coeffs.size() * sizeof(int), cudaMemcpyHostToDevice));
+    return d;
+  };
+  const std::string geo = std::to_string(B) + "x" + std::to_string(inH) + "x" + std::to_string(inW) + "->" + std::to_string(rsH) +
+                          "x" + std::to_string(rsW) + "@" + std::to_string(y0) + "," + std::to_string(x0) + ":" +
+                          std::to_string(H) + "x" + std::to_string(W);
+  // source rows the vertical pass reads (the window's rows when only the width changes); the horizontal pass makes only these
+  ResampleTable tv;
+  int r0 = y0, r1 = y0 + H;
+  if (need_v) {
+    tv = lanczos_table(inH, rsH);
+    r0 = tv.bounds[2 * static_cast<size_t>(y0)];
+    r1 = tv.bounds[2 * static_cast<size_t>(y0 + H - 1)] + tv.bounds[2 * static_cast<size_t>(y0 + H - 1) + 1];
+  }
+  U8View vsrc = src;
+  int col0 = x0, shift = 0;
+  if (need_h) {
+    const ResampleTable th = lanczos_table(inW, rsW);
+    const int* tab = upload(th);
+    const int rows = r1 - r0, ks = th.ksize;
+    U8View hd = dst;
+    if (need_v) {
+      auto buf = alloc_raw(P, static_cast<size_t>(B) * rows * W * 3);
+      P.keep.push_back(buf);
+      hd = U8View();
+      hd.p = static_cast<uint8_t*>(buf.get()); hd.img = static_cast<long long>(rows) * W * 3; hd.w = W;
+    }
+    const long long total = static_cast<long long>(B) * rows * W;
+    const int span = th.bounds[2 * static_cast<size_t>(x0 + W - 1)] + th.bounds[2 * static_cast<size_t>(x0 + W - 1) + 1] -
+                     th.bounds[2 * static_cast<size_t>(x0)];
+    const double bytes = 3.0 * B * rows * (span + W) + 4.0 * W * (2 + ks);
+    const int* coef = tab + 2 * static_cast<size_t>(rsW);
+    add_op(P, [=](cudaStream_t st) {
+      launch_k(resample_h_u8_kernel, dim3(ceil_div_i(total, 256)), dim3(256), 0, st, 0, src.get(), src.img, src.w, r0,
+               hd.get(), rows, W, x0, tab, coef, ks, total);
+    }, "resample_h", 0, bytes, geo);
+    vsrc = hd; col0 = 0; shift = r0;
+  }
+  if (need_v) {
+    const int* tab = upload(tv);
+    const int* coef = tab + 2 * static_cast<size_t>(rsH);
+    const int ks = tv.ksize;
+    const long long total = static_cast<long long>(B) * H * W;
+    const double bytes = 3.0 * B * W * ((r1 - r0) + H) + 4.0 * H * (2 + ks);
+    add_op(P, [=](cudaStream_t st) {
+      launch_k(resample_v_u8_kernel, dim3(ceil_div_i(total, 256)), dim3(256), 0, st, 0, vsrc.get(), vsrc.img, vsrc.w, col0,
+               shift, dst.get(), H, W, y0, tab, coef, ks, total);
+    }, "resample_v", 0, bytes, geo);
+  }
+}
+
+Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached, int io_mode,
+                       const i2it_resize_desc* g) {
+  std::vector<int> key{B, H, W, direction, text_batch, text_cached ? 1 : 0, io_mode};
+  if (g) key.insert(key.end(), {g->in_H, g->in_W, g->resize_H, g->resize_W, g->crop_y, g->crop_x, g->out_H, g->out_W});
   auto it = plans_.find(key);
   if (it != plans_.end()) return it->second.get();
   I2IT_CHECK(finalized_, "i2it_finalize_weights must be called before a forward");
@@ -450,8 +514,25 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
     P.keep.push_back(tmp);
     P.u8_out_tmp = tmp.get();
   }
+  // what the first kernel reads: the caller's [B, H, W, 3] image, or with a geometry the H x W network window of its resize
+  U8View net_in;
+  net_in.slot = &P.io.x_u8; net_in.img = 3ll * H * W; net_in.w = W;
+  if (g) {
+    net_in.img = 3ll * g->in_H * g->in_W; net_in.w = g->in_W;
+    if (g->in_H == g->resize_H && g->in_W == g->resize_W) {
+      net_in.off = 3 * (static_cast<long long>(g->crop_y) * g->in_W + g->crop_x);   // a crop of the input itself: no pass
+    } else {
+      auto buf = alloc_raw(P, static_cast<size_t>(B) * H * W * 3);
+      P.keep.push_back(buf);
+      U8View d;
+      d.p = static_cast<uint8_t*>(buf.get()); d.img = 3ll * H * W; d.w = W;
+      P.ranges.emplace_back(P.ops.size(), "resize_in");
+      resample_u8(P, net_in, B, g->in_H, g->in_W, g->resize_H, g->resize_W, g->crop_y, g->crop_x, H, W, d);
+      net_in = d;
+    }
+  }
   P.ranges.emplace_back(P.ops.size(), "vae_encode");
-  Act z = build_vae_encoder(P, vp, B, H, W, skips, (io_mode & IO_U8_IN) != 0);
+  Act z = build_vae_encoder(P, vp, B, H, W, skips, (io_mode & IO_U8_IN) ? &net_in : nullptr);
   P.ranges.emplace_back(P.ops.size(), "unet");
   Act pred = build_unet(P, z, text_batch, text_cached);
   mark(P, "model_pred", pred);
@@ -480,14 +561,30 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
   P.ranges.emplace_back(P.ops.size(), "vae_decode");
   build_vae_decoder(P, vp, dec_in, skips);
   if (io_mode & IO_U8_OUT) {
-    // the last conv wrote NCHW into an internal buffer (forward() points io.out at it); convert to uint8 HWC for the caller
+    // the last conv wrote NCHW into an internal buffer (forward() points io.out at it); convert to uint8 HWC for the caller,
+    // or with an output size into an internal [B, H, W, 3] image that the resize passes read
     const long long HW = static_cast<long long>(H) * W, total = HW * B;
     const int dt = dtype;
     Plan* plan = &P;
+    U8View out;
+    out.slot = &P.io.out_u8; out.img = 3 * HW; out.w = W;
+    const bool resize_out = g && (g->out_H != H || g->out_W != W);
+    U8View net_out = out;
+    if (resize_out) {
+      auto buf = alloc_raw(P, static_cast<size_t>(total) * 3);
+      P.keep.push_back(buf);
+      net_out = U8View();
+      net_out.p = static_cast<uint8_t*>(buf.get()); net_out.img = 3 * HW; net_out.w = W;
+    }
     add_op(P, [=](cudaStream_t st) {
       DISPATCH_T(dt, (launch_k(nchw_to_u8hwc_kernel<T>, dim3(ceil_div_i(total, 256)), dim3(256), 0, st, 0,
-                         reinterpret_cast<const T*>(plan->io.out), reinterpret_cast<uint8_t*>(plan->io.out_u8), HW, total)));
+                         reinterpret_cast<const T*>(plan->io.out), net_out.get(), HW, total)));
     }, "unpack_u8", 0, 1.0 * total * (6 + 3));
+    if (resize_out) {
+      out.img = 3ll * g->out_H * g->out_W; out.w = g->out_W;
+      P.ranges.emplace_back(P.ops.size(), "resize_out");
+      resample_u8(P, net_out, B, H, W, g->out_H, g->out_W, 0, 0, g->out_H, g->out_W, out);
+    }
   }
   flush_prep();                             // every weight of the plan: one fold/re-layout launch (+ the time-embedding GEMVs)
   I2IT_CUDA(cudaDeviceSynchronize());       // weight preparation ran on the default stream

@@ -177,9 +177,14 @@ class CycleGAN_Turbo(TurboBase):
         return self.forward_with_networks(x_t, direction, self.vae_enc, self.unet, self.vae_dec, self.sched, self.timesteps,
                                           caption_enc, eps)
 
-    def forward_u8(self, images_u8, direction=None, caption=None, caption_emb=None, *, eps=None):
+    def forward_u8(self, images_u8, direction=None, caption=None, caption_emb=None, *, eps=None, resize=None, crop=None,
+                   out_size=None):
         """uint8 HWC boundary (SURVEY 8f #3): [B,H,W,3] uint8 -> [B,H,W,3] uint8 CUDA tensor.  Fuses ToTensor + Normalize([0.5],[0.5])
-        (inference_unpaired.py:45-47) and ToPILImage()(out*0.5+0.5) (:53) around the same fused forward."""
+        (inference_unpaired.py:45-47) and ToPILImage()(out*0.5+0.5) (:53) around the same fused forward.
+
+        resize / crop / out_size (i2it.Engine.forward_u8) also run the CLI's PIL LANCZOS resizes on device, bit-exact:
+        `resize, crop = _host.image_prep_geometry(image_prep, H, W)` replaces build_transform(image_prep) (:40-45), and
+        out_size=(H, W) the resize back to the input size (:53).  eps then has the crop's size."""
         if direction is None:
             assert self.direction is not None
             direction = self.direction
@@ -190,10 +195,11 @@ class CycleGAN_Turbo(TurboBase):
         dt = self.compute_dtype
         text = self._prep(caption_emb if caption_emb is not None else self._encode_text(caption), dt)
         x = images_u8.to(device=_host.DEVICE, non_blocking=True).contiguous()
-        B, H, Wd, _ = x.shape
+        B = x.shape[0]
+        H, Wd, geom = self._u8_geometry(x.shape, resize, crop, out_size)
         if eps is None:
             eps = torch.randn((B, 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)
         eps = self._prep(eps, dt)
         eng = self._finalize(1.0, 1.0, 1.0, -1.0)
         return self._staged_forward(eng, x, text, eps, direction=i2it.A2B if direction == "a2b" else i2it.B2A,
-                                    u8_mode=i2it.IN_NORMALIZE)
+                                    u8_mode=i2it.IN_NORMALIZE, geometry=geom)

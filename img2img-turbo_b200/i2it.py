@@ -31,6 +31,7 @@ SYMBOLS = [
     "i2it_set_text", "i2it_encode_text", "i2it_forward_u8", "i2it_prep_launch_count", "i2it_debug_fast_div", "i2it_launch_count", "i2it_profile", "i2it_read_stage", "i2it_op_conv2d", "i2it_op_group_norm", "i2it_op_layer_norm",
     "i2it_op_attention", "i2it_op_upsample2x", "i2it_op_conv2d_ex", "i2it_op_launches", "i2it_op_vt_proj",
     "i2it_op_upsample_to", "i2it_stage_names", "i2it_prepared_keys", "i2it_read_prepared", "i2it_text_stage_names",
+    "i2it_forward_u8_resize", "i2it_op_resize_u8", "i2it_debug_resample_coeffs",
 ]
 TEXT_TOKEN_EMB = "text_encoder.text_model.embeddings.token_embedding.weight"
 TEXT_POS_EMB = "text_encoder.text_model.embeddings.position_embedding.weight"
@@ -60,6 +61,38 @@ class ConvDesc(C.Structure):
         ("gn_y", C.c_void_p), ("ldg", C.c_int), ("gn_silu", C.c_int), ("gn_eps", C.c_float), ("gn_gamma", C.c_void_p),
         ("gn_beta", C.c_void_p),
     ]
+
+
+class ResizeDesc(C.Structure):
+    """i2it_resize_desc (include/i2it.h); sizes are rows x columns."""
+    _fields_ = [(n, C.c_int) for n in ("in_H", "in_W", "resize_H", "resize_W", "crop_y", "crop_x", "out_H", "out_W")]
+
+
+def resize_geometry(in_hw, resize=None, crop=None, out_size=None):
+    """Complete the LANCZOS geometry of a uint8 forward on an image of in_hw = (H, W): resize (H, W) defaults to the input
+    size, crop (top, left, height, width) to the whole resized image, out_size (H, W) to the crop's size.  Returns
+    ((resize_H, resize_W), (top, left, H, W), (out_H, out_W)); the network runs on the H x W window."""
+    rs = tuple(int(v) for v in (resize if resize is not None else in_hw))
+    cr = tuple(int(v) for v in (crop if crop is not None else (0, 0) + rs))
+    out = tuple(int(v) for v in (out_size if out_size is not None else cr[2:]))
+    if len(rs) != 2 or len(cr) != 4 or len(out) != 2:
+        raise ValueError("resize and out_size are (H, W), crop is (top, left, height, width)")
+    return rs, cr, out
+
+
+def resample_coeffs(in_size: int, out_size: int):
+    """Tables of one LANCZOS pass exactly as the resample kernels get them (host only, no GPU):
+    (ksize, bounds [out][2] = (first input index, taps), 22-bit coefficients [out][ksize])."""
+    lib = load_library()
+    ksize = lib.i2it_debug_resample_coeffs(in_size, out_size, None, None, 0)
+    if ksize < 0:
+        raise ValueError(f"bad resample sizes {in_size} -> {out_size}")
+    bounds = (C.c_int * (2 * out_size))()
+    coeffs = (C.c_int * (out_size * ksize))()
+    if lib.i2it_debug_resample_coeffs(in_size, out_size, bounds, coeffs, out_size * ksize) != ksize:
+        raise RuntimeError("i2it_debug_resample_coeffs failed")
+    return ksize, [tuple(bounds[2 * i: 2 * i + 2]) for i in range(out_size)], \
+        [list(coeffs[i * ksize: (i + 1) * ksize]) for i in range(out_size)]
 
 
 class Config(C.Structure):
@@ -120,6 +153,9 @@ def load_library(path: Optional[str] = None):
     lib.i2it_text_stage_names.argtypes = [vp, C.c_char_p, C.c_size_t]
     lib.i2it_prepared_keys.argtypes = [vp, C.c_char_p, C.c_size_t]
     lib.i2it_read_prepared.argtypes = [vp, C.c_char_p, vp, C.c_size_t, vp, C.c_size_t, C.POINTER(ci)]
+    lib.i2it_forward_u8_resize.argtypes = [vp, vp, ci, C.POINTER(ResizeDesc), vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci, vp]
+    lib.i2it_op_resize_u8.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci, vp]
+    lib.i2it_debug_resample_coeffs.argtypes = [ci, ci, C.POINTER(ci), C.POINTER(ci), ci]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("i2it_destroy", "i2it_last_error"):
@@ -266,17 +302,30 @@ class Engine:
 
     def forward_u8(self, x_u8: torch.Tensor, in_mode: int, text_emb: Optional[torch.Tensor], eps: torch.Tensor,
                    noise_map: Optional[torch.Tensor] = None, r: float = 1.0, direction: int = A2B,
-                   out: Optional[torch.Tensor] = None, out_latent: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """uint8 HWC boundary: x_u8 [B,H,W,3] uint8 CUDA -> [B,H,W,3] uint8 CUDA (pre/post-processing fused on device)."""
-        B, H, W, Cc = x_u8.shape
+                   out: Optional[torch.Tensor] = None, out_latent: Optional[torch.Tensor] = None, *,
+                   resize=None, crop=None, out_size=None) -> torch.Tensor:
+        """uint8 HWC boundary: x_u8 [B,H,W,3] uint8 CUDA -> [B,H,W,3] uint8 CUDA (pre/post-processing fused on device).
+
+        With a geometry (see resize_geometry) the PIL LANCZOS resizes around the forward run on device too: x_u8 is resized to
+        `resize` (H, W), the network runs on the `crop` (top, left, height, width) window, and its output image is resized to
+        `out_size` (H, W).  eps / noise_map / out_latent then have the crop's size."""
+        B, Hi, Wi, Cc = x_u8.shape
         assert Cc == 3 and x_u8.dtype == torch.uint8 and x_u8.is_cuda and x_u8.is_contiguous(), "image must be uint8 CUDA [B,H,W,3]"
+        geom = resize is not None or crop is not None or out_size is not None
+        rs, (cy, cx, H, W), osz = resize_geometry((Hi, Wi), resize, crop, out_size)
         tb = self._check_operands(B, H, W, text_emb, eps, (noise_map, out_latent))
         if out is None:
-            out = torch.empty_like(x_u8)
-        assert out.dtype == torch.uint8 and out.is_cuda and out.is_contiguous() and out.shape == x_u8.shape
-        self._check(self.lib.i2it_forward_u8(self._h, _ptr(x_u8), int(in_mode), _ptr(text_emb), tb, _ptr(eps), _ptr(noise_map),
-                                             float(r), _ptr(out), _ptr(out_latent), B, H, W, direction, _stream()),
-                    "i2it_forward_u8")
+            out = torch.empty(B, osz[0], osz[1], 3, dtype=torch.uint8, device=x_u8.device)
+        assert out.dtype == torch.uint8 and out.is_cuda and out.is_contiguous() and out.shape == (B, osz[0], osz[1], 3)
+        if not geom:
+            self._check(self.lib.i2it_forward_u8(self._h, _ptr(x_u8), int(in_mode), _ptr(text_emb), tb, _ptr(eps), _ptr(noise_map),
+                                                 float(r), _ptr(out), _ptr(out_latent), B, H, W, direction, _stream()),
+                        "i2it_forward_u8")
+            return out
+        d = ResizeDesc(Hi, Wi, rs[0], rs[1], cy, cx, osz[0], osz[1])
+        self._check(self.lib.i2it_forward_u8_resize(self._h, _ptr(x_u8), int(in_mode), C.byref(d), _ptr(text_emb), tb, _ptr(eps),
+                                                    _ptr(noise_map), float(r), _ptr(out), _ptr(out_latent), B, H, W, direction,
+                                                    _stream()), "i2it_forward_u8_resize")
         return out
 
     def prep_launch_count(self) -> int:
@@ -444,4 +493,12 @@ class Engine:
         out = torch.empty(N, Ho, Wo, Cc, device="cuda", dtype=self.dtype)
         self._check(self.lib.i2it_op_upsample_to(self._h, _ptr(x_nhwc), N, H, W, Cc, Ho, Wo, _ptr(out), _stream()),
                     "i2it_op_upsample_to")
+        return out
+
+    def op_resize_u8(self, x, H2, W2):
+        """PIL LANCZOS resize of uint8 HWC CUDA images: [B, H, W, 3] -> [B, H2, W2, 3] (synchronous)."""
+        B, H, W, Cc = x.shape
+        assert Cc == 3 and x.dtype == torch.uint8 and x.is_cuda and x.is_contiguous(), "image must be uint8 CUDA [B,H,W,3]"
+        out = torch.empty(B, H2, W2, 3, dtype=torch.uint8, device=x.device)
+        self._check(self.lib.i2it_op_resize_u8(self._h, _ptr(x), B, H, W, _ptr(out), H2, W2, _stream()), "i2it_op_resize_u8")
         return out

@@ -192,15 +192,19 @@ class Pix2Pix_Turbo(TurboBase):
         return out if in_dtype == dt else out.to(in_dtype)
 
     def forward_u8(self, images_u8, prompt=None, prompt_tokens=None, deterministic=True, r=1.0, noise_map=None, *, eps=None,
-                   sketch=False):
+                   sketch=False, resize=None, crop=None, out_size=None):
         """uint8 HWC boundary (SURVEY 8f #3): `images_u8` [B,H,W,3] uint8 (host or device) -> [B,H,W,3] uint8 CUDA tensor.
         Fuses F.to_tensor (edge/canny images, inference_paired.py:50) or the sketch threshold (:56-57) on the way in and
-        ToPILImage()(out*0.5+0.5) (:72) on the way out; everything between is the same i2it_forward."""
+        ToPILImage()(out*0.5+0.5) (:72) on the way out; everything between is the same i2it_forward.
+
+        resize / crop / out_size (i2it.Engine.forward_u8) also run PIL LANCZOS resizes on device, bit-exact:
+        resize=_host.paired_geometry(H, W) is the CLI's resize to multiples of 8 (:38-41).  eps then has the crop's size."""
         assert (prompt is None) != (prompt_tokens is None), "Either prompt or prompt_tokens should be provided"
         dt = self.compute_dtype
         caption_enc = self._encode_text(prompt, prompt_tokens)
         x = images_u8.to(device=_host.DEVICE, non_blocking=True).contiguous()
-        B, H, Wd, _ = x.shape
+        B = x.shape[0]
+        H, Wd, geom = self._u8_geometry(x.shape, resize, crop, out_size)
         if eps is None:
             eps = torch.randn((B, 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)
             torch.randn((B, 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)
@@ -210,14 +214,14 @@ class Pix2Pix_Turbo(TurboBase):
             if self._twin:
                 raise TypeError("deterministic forward on a TwinConv model: conv_in.r is None (as in the reference)")
             eng = self._finalize(self._lora_w_unet, self._lora_w_vae, float(self.vae.decoder.gamma), -1.0)
-            return self._staged_forward(eng, x, caption_enc, eps, u8_mode=mode)
+            return self._staged_forward(eng, x, caption_enc, eps, u8_mode=mode, geometry=geom)
         if noise_map is None:
             raise ValueError("noise_map is required when deterministic=False")
         self._lora_w_unet = self._lora_w_vae = float(r)
         self.vae.decoder.gamma = r
         eng = self._finalize(r, r, r, r if self._twin else -1.0)
         nm = self._prep(noise_map.expand(B, -1, -1, -1) if noise_map.shape[0] != B else noise_map, dt)
-        out = self._staged_forward(eng, x, caption_enc, eps, noise=nm, r=float(r), u8_mode=mode)
+        out = self._staged_forward(eng, x, caption_enc, eps, noise=nm, r=float(r), u8_mode=mode, geometry=geom)
         if self._twin:
             self.unet.conv_in.r = None
         return out

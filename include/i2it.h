@@ -135,6 +135,26 @@ int i2it_forward_u8(i2it_handle* h, const void* x_u8_hwc, int in_mode, const voi
                     const void* eps, const void* noise_map, float r, void* out_u8_hwc, void* out_latent, int batch,
                     int H, int W, int direction, void* stream);
 
+/* LANCZOS resize geometry of i2it_forward_u8_resize: what the reference CLIs do with PIL on the host around the forward
+ * (src/inference_unpaired.py:40-45,53; src/inference_paired.py:38-41), bit-exact with Image.resize(size, Image.LANCZOS).
+ * The caller's image [batch, in_H, in_W, 3] is resized to resize_H x resize_W; the network runs on the H x W window at
+ * (crop_y, crop_x) of it (transforms.CenterCrop); its output image is resized to out_H x out_W.  All sizes are rows x columns. */
+typedef struct i2it_resize_desc {
+  int in_H, in_W;
+  int resize_H, resize_W;
+  int crop_y, crop_x;
+  int out_H, out_W;
+} i2it_resize_desc;
+
+/* i2it_forward_u8 with a resize geometry: x_u8_hwc [batch, in_H, in_W, 3] -> out_u8_hwc [batch, out_H, out_W, 3] (device
+ * pointers); eps / noise_map / out_latent have the network size H x W (multiples of 8).  Each resize is one or two launches
+ * (horizontal pass if the width changes, then vertical if the height changes; none for an unchanged size), captured in the
+ * same CUDA graph; the coefficient tables are computed on the host once per plan.  The geometry is part of the plan key.
+ * Rejected before any launch: non-positive sizes, or a crop window outside the resized image. */
+int i2it_forward_u8_resize(i2it_handle* h, const void* x_u8_hwc, int in_mode, const i2it_resize_desc* g, const void* text_emb,
+                           int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc, void* out_latent,
+                           int batch, int H, int W, int direction, void* stream);
+
 /* Number of kernel launches one forward of this shape issues (for bench accounting): the plan the last forward used if it
  * has this shape, else the plan with the text embedding passed inline. */
 int i2it_launch_count(i2it_handle* h, int batch, int H, int W, int direction, int* launches);
@@ -147,6 +167,12 @@ int i2it_prep_launch_count(i2it_handle* h, int* launches);
  * quotient the device computes for x / d (magic made for dividends <= max_dividend, 32-bit high multiply), or -1 when the host
  * would refuse that tile space.  No GPU needed: lets the CPU test suite pin the index arithmetic bit for bit. */
 long long i2it_debug_fast_div(long long max_dividend, int d, int x);
+
+/* Host-side tables of one LANCZOS resize pass from in_size to out_size samples, exactly as the resample kernels get them:
+ * bounds [out_size][2] = (first input index, number of taps), coeffs [out_size][ksize] 22-bit fixed-point weights (zero past
+ * the taps).  Either pointer may be NULL; coeffs must hold `cap` ints.  Returns ksize, or -1 for bad sizes or a short buffer.
+ * No GPU needed. */
+int i2it_debug_resample_coeffs(int in_size, int out_size, int* bounds, int* coeffs, int cap);
 
 /* Per-launch device timing of the plan the LAST forward used: runs it `reps` more times with CUDA events around
  * every launch and writes a JSON array [{"i","kind","ms","flops","bytes","shape"}...] (algorithmic flops/bytes per
@@ -224,6 +250,9 @@ int i2it_op_upsample2x(i2it_handle* h, const void* x, int N, int H, int W, int C
 /* F.interpolate(size=(Ho, Wo), mode="nearest") */
 int i2it_op_upsample_to(i2it_handle* h, const void* x, int N, int H, int W, int C, int Ho, int Wo, void* out,
                         void* stream);
+/* LANCZOS resize of uint8 HWC images, bit-exact with PIL: x [B, H, W, 3] -> out [B, H2, W2, 3] (device pointers).
+ * The same passes as i2it_forward_u8_resize; an unchanged size is a device copy (no launch). */
+int i2it_op_resize_u8(i2it_handle* h, const void* x, int B, int H, int W, void* out, int H2, int W2, void* stream);
 
 #ifdef __cplusplus
 }
