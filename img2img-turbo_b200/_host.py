@@ -177,6 +177,9 @@ class NetHandle:
 class TurboBase(torch.nn.Module):
     """Common engine management for the two wrappers."""
     MODEL_KIND = i2it.PIX2PIX
+    # forward plans an engine keeps (least recently run evicted first): a demo or a folder loop over many image sizes stays
+    # bounded; an evicted size is rebuilt with identical outputs when it returns
+    MAX_PLANS = 16
 
     def _init_common(self, cfg, dtype, text_stack, use_cuda_graph=True, keep_stages=False):
         # I2IT_CFG=tiny: reduced-width network when the caller cannot pass `cfg` (e.g. an unmodified inference script under test);
@@ -246,7 +249,8 @@ class TurboBase(torch.nn.Module):
                 self._engine.close()
             te = self._text_encoder_spec()
             eng = i2it.Engine(self.compute_dtype, self.MODEL_KIND, cfg=self._cfg, keep_stages=self._keep_stages,
-                              use_cuda_graph=self._use_graph, **({"text_heads": te["heads"], "text_act": te["act"]} if te else {}))
+                              use_cuda_graph=self._use_graph, max_plans=self.MAX_PLANS,
+                              **({"text_heads": te["heads"], "text_act": te["act"]} if te else {}))
             eng.load_state_dict(self._sd)
             if te:      # the CLIP text tower runs on the engine too (SURVEY 8f #1): same tensors, transformers key names
                 eng.load_state_dict({"text_encoder." + k: v for k, v in self.text_encoder.state_dict().items()})
@@ -255,6 +259,12 @@ class TurboBase(torch.nn.Module):
                 eng.set_adapter_scale(name, s)
             self._engine, self._engine_key, self._final_key = eng, key, None
         return self._engine
+
+    def release_plans(self):
+        """Give back the device memory of every forward plan (the shared workspace included).  Weights, prompt caches and the
+        staging buffers stay; the next forward of each shape rebuilds its plan."""
+        if self._engine is not None:
+            self._engine.release_plans()
 
     def _finalize(self, lw_unet: float, lw_vae: float, gamma: float, twin_r: float):
         eng = self._get_engine()

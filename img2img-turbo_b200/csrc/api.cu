@@ -103,6 +103,31 @@ int i2it_workspace_bytes(i2it_handle* h, int batch, int H, int W, size_t* bytes)
   API_END
 }
 
+int i2it_set_max_plans(i2it_handle* h, int max_plans) {
+  API_BEGIN(h)
+  E.set_max_plans(max_plans);
+  API_END
+}
+
+int i2it_release_plans(i2it_handle* h) {
+  API_BEGIN(h)
+  E.release_plans();
+  API_END
+}
+
+int i2it_memory_stats_get(i2it_handle* h, i2it_memory_stats* s) {
+  API_BEGIN(h)
+  I2IT_CHECK(s != nullptr, "null out pointer");
+  *s = E.memory_stats();
+  API_END
+}
+
+int i2it_debug_poison_workspace(i2it_handle* h, int value) {
+  API_BEGIN(h)
+  E.poison_workspace(value);
+  API_END
+}
+
 int i2it_forward(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps,
                  const void* noise_map, float r, void* out, void* out_latent, int batch, int H, int W, int direction,
                  void* stream) {

@@ -61,6 +61,120 @@ CUtensorMap encode_tmap(const TmapSpec& s, int dtype) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// workspace arena (virtual memory management entry points fetched like cuTensorMapEncodeTiled)
+// ---------------------------------------------------------------------------------------------
+template <typename F> static F driver_fn(const char* name) {
+  void* p = nullptr;
+  cudaDriverEntryPointQueryResult q;
+  I2IT_CUDA(cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &q));
+  I2IT_CHECK(q == cudaDriverEntryPointSuccess && p != nullptr, std::string(name) + " unavailable in this driver");
+  return reinterpret_cast<F>(p);
+}
+
+struct Vmm {
+  decltype(&cuMemAddressReserve) reserve = driver_fn<decltype(&cuMemAddressReserve)>("cuMemAddressReserve");
+  decltype(&cuMemAddressFree) free = driver_fn<decltype(&cuMemAddressFree)>("cuMemAddressFree");
+  decltype(&cuMemGetAllocationGranularity) granularity =
+      driver_fn<decltype(&cuMemGetAllocationGranularity)>("cuMemGetAllocationGranularity");
+  decltype(&cuMemCreate) create = driver_fn<decltype(&cuMemCreate)>("cuMemCreate");
+  decltype(&cuMemRelease) release = driver_fn<decltype(&cuMemRelease)>("cuMemRelease");
+  decltype(&cuMemMap) map = driver_fn<decltype(&cuMemMap)>("cuMemMap");
+  decltype(&cuMemUnmap) unmap = driver_fn<decltype(&cuMemUnmap)>("cuMemUnmap");
+  decltype(&cuMemSetAccess) set_access = driver_fn<decltype(&cuMemSetAccess)>("cuMemSetAccess");
+};
+static const Vmm& vmm() {
+  static const Vmm v;
+  return v;
+}
+
+static void cu_check(CUresult r, const char* what, size_t bytes) {
+  if (r != CUDA_SUCCESS)
+    throw Error(std::string("workspace arena: ") + what + " of " + std::to_string(bytes) + " bytes failed (CUresult " +
+                std::to_string(static_cast<int>(r)) + ")");
+}
+
+static CUmemAllocationProp arena_prop(int device) {
+  CUmemAllocationProp prop;
+  std::memset(&prop, 0, sizeof prop);
+  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  prop.location.id = device;
+  return prop;
+}
+
+char* Arena::ptr() {
+  if (!base) {
+    const Vmm& v = vmm();
+    const CUmemAllocationProp prop = arena_prop(device);
+    cu_check(v.granularity(&gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM), "cuMemGetAllocationGranularity", 0);
+    size_t free_b = 0, total_b = 0;
+    I2IT_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const size_t size = round(total_b);     // no plan can need more than the device holds
+    cu_check(v.reserve(&base, size, 0, 0, 0), "cuMemAddressReserve", size);
+    reserved = size;
+  }
+  return reinterpret_cast<char*>(base);
+}
+
+void Arena::grow(size_t bytes) {
+  ptr();
+  const size_t target = round(bytes);
+  if (target <= mapped) return;
+  I2IT_CHECK(target <= reserved, "workspace arena: " + std::to_string(target) + " bytes exceed the device's memory");
+  const Vmm& v = vmm();
+  const size_t size = target - mapped;
+  const CUmemAllocationProp prop = arena_prop(device);
+  CUmemGenericAllocationHandle h;
+  cu_check(v.create(&h, size, &prop, 0), "cuMemCreate", size);
+  CUresult r = v.map(base + mapped, size, 0, h, 0);
+  if (r != CUDA_SUCCESS) { v.release(h); cu_check(r, "cuMemMap", size); }
+  CUmemAccessDesc acc;
+  std::memset(&acc, 0, sizeof acc);
+  acc.location = prop.location;
+  acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+  r = v.set_access(base + mapped, size, &acc, 1);
+  if (r != CUDA_SUCCESS) { v.unmap(base + mapped, size); v.release(h); cu_check(r, "cuMemSetAccess", size); }
+  chunks.push_back({mapped, size, h});
+  mapped = target;
+}
+
+void Arena::shrink(size_t bytes, size_t keep) {
+  if (!base) return;
+  const Vmm& v = vmm();
+  const size_t target = round(bytes);
+  auto drop_last = [&]() {
+    const Chunk c = chunks.back();
+    chunks.pop_back();
+    mapped = c.off;
+    cu_check(v.unmap(base + c.off, c.size), "cuMemUnmap", c.size);
+    cu_check(v.release(c.h), "cuMemRelease", c.size);
+  };
+  while (!chunks.empty() && chunks.back().off >= target) drop_last();
+  if (mapped > target && chunks.back().off >= keep) {   // re-create the straddling chunk at the new size
+    drop_last();
+    grow(target);
+  }
+}
+
+void Arena::fill(int value) {
+  if (!mapped) return;
+  I2IT_CUDA(cudaMemset(reinterpret_cast<void*>(base), value, mapped));
+  I2IT_CUDA(cudaDeviceSynchronize());
+}
+
+Arena::~Arena() {
+  if (!base) return;
+  try {
+    const Vmm& v = vmm();
+    for (auto it = chunks.rbegin(); it != chunks.rend(); ++it) {
+      v.unmap(base + it->off, it->size);
+      v.release(it->h);
+    }
+    v.free(base, reserved);
+  } catch (...) {}
+}
+
+// ---------------------------------------------------------------------------------------------
 // pool
 // ---------------------------------------------------------------------------------------------
 Pool::~Pool() {
@@ -76,8 +190,12 @@ void* Pool::get(size_t bytes, size_t* actual) {
     return p;
   }
   void* p = nullptr;
-  I2IT_CUDA(cudaMalloc(&p, bytes));
-  blocks.emplace_back(p, bytes);
+  if (arena) {
+    p = arena->ptr() + transient();      // the plan's new transient blocks tile [0, transient()) of the arena
+  } else {
+    I2IT_CUDA(cudaMalloc(&p, bytes));
+    blocks.emplace_back(p, bytes);
+  }
   total += bytes;
   *actual = bytes;
   return p;
@@ -89,6 +207,7 @@ void* Pool::get_fresh(size_t bytes) {
   I2IT_CUDA(cudaMalloc(&p, bytes));
   blocks.emplace_back(p, bytes);
   total += bytes;
+  persistent += bytes;
   return p;
 }
 
@@ -162,9 +281,12 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CUDA(cudaEventCreateWithFlags(&ev_in_, cudaEventDisableTiming));
   I2IT_CUDA(cudaEventCreateWithFlags(&ev_out_, cudaEventDisableTiming));
   encode_fn();
+  arena_.device = c.device;
 }
 
 Engine::~Engine() {
+  cudaSetDevice(cfg.device);
+  cudaDeviceSynchronize();          // graphs and the arena's mappings go below; neither waits for the device by itself
   plans_.clear();
   textkv_.clear();
   textenc_.clear();
@@ -182,6 +304,77 @@ void Engine::check_device_error() {
     throw Error("tapgemm watchdog tripped (pipeline stage code " + std::to_string(code) +
                 ": 1=producer/empty 2=producer/epilogue-done 3=consumer/full)");
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// image-forward plan cache
+// ---------------------------------------------------------------------------------------------
+void Engine::sync_plans() {
+  I2IT_CUDA(cudaStreamSynchronize(gstream_));   // graph replays
+  I2IT_CUDA(cudaDeviceSynchronize());           // eager forwards on the caller's stream
+}
+
+void Engine::trim_arena(bool keep_last) {
+  size_t need = 0;
+  for (const auto& kv : plans_) need = std::max(need, kv.second->pool.transient());
+  // the last forward's stages (i2it_read_stage) live in the arena: those bytes keep their contents unless a forward is about
+  // to overwrite them anyway
+  const size_t keep = (keep_last && last_plan_) ? last_plan_->pool.transient() : 0;
+  try {
+    arena_.shrink(need, keep);
+  } catch (...) {                               // the arena may now be smaller than the resident plans: drop them
+    plans_.clear();
+    last_plan_ = nullptr;
+    throw;
+  }
+}
+
+void Engine::evict_lru(const Plan* also_keep, bool keep_last) {
+  if (max_plans_ <= 0) return;
+  bool evicted = false;
+  while (static_cast<int>(plans_.size()) > max_plans_) {
+    auto victim = plans_.end();
+    for (auto it = plans_.begin(); it != plans_.end(); ++it) {
+      const Plan* p = it->second.get();
+      if (p == last_plan_ || p == also_keep) continue;
+      if (victim == plans_.end() || p->last_run < victim->second->last_run) victim = it;
+    }
+    if (victim == plans_.end()) break;
+    if (!evicted) sync_plans();
+    evicted = true;
+    plans_.erase(victim);
+    ++plan_evictions_;
+  }
+  if (evicted) trim_arena(keep_last);
+}
+
+void Engine::set_max_plans(int n) {
+  I2IT_CHECK(n >= 0, "max_plans must be >= 0 (0: no limit)");
+  max_plans_ = n;
+  evict_lru();
+}
+
+void Engine::release_plans() {
+  sync_plans();
+  plans_.clear();
+  last_plan_ = nullptr;
+  arena_.shrink(0, 0);
+}
+
+i2it_memory_stats Engine::memory_stats() const {
+  i2it_memory_stats s;
+  std::memset(&s, 0, sizeof s);
+  s.arena_bytes = arena_.mapped;
+  for (const auto& kv : plans_) s.plan_bytes += kv.second->pool.persistent;
+  s.plans = static_cast<int>(plans_.size());
+  s.plan_builds = plan_builds_;
+  s.plan_evictions = plan_evictions_;
+  return s;
+}
+
+void Engine::poison_workspace(int value) {
+  sync_plans();
+  arena_.fill(value);
 }
 
 void* Engine::dmalloc(size_t bytes) {
@@ -245,9 +438,9 @@ float Engine::adapter_weight(const std::string& name, const std::string& adapter
 }
 
 void Engine::finalize(float lw_unet, float lw_vae, float skip_gamma, float twin_r) {
-  I2IT_CUDA(cudaDeviceSynchronize());
+  sync_plans();
   lw_unet_ = lw_unet; lw_vae_ = lw_vae; skip_gamma_ = skip_gamma; twin_r_ = twin_r;
-  plans_.clear();
+  plans_.clear();                  // the arena stays mapped: the plans rebuilt with the new weights need the same bytes
   textkv_.clear();                 // cached cross-attention operands were projected with the old (LoRA-scaled) weights
   textenc_.clear();
   last_plan_ = nullptr;
@@ -1439,10 +1632,12 @@ void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int te
     // nothing to resize or crop: the plan (and its key) of the plain uint8 forward
     if (g->in_H == H && g->in_W == W && g->resize_H == H && g->resize_W == W && g->out_H == H && g->out_W == W) g = nullptr;
   }
-  Plan* P = plan_for(B, H, W, direction, text_batch, text_cached, io_mode, g);
+  Plan* P = plan_for(B, H, W, direction, text_batch, text_cached, io_mode, g, /*evict=*/false);
   if (io_mode & IO_U8_OUT) io.out = P->u8_out_tmp;
   P->io = io;
   last_plan_ = P;
+  P->last_run = ++tick_;
+  evict_lru(nullptr, /*keep_last=*/false);   // this forward rewrites the workspace: no byte of it needs to survive
   if (cfg.use_cuda_graph) {
     // replay on the engine's own stream, ordered after/before the caller's stream with events
     I2IT_CUDA(cudaEventRecord(ev_in_, st));

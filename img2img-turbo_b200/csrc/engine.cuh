@@ -30,16 +30,45 @@ struct TmapSpec {
 CUtensorMap encode_tmap(const TmapSpec& s, int dtype);
 
 // ---------------------------------------------------------------------------------------------
+// workspace arena: one reserved virtual address range per handle whose head is backed by physical memory (CUDA virtual memory
+// management).  Physical memory is mapped and unmapped at the tail only, so an address, once handed out, never moves: tensor
+// maps and captured graphs stay valid while the arena grows and shrinks.
+// ---------------------------------------------------------------------------------------------
+struct Arena {
+  int device = 0;
+  CUdeviceptr base = 0;
+  size_t reserved = 0, gran = 0, mapped = 0;
+  struct Chunk { size_t off, size; CUmemGenericAllocationHandle h; };
+  std::vector<Chunk> chunks;                 // physical allocations mapped back to back from `base`
+  ~Arena();
+  char* ptr();                               // base address (the range is reserved on first use)
+  size_t round(size_t bytes) const { return (bytes + gran - 1) / gran * gran; }
+  void grow(size_t bytes);                   // map [mapped, round(bytes)); throws with the old mapping intact
+  // unmap down to round(bytes); the first `keep` bytes keep their contents (a chunk straddling the new end is re-created
+  // smaller only when none of its bytes lie below `keep`).  Callers synchronise the device first.
+  void shrink(size_t bytes, size_t keep);
+  void fill(int value);                      // memset every mapped byte (synchronous)
+};
+
+// ---------------------------------------------------------------------------------------------
 // workspace pool (plan-build time only; execution never allocates)
 // ---------------------------------------------------------------------------------------------
 struct Pool {
-  std::vector<std::pair<void*, size_t>> blocks;
+  std::vector<std::pair<void*, size_t>> blocks;   // cudaMalloc'd blocks, freed with the pool
   std::multimap<size_t, void*> free_;
-  size_t total = 0;
+  size_t total = 0;                // transient + persistent bytes
+  size_t persistent = 0;           // get_fresh bytes
+  // Transient blocks (get) are recycled by build-order liveness and written by every forward before it reads them.  With an
+  // arena they are offsets from its base, shared with every other plan of the handle (whose forwards never overlap); the
+  // arena maps them when the plan is complete (Engine::plan_for).  Without one, each is its own cudaMalloc.
+  Arena* arena = nullptr;
   ~Pool();
   void* get(size_t bytes, size_t* actual);
-  void* get_fresh(size_t bytes);   // never recycled (zero-padded small-channel tensors must stay clean at run time)
+  // never recycled and never in the arena: state written at build time or kept between replays (zero-padded small-channel
+  // tensors, GroupNorm tickets, resample tables)
+  void* get_fresh(size_t bytes);
   void put(void* p, size_t bytes) { free_.emplace(bytes, p); }
+  size_t transient() const { return total - persistent; }
 };
 
 // GroupNorm partial statistics written by the epilogue of the GEMM that PRODUCED a tensor (see TapGemmParams::gn_part):
@@ -130,6 +159,7 @@ struct Plan {
   std::vector<Trace> traces;                           // I2IT_TRACE=1 only
   std::vector<std::shared_ptr<void>> keep;
   std::vector<int> key;                                // (B, H, W, direction, text_batch, text_cached, io_mode[, resize geometry])
+  unsigned long long last_run = 0;                     // engine tick of the last forward (or the build): LRU eviction order
   void* u8_out_tmp = nullptr;                          // NCHW image the last conv writes when the caller wants uint8 HWC
   int* gn_counter = nullptr;                           // per-image tickets of the GroupNorm last-block reductions (zero between launches)
   std::vector<std::pair<size_t, const char*>> ranges;  // (first op index, name): NVTX stage ranges of the eager path
@@ -185,8 +215,9 @@ class Engine {
   void set_adapter_scale(const std::string& a, float s) { adapter_scale_[a] = s; }
   void finalize(float lw_unet, float lw_vae, float skip_gamma, float twin_r);
   // g: LANCZOS resize geometry of a uint8 forward (i2it_forward_u8_resize); part of the plan key
+  // evict: enforce the plan limit once the plan is in (forward() does it itself after the plan becomes the last-run one)
   Plan* plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached = false, int io_mode = 0,
-                 const i2it_resize_desc* g = nullptr);
+                 const i2it_resize_desc* g = nullptr, bool evict = true);
   void forward(const IO& io, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
                const i2it_resize_desc* g = nullptr);
   // cross-attention K / V^T of the prompt, computed once per prompt (i2it_set_text) instead of once per forward
@@ -195,6 +226,11 @@ class Engine {
   void encode_text(const int* tokens, int batch, void* out, cudaStream_t st);
   bool has_text_encoder() const { return has("text_encoder.text_model.embeddings.token_embedding.weight"); }
   Plan* last_plan() const { return last_plan_; }
+  // ---- image-forward plan cache: transient buffers of every plan share one arena; plans are evicted least recently run ----
+  void set_max_plans(int n);                                          // 0: no limit
+  void release_plans();                                               // drop every image-forward plan, unmap the arena
+  i2it_memory_stats memory_stats() const;
+  void poison_workspace(int value);                                   // memset every mapped arena byte (tests)
   void read_stage(const std::string& name, float* dst, size_t dst_elems, int dims[4]);
   std::string stage_names_json(bool text = false) const;             // last forward's (text: last encode_text's) stages
   std::string prepared_keys_json() const;                            // every prepared-weight cache key, sorted
@@ -306,6 +342,14 @@ class Engine {
                      const float* b1 = nullptr, float c1 = 0.f);
   std::map<int, std::unique_ptr<struct TextKV>> textkv_;   // by text_batch
   std::map<int, std::unique_ptr<Plan>> textenc_;            // CLIP text tower plans, by batch
+  Arena arena_;                                             // declared before plans_: outlives them
+  int max_plans_ = 0;
+  unsigned long long tick_ = 0;
+  int plan_builds_ = 0, plan_evictions_ = 0;
+  void sync_plans();                                        // gstream_ and the device: before a plan dies or memory unmaps
+  // down to max_plans_, never the last-run plan; keep_last: the last forward's workspace bytes keep their contents
+  void evict_lru(const Plan* also_keep = nullptr, bool keep_last = true);
+  void trim_arena(bool keep_last);                          // unmap what no resident plan needs
   std::map<std::vector<int>, std::unique_ptr<Plan>> plans_;
   Plan* last_plan_ = nullptr;
   Plan* last_text_plan_ = nullptr;   // the plan of the last encode_text (its stages: i2it_text_stage_names)

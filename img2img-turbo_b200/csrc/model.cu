@@ -490,7 +490,7 @@ void Engine::resample_u8(Plan& P, const U8View& src, int B, int inH, int inW, in
 }
 
 Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached, int io_mode,
-                       const i2it_resize_desc* g) {
+                       const i2it_resize_desc* g, bool evict) {
   std::vector<int> key{B, H, W, direction, text_batch, text_cached ? 1 : 0, io_mode};
   if (g) key.insert(key.end(), {g->in_H, g->in_W, g->resize_H, g->resize_W, g->crop_y, g->crop_x, g->out_H, g->out_W});
   auto it = plans_.find(key);
@@ -501,6 +501,7 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
   std::unique_ptr<Plan> up(new Plan());
   Plan& P = *up;
   P.key = key;
+  P.pool.arena = &arena_;      // transient buffers alias those of the handle's other forward plans
   // a build that throws must not leave engine members pointing into the dying plan's pool (text_ holds a pool block):
   // declared after `up`, so it runs before the plan is destroyed
   struct BuildGuard {
@@ -589,9 +590,15 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
   flush_prep();                             // every weight of the plan: one fold/re-layout launch (+ the time-embedding GEMVs)
   I2IT_CUDA(cudaDeviceSynchronize());       // weight preparation ran on the default stream
   I2IT_CUDA(cudaGetLastError());
+  // back the plan's transient bytes before it can run; a failed mapping throws here, before the plan is inserted, and
+  // leaves the arena and the resident plans as they were
+  arena_.grow(P.pool.transient());
+  P.last_run = ++tick_;
   Plan* raw_plan = up.get();
   plans_[key] = std::move(up);
   guard.ok = true;
+  ++plan_builds_;
+  if (evict) evict_lru(raw_plan);
   return raw_plan;
 }
 

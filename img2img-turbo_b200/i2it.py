@@ -32,6 +32,7 @@ SYMBOLS = [
     "i2it_op_attention", "i2it_op_upsample2x", "i2it_op_conv2d_ex", "i2it_op_launches", "i2it_op_vt_proj",
     "i2it_op_upsample_to", "i2it_stage_names", "i2it_prepared_keys", "i2it_read_prepared", "i2it_text_stage_names",
     "i2it_forward_u8_resize", "i2it_op_resize_u8", "i2it_debug_resample_coeffs",
+    "i2it_set_max_plans", "i2it_release_plans", "i2it_memory_stats_get", "i2it_debug_poison_workspace",
 ]
 TEXT_TOKEN_EMB = "text_encoder.text_model.embeddings.token_embedding.weight"
 TEXT_POS_EMB = "text_encoder.text_model.embeddings.position_embedding.weight"
@@ -95,6 +96,14 @@ def resample_coeffs(in_size: int, out_size: int):
         [list(coeffs[i * ksize: (i + 1) * ksize]) for i in range(out_size)]
 
 
+class MemoryStats(C.Structure):
+    """i2it_memory_stats (include/i2it.h)."""
+    _fields_ = [
+        ("arena_bytes", C.c_size_t), ("plan_bytes", C.c_size_t), ("plans", C.c_int),
+        ("plan_builds", C.c_int), ("plan_evictions", C.c_int),
+    ]
+
+
 class Config(C.Structure):
     _fields_ = [
         ("dtype", C.c_int), ("model_kind", C.c_int), ("device", C.c_int),
@@ -156,6 +165,10 @@ def load_library(path: Optional[str] = None):
     lib.i2it_forward_u8_resize.argtypes = [vp, vp, ci, C.POINTER(ResizeDesc), vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci, vp]
     lib.i2it_op_resize_u8.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci, vp]
     lib.i2it_debug_resample_coeffs.argtypes = [ci, ci, C.POINTER(ci), C.POINTER(ci), ci]
+    lib.i2it_set_max_plans.argtypes = [vp, ci]
+    lib.i2it_release_plans.argtypes = [vp]
+    lib.i2it_memory_stats_get.argtypes = [vp, C.POINTER(MemoryStats)]
+    lib.i2it_debug_poison_workspace.argtypes = [vp, ci]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("i2it_destroy", "i2it_last_error"):
@@ -177,7 +190,7 @@ class Engine:
 
     def __init__(self, dtype: torch.dtype = torch.bfloat16, model_kind: int = PIX2PIX, cfg: Optional[dict] = None,
                  device: Optional[int] = None, keep_stages: int = 0, use_cuda_graph: bool = True,
-                 text_heads: int = 0, text_act: str = "gelu"):
+                 text_heads: int = 0, text_act: str = "gelu", max_plans: int = 0):
         if not torch.cuda.is_available():
             raise RuntimeError("libi2it needs a CUDA device (H100 / sm_90a); no CPU fallback exists")
         self.lib = load_library()
@@ -205,6 +218,8 @@ class Engine:
         rc = self.lib.i2it_create(C.byref(c), C.byref(self._h))
         if rc != 0:
             raise RuntimeError("i2it_create failed: " + self.lib.i2it_last_error(C.c_void_p(0)).decode())
+        if max_plans:
+            self.set_max_plans(max_plans)
 
     def _check(self, rc: int, what: str):
         if rc != 0:
@@ -350,6 +365,27 @@ class Engine:
         n = C.c_size_t(0)
         self._check(self.lib.i2it_workspace_bytes(self._h, B, H, W, C.byref(n)), "i2it_workspace_bytes")
         return n.value
+
+    # ---- plan cache ------------------------------------------------------------------------------
+    def set_max_plans(self, max_plans: int):
+        """Keep at most `max_plans` forward plans (0: no limit); the least recently run one is evicted first and rebuilt,
+        with identical outputs, when its shape returns.  The last forward's plan is never evicted."""
+        self._check(self.lib.i2it_set_max_plans(self._h, int(max_plans)), "i2it_set_max_plans")
+
+    def release_plans(self):
+        """Drop every forward plan and unmap the shared workspace (prepared weights and the set_text cache are kept)."""
+        self._check(self.lib.i2it_release_plans(self._h), "i2it_release_plans")
+
+    def memory_stats(self) -> dict:
+        """{"arena_bytes", "plan_bytes", "plans", "plan_builds", "plan_evictions"}: the workspace shared by the forward plans,
+        the plans' own persistent bytes, the resident plans and the build / eviction counters."""
+        s = MemoryStats()
+        self._check(self.lib.i2it_memory_stats_get(self._h, C.byref(s)), "i2it_memory_stats_get")
+        return {name: getattr(s, name) for name, _ in MemoryStats._fields_}
+
+    def _debug_poison_workspace(self, value: int = 0xFF):
+        """Fill the shared workspace with `value` (tests: no forward may read workspace it did not write)."""
+        self._check(self.lib.i2it_debug_poison_workspace(self._h, int(value)), "i2it_debug_poison_workspace")
 
     def read_stage(self, name: str, max_elems: int = 1 << 26, image: Optional[int] = None) -> torch.Tensor:
         """fp32 NCHW copy of a named stage of the last forward (keep_stages engines); image=i reads one image of the batch."""

@@ -89,8 +89,31 @@ int i2it_finalize_weights(i2it_handle* h, float lora_weight_unet, float lora_wei
                           float twin_r);
 
 /* Bytes of device workspace the engine holds for a (batch, H, W) forward: the last forward's plan when it has this shape,
- * else the plan is built.  Every buffer grows linearly in H*W (the VAE attention runs fused above 8192 tokens). */
+ * else the plan is built.  Every buffer grows linearly in H*W (the VAE attention runs fused above 8192 tokens).
+ * The count is the plan's own need, transient plus persistent bytes: its transient part lives in the arena the handle's
+ * forward plans share (i2it_memory_stats_get).  Building a plan here never evicts the last forward's plan. */
 int i2it_workspace_bytes(i2it_handle* h, int batch, int H, int W, size_t* bytes);
+
+/* Keep at most max_plans image-forward plans (0 = no limit, the default); the least recently run plan is evicted first and
+ * rebuilt, bit-identically, when its key returns.  The plan of the last forward is never evicted.  Evicting synchronises
+ * the device. */
+int i2it_set_max_plans(i2it_handle* h, int max_plans);
+
+/* Drop every image-forward plan and its graphs and unmap the shared workspace.  Prepared weights, the i2it_set_text cache and
+ * the text-tower plans are kept.  Synchronous. */
+int i2it_release_plans(i2it_handle* h);
+
+typedef struct i2it_memory_stats {
+  size_t arena_bytes;        /* physical bytes mapped for the transient workspace shared by all forward plans */
+  size_t plan_bytes;         /* persistent per-plan bytes, summed over resident plans */
+  int plans;                 /* resident image-forward plans */
+  int plan_builds, plan_evictions;   /* counters since create */
+} i2it_memory_stats;
+int i2it_memory_stats_get(i2it_handle* h, i2it_memory_stats* s);
+
+/* Test hook: memset every mapped arena byte to `value` (synchronous).  A forward must not read transient workspace it did not
+ * write itself, so poisoning between forwards must leave every output unchanged. */
+int i2it_debug_poison_workspace(i2it_handle* h, int value);
 
 /* The fused hot path.  All pointers are DEVICE pointers in the handle dtype, NCHW contiguous:
  *   x        [batch, 3, H, W]          control image / input image (fed to the VAE as is)
@@ -106,8 +129,11 @@ int i2it_workspace_bytes(i2it_handle* h, int batch, int H, int W, size_t* bytes)
  * (src/pix2pix_turbo.py:162,200-201: 1-D timesteps), three activation-dtype roundings for I2IT_CYCLEGAN
  * (src/cyclegan_turbo.py:205: 0-dim timestep).
  * H and W must be multiples of 8.  4032x3024 (12 MP) at batch 1 runs on one 80 GB H100 (measured workspace and time
- * in DESIGN section 8).  Each (batch, H, W) keeps its own plan and workspace for the handle's lifetime.
- * `stream` is a cudaStream_t. */
+ * in DESIGN section 8).  Each forward key (batch, H, W, direction, text mode, io mode, resize geometry) has its own plan.
+ * The transient workspace of all of a handle's forward plans is one shared arena, sized by the largest resident plan;
+ * each plan also holds a few small persistent buffers of its own.  Plans stay until i2it_finalize_weights,
+ * i2it_release_plans or an eviction under i2it_set_max_plans; an evicted plan is rebuilt, bit-identically, when its key
+ * returns.  `stream` is a cudaStream_t. */
 int i2it_forward(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps,
                  const void* noise_map, float r, void* out, void* out_latent, int batch, int H, int W,
                  int direction, void* stream);
