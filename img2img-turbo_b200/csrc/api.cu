@@ -308,6 +308,7 @@ int i2it_op_conv2d_ex(i2it_handle* h, const i2it_conv_desc* d, void* stream) {
   E.finalize(1.f, 1.f, 1.f, -1.f);
   {
     Plan P;
+    P.debug_tapgemm = true;
     // Ho = ceil(H / stride): Engine::conv pads an odd map to even before a stride-2 conv
     const int Ho = d->up2x ? 2 * d->H : (d->H + stride - 1) / stride, Wo = d->up2x ? 2 * d->W : (d->W + stride - 1) / stride;
     Act xin = view(d->x, d->N, d->H, d->W, d->Cin, d->ldx);
@@ -402,6 +403,7 @@ int i2it_op_attention(i2it_handle* h, const void* q, int ldq, const void* k, int
   I2IT_CHECK(!causal || (d == FA_D && E.use_flash), "i2it_op_attention: causal attention runs on the flash path (d = 64)");
   {
     Plan P;
+    P.debug_tapgemm = true;
     const int C = heads * d;
     const Act qa = view(q, B, 1, Nq, C, ldq), ka = view(k, kv_batch, 1, Nk, C, ldk), va = view(vt, kv_batch, 1, C, ldv, ldv);
     Act o = causal ? E.flash_attention(P, qa, ka, va, B, Nq, Nk, heads, kv_batch, true)
@@ -421,6 +423,7 @@ int i2it_op_vt_proj(i2it_handle* h, const void* x, int B, int ntok, int Cin, int
   E.finalize(1.f, 1.f, 1.f, -1.f);
   {
     Plan P;
+    P.debug_tapgemm = true;
     const PW pw = E.prep("__op.vt", {"__op.vt"});
     const Act vt = E.vt_proj(P, view(x, 1, 1, B * ntok, Cin, ldx), B, ntok, pw);
     E.copy_channels(P, vt, view(out, B, 1, Cout, vt.C, vt.C));
@@ -448,6 +451,13 @@ int i2it_op_upsample_to(i2it_handle* h, const void* x, int N, int H, int W, int 
     E.copy_channels(P, y, view(out, N, Ho, Wo, C, C));
     run_plan(h, P, static_cast<cudaStream_t>(stream));
   }
+  API_END
+}
+
+int i2it_debug_tapgemm_override(i2it_handle* h, int bn, int stages, int grid) {
+  API_BEGIN(h)
+  I2IT_CHECK(bn >= 0 && stages >= 0 && grid >= 0, "i2it_debug_tapgemm_override: values must be >= 0 (0: the engine's choice)");
+  E.dbg_bn = bn; E.dbg_stages = stages; E.dbg_grid = grid;
   API_END
 }
 

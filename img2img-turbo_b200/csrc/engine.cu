@@ -762,6 +762,19 @@ int Engine::pick_bn(long long m_tiles, int N, int step) const {
   return best;
 }
 
+int Engine::plan_bn(const Plan& P, long long m_tiles, int N, int step) const {
+  if (!P.debug_tapgemm || dbg_bn == 0) return pick_bn(m_tiles, N, step);
+  const int hi = round_up(N, 16);
+  if (tapgemm_for<__half>(false, dbg_bn) == nullptr || dbg_bn > hi) {
+    std::string legal;
+#define TG_LIST(n) if (n <= hi) legal += (legal.empty() ? "" : ", ") + std::to_string(n);
+    TG_BN_FULL(TG_LIST)
+#undef TG_LIST
+    throw Error("tapgemm override: BN=" + std::to_string(dbg_bn) + " is illegal for N=" + std::to_string(N) + "; legal: " + legal);
+  }
+  return dbg_bn;
+}
+
 // The TMA-store epilogue handles 16-bit row-major outputs whose channel count and tile width are whole 64-column rounds (128
 // accumulator columns for GEGLU) with 16-byte aligned rows; everything else keeps per-thread stores.
 bool Engine::tma_eligible(const TapGemmParams& p, bool out_from_io) const {
@@ -804,17 +817,30 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
     p.ostg2 = (use_ostg2 && p.tma_out && ksteps <= 48 && (budget - TG_OSTG_BYTES) / per >= 4) ? 1 : 0;
     if (p.ostg2) budget -= TG_OSTG_BYTES;
     p.stages = std::max(2, std::min(TG_MAX_STAGES, budget / per));
+    if (P.debug_tapgemm && dbg_stages) {
+      I2IT_CHECK(dbg_stages >= 2 && dbg_stages <= p.stages, "tapgemm override: stages=" + std::to_string(dbg_stages) +
+                                                               " is illegal for " + kind + " BN=" + std::to_string(p.BN) +
+                                                               "; legal: 2.." + std::to_string(p.stages));
+      p.stages = dbg_stages;
+    }
   }
   const CUtensorMap ta = encode_tmap(sa, dtype), tb = encode_tmap(sb, dtype);
   const CUtensorMap ta2 = sa2p ? encode_tmap(*sa2p, dtype) : ta, tb2 = sb2p ? encode_tmap(sb2, dtype) : tb;
   const int dt = dtype;
   Plan* plan = &P;
   const double m_valid = 1.0 * p.ext[0] * p.ext[1] * p.ext[2] * p.ext[3];
-  const int grid = static_cast<int>(std::min<long long>(total_tiles, num_sms));
-  char shp[160];
-  snprintf(shp, sizeof shp, "M=%.0f N=%d K=%.0f taps=%d BN=%d tiles=%lld grid=%d st=%d%s%s", m_valid, p.N, k_valid, p.num_taps, p.BN,
-           total_tiles, grid, p.stages, p.tma_out ? (p.ostg2 ? " tma2" : " tma") : "",
-           (p.gn_part && p.tma_out) ? " gn" : "");
+  const int max_grid = static_cast<int>(std::min<long long>(total_tiles, num_sms));
+  int grid = max_grid;
+  if (P.debug_tapgemm && dbg_grid) {
+    I2IT_CHECK(dbg_grid <= max_grid, "tapgemm override: grid=" + std::to_string(dbg_grid) + " is illegal for " + kind + " with " +
+                                         std::to_string(total_tiles) + " tiles; legal: 1.." + std::to_string(max_grid));
+    grid = dbg_grid;
+  }
+  const bool lean = use_lean && p.tma_out && p.act == TG_ACT_NONE;      // the epilogue variant without activation / direct-store code
+  char shp[168];
+  snprintf(shp, sizeof shp, "M=%.0f N=%d K=%.0f taps=%d BN=%d tiles=%lld grid=%d st=%d%s%s%s", m_valid, p.N, k_valid, p.num_taps,
+           p.BN, total_tiles, grid, p.stages, p.tma_out ? (p.ostg2 ? " tma2" : " tma") : "",
+           (p.gn_part && p.tma_out) ? " gn" : "", lean ? " lean" : "");
   // TMA-store epilogue: the output tensor map has the tile's row dims (extents = logical extents, so ragged edges are clipped
   // by the hardware) and a box of 64 columns x the 32 rows one epilogue warp owns
   if (!p.tma_out) p.gn_part = nullptr;
@@ -850,7 +876,6 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
     p.gn_shift = 0;
     while ((1 << p.gn_shift) < p.gn_red) ++p.gn_shift;
   }
-  const bool lean = use_lean && p.tma_out && p.act == TG_ACT_NONE;      // the epilogue variant without activation / direct-store code
   I2IT_CHECK(tapgemm_for<__half>(lean, p.BN) != nullptr, "tapgemm: no kernel instantiated for BN=" + std::to_string(p.BN));
   add_op(P, [ta, tb, ta2, tb2, to, p, grid, dt, out_from_io, plan, lean](cudaStream_t st) {
     TapGemmParams q = p;
@@ -990,7 +1015,7 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
     // whole 64-column store rounds (128 accumulator columns for GEGLU) when the output can take the TMA-store epilogue
     const int acols = (o.act == TG_ACT_GEGLU) ? 128 : 64;
     const bool rounds = use_tmaout && !o.to_io_out_nchw && !o.out_fp32 && gemm_n % acols == 0 && (ldo % 8) == 0;
-    p.BN = pick_bn(m_tiles, gemm_n, rounds ? acols : 0);
+    p.BN = plan_bn(P, m_tiles, gemm_n, rounds ? acols : 0);
   }
   p.n_tiles = ceil_div(gemm_n, p.BN);
   sb.box[0] = 64; sb.box[1] = p.BN; sb.box[2] = 1; sb.box[3] = 1; sb.box[4] = 1;
@@ -1302,7 +1327,7 @@ Act Engine::vt_proj(Plan& P, const Act& x, int B, int ntok, const PW& wv) {
   p.b_mul[0] = 0; p.b_mul[1] = 1; p.b_mul[2] = 0;
   const long long m_tiles = 1ll * p.tdim[0] * B;
   p.N = ntok;
-  p.BN = pick_bn(m_tiles, ntok, false);
+  p.BN = plan_bn(P, m_tiles, ntok, false);
   p.n_tiles = ceil_div(ntok, p.BN);
   sb.box[0] = 64; sb.box[1] = p.BN;
   p.num_taps = 1;
@@ -1358,7 +1383,7 @@ Act Engine::attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B,
     p.b_mul[0] = 1; p.b_mul[1] = kvb; p.b_mul[2] = 0;
     const long long m_tiles = 1ll * p.tdim[0] * heads * B;
     p.N = Nk;
-    p.BN = pick_bn(m_tiles, Nk, false);
+    p.BN = plan_bn(P, m_tiles, Nk, false);
     p.n_tiles = ceil_div(Nk, p.BN);
     sb.box[0] = 64; sb.box[1] = p.BN;
     p.num_taps = 1;

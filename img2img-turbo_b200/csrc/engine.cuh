@@ -163,6 +163,7 @@ struct Plan {
   void* u8_out_tmp = nullptr;                          // NCHW image the last conv writes when the caller wants uint8 HWC
   int* gn_counter = nullptr;                           // per-image tickets of the GroupNorm last-block reductions (zero between launches)
   std::vector<std::pair<size_t, const char*>> ranges;  // (first op index, name): NVTX stage ranges of the eager path
+  bool debug_tapgemm = false;                          // a diagnostic op plan: its tapgemm launches take the engine's dbg_* override
   IO io;
   std::vector<std::pair<IO, cudaGraphExec_t>> graphs;  // small cache: one instantiated graph per distinct IO pointer set
   ~Plan() { for (auto& g : graphs) cudaGraphExecDestroy(g.second); }
@@ -317,6 +318,9 @@ class Engine {
   std::string profile_json(int reps, cudaStream_t st);
   void dump_trace(Plan& P, cudaStream_t st);
   int pick_bn(long long m_tiles, int N, int step) const;   // step 64 / 128: BN restricted to multiples (TMA-store rounds)
+  // pick_bn, or the forced width of i2it_debug_tapgemm_override in a diagnostic op plan
+  int plan_bn(const Plan& P, long long m_tiles, int N, int step) const;
+  int dbg_bn = 0, dbg_stages = 0, dbg_grid = 0;            // i2it_debug_tapgemm_override (0: the engine's choice)
 
   int* d_err = nullptr;      // device alias of a mapped host word written by the tapgemm watchdog
   int* err_host_ = nullptr;

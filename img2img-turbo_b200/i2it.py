@@ -33,6 +33,7 @@ SYMBOLS = [
     "i2it_op_upsample_to", "i2it_stage_names", "i2it_prepared_keys", "i2it_read_prepared", "i2it_text_stage_names",
     "i2it_forward_u8_resize", "i2it_op_resize_u8", "i2it_debug_resample_coeffs",
     "i2it_set_max_plans", "i2it_release_plans", "i2it_memory_stats_get", "i2it_debug_poison_workspace",
+    "i2it_debug_tapgemm_override",
 ]
 TEXT_TOKEN_EMB = "text_encoder.text_model.embeddings.token_embedding.weight"
 TEXT_POS_EMB = "text_encoder.text_model.embeddings.position_embedding.weight"
@@ -169,6 +170,7 @@ def load_library(path: Optional[str] = None):
     lib.i2it_release_plans.argtypes = [vp]
     lib.i2it_memory_stats_get.argtypes = [vp, C.POINTER(MemoryStats)]
     lib.i2it_debug_poison_workspace.argtypes = [vp, ci]
+    lib.i2it_debug_tapgemm_override.argtypes = [vp, ci, ci, ci]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("i2it_destroy", "i2it_last_error"):
@@ -386,6 +388,12 @@ class Engine:
     def _debug_poison_workspace(self, value: int = 0xFF):
         """Fill the shared workspace with `value` (tests: no forward may read workspace it did not write)."""
         self._check(self.lib.i2it_debug_poison_workspace(self._h, int(value)), "i2it_debug_poison_workspace")
+
+    def _debug_tapgemm_override(self, bn: int = 0, stages: int = 0, grid: int = 0):
+        """Force tapgemm's tile width, ring depth and persistent grid in the op_* calls that follow (0: the engine's choice;
+        forward plans never read it).  An op whose launch cannot take a value raises with the legal range."""
+        self._check(self.lib.i2it_debug_tapgemm_override(self._h, int(bn), int(stages), int(grid)),
+                    "i2it_debug_tapgemm_override")
 
     def read_stage(self, name: str, max_elems: int = 1 << 26, image: Optional[int] = None) -> torch.Tensor:
         """fp32 NCHW copy of a named stage of the last forward (keep_stages engines); image=i reads one image of the batch."""

@@ -279,6 +279,12 @@ int i2it_op_upsample_to(i2it_handle* h, const void* x, int N, int H, int W, int 
 /* LANCZOS resize of uint8 HWC images, bit-exact with PIL: x [B, H, W, 3] -> out [B, H2, W2, 3] (device pointers).
  * The same passes as i2it_forward_u8_resize; an unchanged size is a device copy (no launch). */
 int i2it_op_resize_u8(i2it_handle* h, const void* x, int B, int H, int W, void* out, int H2, int W2, void* stream);
+/* Test hook: force tapgemm's tile width, ring depth and persistent grid in the plans of the i2it_op_* calls made after it
+ * (forward, encode_text and set_text plans never read it).  0 keeps the engine's choice.  bn replaces pick_bn's width (one of
+ * 16, 32, 48, 64, 80, 96, 112, 128, 160, 192, 224, 256, at most round_up(N, 16)); launches that fix their width themselves
+ * (split-K: 256, the P V GEMM: the head dim) keep it.  stages: 2 .. the ring depth the launch would get; grid: 1 .. min(tiles,
+ * SMs).  Each applies to every tapgemm launch of the op; an op whose launch cannot take a value fails with the legal range. */
+int i2it_debug_tapgemm_override(i2it_handle* h, int bn, int stages, int grid);
 
 #ifdef __cplusplus
 }
