@@ -342,17 +342,20 @@ class TurboBase(torch.nn.Module):
         rs, cr, out = i2it.resize_geometry((shape[1], shape[2]), resize, crop, out_size)
         return cr[2], cr[3], {"resize": rs, "crop": cr, "out_size": out}
 
-    def _staged_forward(self, eng, x, text, eps, noise=None, r=1.0, direction=i2it.A2B, u8_mode=None, geometry=None):
+    def _staged_forward(self, eng, x, text, eps, noise=None, r=1.0, direction=i2it.A2B, u8_mode=None, geometry=None,
+                        variations=False):
         """Run the engine through persistent device staging buffers (per shape/dtype): the captured CUDA graph bakes the IO
         pointers in, so stable addresses mean every call replays the same graph.  Costs two small device-to-device copies;
         the result is returned in a fresh tensor (never aliased across calls).  The text embedding is not an input of the
-        graph: its projections are cached on the engine (_bind_text).  `geometry`: forward_u8 resize keywords."""
+        graph: its projections are cached on the engine (_bind_text).  `geometry`: forward_u8 resize keywords.
+        variations: x is one image and the eps.shape[0] outputs are its variations (forward_variations)."""
         self._bind_text(eng, text)
         gkey = tuple(sorted(geometry.items())) if geometry else None
-        key = (tuple(x.shape), x.dtype, eps.dtype, noise is not None, _cur_dev(), gkey)
+        n = eps.shape[0] if variations else x.shape[0]
+        key = (tuple(x.shape), x.dtype, eps.dtype, noise is not None, _cur_dev(), gkey) + ((n,) if variations else ())
         st = self.__dict__.setdefault("_stage", {}).get(key)
         if st is None:
-            out = torch.empty_like(x) if geometry is None else x.new_empty((x.shape[0],) + geometry["out_size"] + (3,))
+            out = x.new_empty((n,) + tuple(x.shape[1:]) if geometry is None else (n,) + geometry["out_size"] + (3,))
             st = {"x": torch.empty_like(x), "eps": torch.empty_like(eps), "out": out,
                   "noise": torch.empty_like(eps) if noise is not None else None}
             if len(self._stage) > 8:
@@ -363,11 +366,28 @@ class TurboBase(torch.nn.Module):
         if noise is not None:
             st["noise"].copy_(noise, non_blocking=True)
         if u8_mode is None:
-            eng.forward(st["x"], None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction, out=st["out"])
+            fwd = eng.forward_variations if variations else eng.forward
+            fwd(st["x"], None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction, out=st["out"])
         else:
-            eng.forward_u8(st["x"], u8_mode, None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction, out=st["out"],
-                           **(geometry or {}))
+            fwd = eng.forward_u8_variations if variations else eng.forward_u8
+            fwd(st["x"], u8_mode, None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction, out=st["out"],
+                **(geometry or {}))
         return st["out"].clone()
+
+    @staticmethod
+    def _variation_count(n, text, noise_map, eps) -> int:
+        """n of a variations call: from n=, eps, a noise_map or prompt batch other than 1 (a batch of 1 is shared by all
+        variations); every one of them that is given must agree.  1 when none is."""
+        got = {"n": n, "eps": None if eps is None else eps.shape[0],
+               "noise_map": noise_map.shape[0] if noise_map is not None and noise_map.shape[0] != 1 else None,
+               "prompt": text.shape[0] if text.shape[0] != 1 else None}
+        got = {k: int(v) for k, v in got.items() if v is not None}
+        if len(set(got.values())) > 1:
+            raise ValueError(f"the number of variations differs between arguments: {got}")
+        n = next(iter(got.values()), 1)
+        if n < 1:
+            raise ValueError(f"the number of variations must be >= 1, got {n}")
+        return n
 
     @staticmethod
     def _prep(t: Optional[torch.Tensor], dtype) -> Optional[torch.Tensor]:

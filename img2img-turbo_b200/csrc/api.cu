@@ -184,6 +184,35 @@ int i2it_forward_u8_resize(i2it_handle* h, const void* x_u8_hwc, int in_mode, co
   API_END
 }
 
+int i2it_forward_variations(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps,
+                            const void* noise_map, float r, void* out, void* out_latent, int n, int H, int W, int direction,
+                            void* stream) {
+  API_BEGIN(h)
+  I2IT_CHECK(n >= 1, "i2it_forward_variations: n must be >= 1");
+  IO io;
+  std::memset(&io, 0, sizeof io);
+  io.x = x; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r; io.out = out; io.out_latent = out_latent;
+  E.check_device_error();
+  E.forward(io, n, H, W, direction, text_batch, static_cast<cudaStream_t>(stream), nullptr, /*shared_input=*/true);
+  API_END
+}
+
+int i2it_forward_u8_variations(i2it_handle* h, const void* x_u8_hwc, int in_mode, const i2it_resize_desc* g, const void* text_emb,
+                               int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc,
+                               void* out_latent, int n, int H, int W, int direction, void* stream) {
+  API_BEGIN(h)
+  I2IT_CHECK(n >= 1, "i2it_forward_u8_variations: n must be >= 1");
+  I2IT_CHECK(in_mode >= 0 && in_mode <= 2, "i2it_forward_u8_variations: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
+  I2IT_CHECK(x_u8_hwc && out_u8_hwc, "i2it_forward_u8_variations: null image pointer");
+  IO io;
+  std::memset(&io, 0, sizeof io);
+  io.x_u8 = x_u8_hwc; io.in_mode = in_mode; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r;
+  io.out_u8 = out_u8_hwc; io.out_latent = out_latent;
+  E.check_device_error();
+  E.forward(io, n, H, W, direction, text_batch, static_cast<cudaStream_t>(stream), g, /*shared_input=*/true);
+  API_END
+}
+
 int i2it_debug_resample_coeffs(int in_size, int out_size, int* bounds, int* coeffs, int cap) {
   try {
     const i2it::ResampleTable t = i2it::lanczos_table(in_size, out_size);   // the host function the plans upload from

@@ -1303,6 +1303,21 @@ void Engine::copy_channels(Plan& P, const Act& src, const Act& dst) {
   }, "concat_copy", 0, 4.0 * total * 8);
 }
 
+Act Engine::replicate_image(Plan& P, const Act& src, int n) {
+  I2IT_CHECK(src.N == 1 && src.C % 8 == 0 && n >= 1, "replicate_image: needs one image with C % 8 == 0");
+  Act y = alloc_act(P, n, src.H, src.W, src.C);
+  const long long rows = src.rows(), total = rows * n * (src.C / 8);
+  const uint16_t* xp = src.p;
+  uint16_t* yp = y.p;
+  const int ldx = src.ld, C = src.C, dt = dtype;
+  const std::string shape = std::to_string(n) + "x" + std::to_string(src.H) + "x" + std::to_string(src.W) + "x" + std::to_string(C);
+  add_op(P, [=](cudaStream_t st) {
+    DISPATCH_T(dt, (launch_k(replicate_image_kernel<T>, dim3(ceil_div(total, 256)), dim3(256), 0, st, 0,
+                             reinterpret_cast<const T*>(xp), ldx, reinterpret_cast<T*>(yp), C, C, rows, total)));
+  }, "replicate", 0, 2.0 * rows * C * (n + 1), shape);
+  return y;
+}
+
 Act Engine::vt_proj(Plan& P, const Act& x, int B, int ntok, const PW& wv) {
   I2IT_CHECK(x.rows() == static_cast<long long>(B) * ntok, "vt_proj: token count mismatch");
   I2IT_CHECK(x.C == wv.cin || x.C == wv.cin_pad, "vt_proj: width mismatch");
@@ -1636,11 +1651,12 @@ void Engine::encode_text(const int* tokens, int batch, void* out, cudaStream_t s
 }
 
 void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
-                     const i2it_resize_desc* g) {
+                     const i2it_resize_desc* g, bool shared_input) {
   I2IT_CHECK(H % 8 == 0 && W % 8 == 0 && H > 0 && W > 0, "H and W must be positive multiples of 8 (as the reference CLIs crop them)");
   I2IT_CHECK(B > 0 && (text_batch == 1 || text_batch == B), "text_batch must be 1 or batch");
   IO io = io_in;
-  const int io_mode = (io.x_u8 ? IO_U8_IN : 0) | (io.out_u8 ? IO_U8_OUT : 0);
+  // one variation of one image is the plain batch-1 forward: same plan, same output
+  const int io_mode = (io.x_u8 ? IO_U8_IN : 0) | (io.out_u8 ? IO_U8_OUT : 0) | (shared_input && B > 1 ? IO_SHARED_IN : 0);
   I2IT_CHECK((io.x || io.x_u8) && io.eps && (io.out || io.out_u8), "null input/output pointer");
   const bool text_cached = io.text == nullptr;
   if (text_cached) {

@@ -131,7 +131,8 @@ struct IO {
   int pad_ = 0;
   bool operator==(const IO& o) const { return std::memcmp(this, &o, sizeof(IO)) == 0; }
 };
-enum IoMode : int { IO_U8_IN = 1, IO_U8_OUT = 2 };
+// IO_SHARED_IN: a variations forward, one input image for the whole batch (its encoder runs at batch 1)
+enum IoMode : int { IO_U8_IN = 1, IO_U8_OUT = 2, IO_SHARED_IN = 4 };
 
 // uint8 HWC images [B][img bytes][w pixels per row][3] an op reads or writes: a caller pointer read from the plan's IO at
 // launch time (slot), or a plan-internal buffer (p); off selects a window's first pixel
@@ -219,8 +220,9 @@ class Engine {
   // evict: enforce the plan limit once the plan is in (forward() does it itself after the plan becomes the last-run one)
   Plan* plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached = false, int io_mode = 0,
                  const i2it_resize_desc* g = nullptr, bool evict = true);
+  // shared_input: x / x_u8 hold ONE image that all B outputs start from (i2it_forward_variations); B == 1 is the plain forward
   void forward(const IO& io, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
-               const i2it_resize_desc* g = nullptr);
+               const i2it_resize_desc* g = nullptr, bool shared_input = false);
   // cross-attention K / V^T of the prompt, computed once per prompt (i2it_set_text) instead of once per forward
   void set_text(const void* text, int text_batch, cudaStream_t st);
   // CLIP text tower (SURVEY 8f #1): tokens [batch, 77] int32 -> last_hidden_state [batch, 77, hidden] in the handle dtype
@@ -255,6 +257,7 @@ class Engine {
   void resample_u8(Plan& P, const U8View& src, int B, int inH, int inW, int rsH, int rsW, int y0, int x0, int H, int W,
                    const U8View& dst);
   void copy_channels(Plan& P, const Act& src, const Act& dst_slice);
+  Act replicate_image(Plan& P, const Act& src, int n);               // [1,H,W,C] -> [n,H,W,C], every image a copy of src
   // V^T[b] = Wv X[b]^T (+ row bias): returns [B][C][ldv] as an Act with N=B,H=1,W=C,ld=ldv (C field = Ntok)
   Act vt_proj(Plan& P, const Act& x_tokens, int B, int ntok, const PW& wv);
   // attention core on projected operands; q/k are column slices of token matrices; returns [B*Nq, heads*d]
@@ -282,8 +285,9 @@ class Engine {
   int prep_launches_ = 0;
 
   // ---- model graph ----
+  // shared_input: the encoder runs on one image and the posterior sample at batch B from its moments
   Act build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int W, std::vector<Act>& skips,
-                        const U8View* u8_in = nullptr);
+                        const U8View* u8_in = nullptr, bool shared_input = false);
   Act build_unet(Plan& P, const Act& z, int text_batch, bool text_cached);
   void build_text_kv(struct TextKV& T);
   std::vector<std::string> xformer_prefixes() const;

@@ -490,19 +490,22 @@ __global__ void nchw_to_u8hwc_kernel(const T* __restrict__ x, uint8_t* __restric
 
 // DiagonalGaussianDistribution.sample() * scaling_factor (+ the stochastic blend of
 // src/pix2pix_turbo.py:210): moments NHWC (ld) -> latent NHWC8 (channels 4..7 zero).
+// mom_img: pixels between two images' moments, HW; 0 reads image 0's moments for every image (a variations forward, whose
+// encoder ran once at batch 1), with each image's own eps and noise rows.
 template <typename T>
-__global__ void latent_sample_kernel(const T* __restrict__ mom, int ldm, const T* __restrict__ eps_nchw,
+__global__ void latent_sample_kernel(const T* __restrict__ mom, int ldm, long long mom_img, const T* __restrict__ eps_nchw,
                                      const T* __restrict__ noise_nchw, float r, float sf, T* __restrict__ z,
                                      long long HW, long long total) {
   pdl_sync();
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const long long n = i / HW, p = i % HW;
+  const long long m = n * mom_img + p;
   float o[8];
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
-    const float mean = Elem<T>::to_f(mom[i * ldm + c]);
-    const float logvar = fminf(fmaxf(Elem<T>::to_f(mom[i * ldm + 4 + c]), -30.f), 20.f);
+    const float mean = Elem<T>::to_f(mom[m * ldm + c]);
+    const float logvar = fminf(fmaxf(Elem<T>::to_f(mom[m * ldm + 4 + c]), -30.f), 20.f);
     const float e = Elem<T>::to_f(eps_nchw[(n * 4 + c) * HW + p]);
     float v = (mean + expf(0.5f * logvar) * e) * sf;
     if (noise_nchw) {
@@ -628,6 +631,20 @@ __global__ void copy2d_kernel(const T* __restrict__ x, int ldx, T* __restrict__ 
   const long long r = i / vecs;
   const int v = static_cast<int>(i % vecs);
   st16(y + r * ldy + v * 8, ld_nc16(x + r * ldx + v * 8));
+}
+
+// one image [rows][C] (pixel stride ldx) copied into every image of y [n][rows][C] (pixel stride ldy), 16-byte vectors:
+// the batch-1 encoder skips of a variations forward, replicated for the decoder conv that reads them
+template <typename T>
+__global__ void replicate_image_kernel(const T* __restrict__ x, int ldx, T* __restrict__ y, int ldy, int C, long long rows,
+                                       long long total /* n*rows*(C/8) */) {
+  pdl_sync();
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int vecs = C >> 3;
+  const long long r = i / vecs;
+  const int v = static_cast<int>(i % vecs);
+  st16(y + r * ldy + v * 8, ld_nc16(x + (r % rows) * ldx + v * 8));
 }
 
 }  // namespace i2it

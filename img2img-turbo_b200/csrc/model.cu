@@ -65,9 +65,12 @@ Act Engine::vae_attn(Plan& P, const std::string& p, const Act& x) {
   return y;
 }
 
-Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int W, std::vector<Act>& skips,
-                              const U8View* u8_in) {
+Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B_out, int H, int W, std::vector<Act>& skips,
+                              const U8View* u8_in, bool shared_input) {
   const std::string e = vp + "encoder";
+  // a variations forward encodes its one input image once: everything up to the moments (and the skips) at batch 1, the
+  // posterior sample at batch B_out
+  const int B = shared_input ? 1 : B_out;
   // conv_in (3 -> C0, 3x3): the NCHW boundary tensor is packed straight into im2col rows [B,H,W,32] (27 taps*channels + 5
   // zeros), so the conv is ONE K=32 GEMM tap with 64-byte TMA rows instead of nine taps of 16-byte rows
   Act xcol = alloc_act(P, B, H, W, 32);
@@ -118,9 +121,9 @@ Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int 
   ConvOpts o1; o1.ksize = 1;
   Act mom = conv(P, s, prep(vp + "quant_conv", {vp + "quant_conv"}), o1);
   mark(P, "moments", mom);
-  Act z = alloc_act(P, B, H / 8, W / 8, 8, 8, true);
+  Act z = alloc_act(P, B_out, H / 8, W / 8, 8, 8, true);
   {
-    const long long HW = static_cast<long long>(H / 8) * (W / 8), total = HW * B;
+    const long long HW = static_cast<long long>(H / 8) * (W / 8), total = HW * B_out, mom_img = shared_input ? 0 : HW;
     const uint16_t* mp = mom.p;
     const int ldm = mom.ld, dt = dtype;
     uint16_t* zp = z.p;
@@ -129,7 +132,7 @@ Act Engine::build_vae_encoder(Plan& P, const std::string& vp, int B, int H, int 
     P.keep.push_back(mom.hold);
     add_op(P, [=](cudaStream_t st) {
       DISPATCH_T(dt, (launch_k(latent_sample_kernel<T>, dim3(ceil_div_i(total, 128)), dim3(128), 0, st, 0,
-                         reinterpret_cast<const T*>(mp), ldm, reinterpret_cast<const T*>(plan->io.eps),
+                         reinterpret_cast<const T*>(mp), ldm, mom_img, reinterpret_cast<const T*>(plan->io.eps),
                          reinterpret_cast<const T*>(plan->io.noise), plan->io.r, sf, reinterpret_cast<T*>(zp), HW, total)));
     });
   }
@@ -148,12 +151,21 @@ void Engine::build_vae_decoder(Plan& P, const std::string& vp, const Act& dec_in
   // for up-block i: mid_block.resnets.1.conv2 for i = 0, the previous block's upsampler conv for i >= 1.  gamma is folded
   // into the bias-free 1x1 weights.
   auto skip_w = [&](int i) { const std::string sk = d + ".skip_conv_" + std::to_string(i + 1); return prep(sk, {sk}, false, skip_gamma_); };
+  // the skip that skip_conv_(k+1) reads.  A variations forward encoded one image: its batch-1 skip is replicated to the
+  // decoder's batch right before the block that reads it, so a batch-n copy lives for one layer, not across the UNet
+  auto skip_in = [&](int i, int k) {
+    if (skips[i].N == dec_in.N) return skips[i];
+    Act rep = replicate_image(P, skips[i], dec_in.N);
+    mark_layer(P, d + ".skip_conv_" + std::to_string(k + 1) + ".replica", rep);
+    return rep;
+  };
   s = vae_resnet(P, d + ".mid_block.resnets.0", s);
   s = vae_attn(P, d + ".mid_block.attentions.0", s);
   {
     PW w0 = skip_w(0);
-    s = vae_resnet(P, d + ".mid_block.resnets.1", s, &skips[3], &w0);
+    const Act sk = skip_in(3, 0);
     skips[3] = Act();
+    s = vae_resnet(P, d + ".mid_block.resnets.1", s, &sk, &w0);
   }
   mark(P, "dec_mid", s);
   for (int i = 0; i < 4; ++i) {
@@ -165,9 +177,10 @@ void Engine::build_vae_decoder(Plan& P, const std::string& vp, const Act& dec_in
       // upsampled tensor never exists); the next block's skip conv rides along as a second source at output resolution
       const std::string u = d + ".up_blocks." + std::to_string(i) + ".upsamplers.0.conv";
       PW wn = skip_w(i + 1);
-      s = conv_up2x(P, s, prep_subpixel(u), &skips[2 - i], &wn, true);
-      mark_layer(P, u, s);
+      const Act sk = skip_in(2 - i, i + 1);
       skips[2 - i] = Act();
+      s = conv_up2x(P, s, prep_subpixel(u), &sk, &wn, true);
+      mark_layer(P, u, s);
     }
     mark(P, "dec_up" + std::to_string(i), s);
   }
@@ -509,6 +522,8 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
     ~BuildGuard() { if (!ok) { e->text_ = Act(); e->text_kv_ = nullptr; } }
   } guard{this};
   std::vector<Act> skips;
+  const bool shared_input = (io_mode & IO_SHARED_IN) != 0;
+  const int B_in = shared_input ? 1 : B;      // images the input side (resize_in, packing, VAE encoder) runs on
   if (io_mode & IO_U8_OUT) {
     // allocated FIRST and held for the plan's lifetime: pool liveness follows build order, and the last conv writes here
     auto tmp = alloc_raw(P, static_cast<size_t>(B) * 3 * H * W * 2);
@@ -523,17 +538,17 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
     if (g->in_H == g->resize_H && g->in_W == g->resize_W) {
       net_in.off = 3 * (static_cast<long long>(g->crop_y) * g->in_W + g->crop_x);   // a crop of the input itself: no pass
     } else {
-      auto buf = alloc_raw(P, static_cast<size_t>(B) * H * W * 3);
+      auto buf = alloc_raw(P, static_cast<size_t>(B_in) * H * W * 3);
       P.keep.push_back(buf);
       U8View d;
       d.p = static_cast<uint8_t*>(buf.get()); d.img = 3ll * H * W; d.w = W;
       P.ranges.emplace_back(P.ops.size(), "resize_in");
-      resample_u8(P, net_in, B, g->in_H, g->in_W, g->resize_H, g->resize_W, g->crop_y, g->crop_x, H, W, d);
+      resample_u8(P, net_in, B_in, g->in_H, g->in_W, g->resize_H, g->resize_W, g->crop_y, g->crop_x, H, W, d);
       net_in = d;
     }
   }
   P.ranges.emplace_back(P.ops.size(), "vae_encode");
-  Act z = build_vae_encoder(P, vp, B, H, W, skips, (io_mode & IO_U8_IN) ? &net_in : nullptr);
+  Act z = build_vae_encoder(P, vp, B, H, W, skips, (io_mode & IO_U8_IN) ? &net_in : nullptr, shared_input);
   P.ranges.emplace_back(P.ops.size(), "unet");
   Act pred = build_unet(P, z, text_batch, text_cached);
   mark(P, "model_pred", pred);

@@ -33,7 +33,7 @@ SYMBOLS = [
     "i2it_op_upsample_to", "i2it_stage_names", "i2it_prepared_keys", "i2it_read_prepared", "i2it_text_stage_names",
     "i2it_forward_u8_resize", "i2it_op_resize_u8", "i2it_debug_resample_coeffs",
     "i2it_set_max_plans", "i2it_release_plans", "i2it_memory_stats_get", "i2it_debug_poison_workspace",
-    "i2it_debug_tapgemm_override",
+    "i2it_debug_tapgemm_override", "i2it_forward_variations", "i2it_forward_u8_variations",
 ]
 TEXT_TOKEN_EMB = "text_encoder.text_model.embeddings.token_embedding.weight"
 TEXT_POS_EMB = "text_encoder.text_model.embeddings.position_embedding.weight"
@@ -171,6 +171,9 @@ def load_library(path: Optional[str] = None):
     lib.i2it_memory_stats_get.argtypes = [vp, C.POINTER(MemoryStats)]
     lib.i2it_debug_poison_workspace.argtypes = [vp, ci]
     lib.i2it_debug_tapgemm_override.argtypes = [vp, ci, ci, ci]
+    lib.i2it_forward_variations.argtypes = [vp, vp, vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci, vp]
+    lib.i2it_forward_u8_variations.argtypes = [vp, vp, ci, C.POINTER(ResizeDesc), vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci,
+                                               vp]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("i2it_destroy", "i2it_last_error"):
@@ -343,6 +346,46 @@ class Engine:
         self._check(self.lib.i2it_forward_u8_resize(self._h, _ptr(x_u8), int(in_mode), C.byref(d), _ptr(text_emb), tb, _ptr(eps),
                                                     _ptr(noise_map), float(r), _ptr(out), _ptr(out_latent), B, H, W, direction,
                                                     _stream()), "i2it_forward_u8_resize")
+        return out
+
+    def forward_variations(self, x1: torch.Tensor, text_emb: Optional[torch.Tensor], eps: torch.Tensor,
+                           noise_map: Optional[torch.Tensor] = None, r: float = 1.0, direction: int = A2B,
+                           out: Optional[torch.Tensor] = None, out_latent: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """n = eps.shape[0] variations of ONE image x1 [1,3,H,W]: eps / noise_map / out / out_latent have batch n, text_emb
+        batch 1 or n.  The VAE encoder runs once; output i equals image i of forward() on x1 repeated n times, bit for bit."""
+        B, Cc, H, W = x1.shape
+        if B != 1 or Cc != 3:
+            raise ValueError(f"forward_variations takes one image [1,3,H,W], got {list(x1.shape)}")
+        n = eps.shape[0]
+        tb = self._check_operands(n, H, W, text_emb, eps, (x1, noise_map, out, out_latent))
+        if out is None:
+            out = torch.empty(n, 3, H, W, device=x1.device, dtype=x1.dtype)
+        self._check(self.lib.i2it_forward_variations(self._h, _ptr(x1), _ptr(text_emb), tb, _ptr(eps), _ptr(noise_map),
+                                                     float(r), _ptr(out), _ptr(out_latent), n, H, W, direction, _stream()),
+                    "i2it_forward_variations")
+        return out
+
+    def forward_u8_variations(self, x_u8_1: torch.Tensor, in_mode: int, text_emb: Optional[torch.Tensor], eps: torch.Tensor,
+                              noise_map: Optional[torch.Tensor] = None, r: float = 1.0, direction: int = A2B,
+                              out: Optional[torch.Tensor] = None, out_latent: Optional[torch.Tensor] = None, *,
+                              resize=None, crop=None, out_size=None) -> torch.Tensor:
+        """forward_u8 on ONE image x_u8_1 [1,H,W,3] with n = eps.shape[0] outputs [n,out_H,out_W,3] (see forward_variations);
+        the resize / crop / out_size geometry is forward_u8's.  The input resize runs once, the output resize per output."""
+        B, Hi, Wi, Cc = x_u8_1.shape
+        assert Cc == 3 and x_u8_1.dtype == torch.uint8 and x_u8_1.is_cuda and x_u8_1.is_contiguous(), \
+            "image must be uint8 CUDA [1,H,W,3]"
+        if B != 1:
+            raise ValueError(f"forward_u8_variations takes one image [1,H,W,3], got {list(x_u8_1.shape)}")
+        n = eps.shape[0]
+        rs, (cy, cx, H, W), osz = resize_geometry((Hi, Wi), resize, crop, out_size)
+        tb = self._check_operands(n, H, W, text_emb, eps, (noise_map, out_latent))
+        if out is None:
+            out = torch.empty(n, osz[0], osz[1], 3, dtype=torch.uint8, device=x_u8_1.device)
+        assert out.dtype == torch.uint8 and out.is_cuda and out.is_contiguous() and out.shape == (n, osz[0], osz[1], 3)
+        d = ResizeDesc(Hi, Wi, rs[0], rs[1], cy, cx, osz[0], osz[1])
+        self._check(self.lib.i2it_forward_u8_variations(self._h, _ptr(x_u8_1), int(in_mode), C.byref(d), _ptr(text_emb), tb,
+                                                        _ptr(eps), _ptr(noise_map), float(r), _ptr(out), _ptr(out_latent), n,
+                                                        H, W, direction, _stream()), "i2it_forward_u8_variations")
         return out
 
     def prep_launch_count(self) -> int:

@@ -157,6 +157,35 @@ class Pix2Pix_Turbo(TurboBase):
         """Convenience alias (the reference has only the constructor)."""
         return cls(pretrained_name=pretrained_name, **kw)
 
+    def _draw_eps(self, eps, B, H, Wd):
+        dt = self.compute_dtype
+        if eps is None:
+            # latent_dist.sample(): randn from the global RNG on the device, in the activation dtype (SURVEY fact 5)
+            eps = torch.randn((B, 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)
+            torch.randn((B, 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)   # DDPM variance noise: drawn, x1e-10, discarded
+        return self._prep(eps, dt)
+
+    def _fold_and_run(self, x, caption_enc, eps, B, deterministic, r, noise_map, **staged):
+        """Fold the weights of a deterministic or stochastic call, then run it through _staged_forward (keywords `staged`)
+        with the noise map expanded to the B outputs."""
+        if deterministic:
+            if self._twin:
+                raise TypeError("deterministic forward on a TwinConv model: conv_in.r is None (as in the reference)")
+            eng = self._finalize(self._lora_w_unet, self._lora_w_vae, float(self.vae.decoder.gamma), -1.0)
+            return self._staged_forward(eng, x, caption_enc, eps, **staged)
+        if noise_map is None:
+            raise ValueError("noise_map is required when deterministic=False")
+        # unet.set_adapters(["default"],[r]); set_weights_and_activate_adapters(vae,["vae_skip"],[r]);
+        # conv_in.r = r; decoder.gamma = r   (reference :206-217)
+        self._lora_w_unet = self._lora_w_vae = float(r)
+        self.vae.decoder.gamma = r
+        eng = self._finalize(r, r, r, r if self._twin else -1.0)
+        nm = self._prep(noise_map.expand(B, -1, -1, -1) if noise_map.shape[0] != B else noise_map, self.compute_dtype)
+        out = self._staged_forward(eng, x, caption_enc, eps, noise=nm, r=float(r), **staged)
+        if self._twin:
+            self.unet.conv_in.r = None
+        return out
+
     def forward(self, c_t, prompt=None, prompt_tokens=None, deterministic=True, r=1.0, noise_map=None, *, eps=None):
         # either the prompt or the prompt_tokens should be provided  (reference :188)
         assert (prompt is None) != (prompt_tokens is None), "Either prompt or prompt_tokens should be provided"
@@ -165,30 +194,29 @@ class Pix2Pix_Turbo(TurboBase):
         caption_enc = self._encode_text(prompt, prompt_tokens)
         B, _, H, Wd = c_t.shape
         x = self._prep(c_t, dt)
-        if eps is None:
-            # latent_dist.sample(): randn from the global RNG on the device, in the activation dtype (SURVEY fact 5)
-            eps = torch.randn((B, 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)
-            torch.randn((B, 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)   # DDPM variance noise: drawn, x1e-10, discarded
-        eps = self._prep(eps, dt)
+        eps = self._draw_eps(eps, B, H, Wd)
         if caption_enc.shape[0] not in (1, B):
             raise ValueError("prompt batch must be 1 or match the image batch")
-        if deterministic:
-            if self._twin:
-                raise TypeError("deterministic forward on a TwinConv model: conv_in.r is None (as in the reference)")
-            eng = self._finalize(self._lora_w_unet, self._lora_w_vae, float(self.vae.decoder.gamma), -1.0)
-            out = self._staged_forward(eng, x, caption_enc, eps)
-        else:
-            if noise_map is None:
-                raise ValueError("noise_map is required when deterministic=False")
-            # unet.set_adapters(["default"],[r]); set_weights_and_activate_adapters(vae,["vae_skip"],[r]);
-            # conv_in.r = r; decoder.gamma = r   (reference :206-217)
-            self._lora_w_unet = self._lora_w_vae = float(r)
-            self.vae.decoder.gamma = r
-            eng = self._finalize(r, r, r, r if self._twin else -1.0)
-            nm = self._prep(noise_map.expand(B, -1, -1, -1) if noise_map.shape[0] != B else noise_map, dt)
-            out = self._staged_forward(eng, x, caption_enc, eps, noise=nm, r=float(r))
-            if self._twin:
-                self.unet.conv_in.r = None
+        out = self._fold_and_run(x, caption_enc, eps, B, deterministic, r, noise_map)
+        return out if in_dtype == dt else out.to(in_dtype)
+
+    def variations(self, c_t, prompt=None, prompt_tokens=None, deterministic=True, r=1.0, noise_map=None, *, n=None, eps=None):
+        """n outputs of ONE control image c_t [1,3,H,W] in one forward that runs the VAE encoder once
+        (i2it.Engine.forward_variations): output i equals image i of forward() on c_t repeated n times with the same eps,
+        noise_map and prompts, bit for bit.  prompt (a string or a list of 1 or n) / prompt_tokens [1|n, 77] give one prompt
+        for all variations or one each; noise_map is [n,4,H/8,W/8] (or [1,...], shared); eps [n,4,H/8,W/8] is drawn as
+        forward() draws it when not given.  n comes from n=, eps, noise_map or the prompt batch, which must agree."""
+        assert (prompt is None) != (prompt_tokens is None), "Either prompt or prompt_tokens should be provided"
+        if c_t.dim() != 4 or c_t.shape[0] != 1:
+            raise ValueError(f"variations takes one control image [1,3,H,W], got {list(c_t.shape)}")
+        dt = self.compute_dtype
+        in_dtype = c_t.dtype
+        caption_enc = self._encode_text(prompt, prompt_tokens)
+        _, _, H, Wd = c_t.shape
+        n = self._variation_count(n, caption_enc, noise_map, eps)
+        x = self._prep(c_t, dt)
+        eps = self._draw_eps(eps, n, H, Wd)
+        out = self._fold_and_run(x, caption_enc, eps, n, deterministic, r, noise_map, variations=True)
         return out if in_dtype == dt else out.to(in_dtype)
 
     def forward_u8(self, images_u8, prompt=None, prompt_tokens=None, deterministic=True, r=1.0, noise_map=None, *, eps=None,
@@ -200,28 +228,27 @@ class Pix2Pix_Turbo(TurboBase):
         resize / crop / out_size (i2it.Engine.forward_u8) also run PIL LANCZOS resizes on device, bit-exact:
         resize=_host.paired_geometry(H, W) is the CLI's resize to multiples of 8 (:38-41).  eps then has the crop's size."""
         assert (prompt is None) != (prompt_tokens is None), "Either prompt or prompt_tokens should be provided"
-        dt = self.compute_dtype
         caption_enc = self._encode_text(prompt, prompt_tokens)
         x = images_u8.to(device=_host.DEVICE, non_blocking=True).contiguous()
         B = x.shape[0]
         H, Wd, geom = self._u8_geometry(x.shape, resize, crop, out_size)
-        if eps is None:
-            eps = torch.randn((B, 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)
-            torch.randn((B, 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)
-        eps = self._prep(eps, dt)
+        eps = self._draw_eps(eps, B, H, Wd)
         mode = i2it.IN_SKETCH if sketch else i2it.IN_UNIT
-        if deterministic:
-            if self._twin:
-                raise TypeError("deterministic forward on a TwinConv model: conv_in.r is None (as in the reference)")
-            eng = self._finalize(self._lora_w_unet, self._lora_w_vae, float(self.vae.decoder.gamma), -1.0)
-            return self._staged_forward(eng, x, caption_enc, eps, u8_mode=mode, geometry=geom)
-        if noise_map is None:
-            raise ValueError("noise_map is required when deterministic=False")
-        self._lora_w_unet = self._lora_w_vae = float(r)
-        self.vae.decoder.gamma = r
-        eng = self._finalize(r, r, r, r if self._twin else -1.0)
-        nm = self._prep(noise_map.expand(B, -1, -1, -1) if noise_map.shape[0] != B else noise_map, dt)
-        out = self._staged_forward(eng, x, caption_enc, eps, noise=nm, r=float(r), u8_mode=mode, geometry=geom)
-        if self._twin:
-            self.unet.conv_in.r = None
-        return out
+        return self._fold_and_run(x, caption_enc, eps, B, deterministic, r, noise_map, u8_mode=mode, geometry=geom)
+
+    def variations_u8(self, images_u8, prompt=None, prompt_tokens=None, deterministic=True, r=1.0, noise_map=None, *, n=None,
+                      eps=None, sketch=False, resize=None, crop=None, out_size=None):
+        """variations() on the uint8 HWC boundary of forward_u8: ONE image [1,H,W,3] uint8 -> [n,out_H,out_W,3] uint8 CUDA.
+        The input resize / crop and the encoder run once; output i equals image i of forward_u8 on the image repeated n
+        times."""
+        assert (prompt is None) != (prompt_tokens is None), "Either prompt or prompt_tokens should be provided"
+        if images_u8.dim() != 4 or images_u8.shape[0] != 1:
+            raise ValueError(f"variations_u8 takes one image [1,H,W,3], got {list(images_u8.shape)}")
+        caption_enc = self._encode_text(prompt, prompt_tokens)
+        x = images_u8.to(device=_host.DEVICE, non_blocking=True).contiguous()
+        H, Wd, geom = self._u8_geometry(x.shape, resize, crop, out_size)
+        n = self._variation_count(n, caption_enc, noise_map, eps)
+        eps = self._draw_eps(eps, n, H, Wd)
+        mode = i2it.IN_SKETCH if sketch else i2it.IN_UNIT
+        return self._fold_and_run(x, caption_enc, eps, n, deterministic, r, noise_map, u8_mode=mode, geometry=geom,
+                                  variations=True)

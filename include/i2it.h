@@ -181,6 +181,27 @@ int i2it_forward_u8_resize(i2it_handle* h, const void* x_u8_hwc, int in_mode, co
                            int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc, void* out_latent,
                            int batch, int H, int W, int direction, void* stream);
 
+/* n variations of ONE image in one forward: i2it_forward with x [1, 3, H, W] and every other operand at batch n
+ * (eps [n, 4, H/8, W/8], noise_map [n, 4, H/8, W/8] or NULL, out [n, 3, H, W], out_latent [n, 4, H/8, W/8] or NULL,
+ * text_emb [text_batch, 77, cross] with text_batch 1 or n, or NULL for the i2it_set_text cache).  The VAE encoder runs once, at
+ * batch 1: its moments feed every image's posterior sample (each with its own eps and noise_map rows), and each of its four
+ * skips is replicated to batch n right before the decoder conv that reads it.  Output image i is bit-identical to image i of
+ * i2it_forward on the image repeated n times (and to a batch-1 forward of it with eps[i], noise_map[i]): the encoder of a
+ * batch computes each image alone.  A variations key is its own plan (n = 1 is the plain batch-1 plan).  Rejected before any
+ * launch: n < 1, text_batch not 1 or n, and whatever i2it_forward rejects.  Replaces the one-forward-per-seed loop of
+ * gradio_sketch2image.py. */
+int i2it_forward_variations(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps,
+                            const void* noise_map, float r, void* out, void* out_latent, int n, int H, int W, int direction,
+                            void* stream);
+
+/* i2it_forward_variations with the uint8 HWC boundary of i2it_forward_u8 / i2it_forward_u8_resize: x_u8_hwc [1, in_H, in_W, 3]
+ * -> out_u8_hwc [n, out_H, out_W, 3].  g is a resize geometry or NULL (then in_H = out_H = H, in_W = out_W = W); the input
+ * resize passes and packing run at batch 1, the output conversion and resize at batch n.  Rejected before any launch: what
+ * i2it_forward_variations and i2it_forward_u8_resize reject. */
+int i2it_forward_u8_variations(i2it_handle* h, const void* x_u8_hwc, int in_mode, const i2it_resize_desc* g, const void* text_emb,
+                               int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc,
+                               void* out_latent, int n, int H, int W, int direction, void* stream);
+
 /* Number of kernel launches one forward of this shape issues (for bench accounting): the plan the last forward used if it
  * has this shape, else the plan with the text embedding passed inline. */
 int i2it_launch_count(i2it_handle* h, int batch, int H, int W, int direction, int* launches);
