@@ -117,6 +117,24 @@ def image_prep_geometry(image_prep: str, H: int, W: int):
     raise ValueError(f"image_prep {image_prep!r} has no deterministic resize geometry (random crops are training-only)")
 
 
+def ragged_geometries(sizes, image_prep: Optional[str] = None, resize=None):
+    """(H, W, geometries) of a ragged uint8 batch of images of `sizes` [(H_i, W_i), ...]: image i goes through
+    image_prep_geometry(image_prep, H_i, W_i), or a LANCZOS resize to `resize` (H, W) when image_prep is None, and its output
+    comes back at (H_i, W_i).  H x W is the network size they share; raises ValueError when they would not share one."""
+    if len(sizes) == 0:
+        raise ValueError("a ragged batch needs at least one image")
+    geoms, net = [], set()
+    for h, w in sizes:
+        h, w = int(h), int(w)
+        rs, crop = image_prep_geometry(image_prep, h, w) if image_prep is not None else (tuple(int(v) for v in resize), None)
+        net.add(tuple(crop[2:]) if crop is not None else tuple(rs))
+        geoms.append({"resize": tuple(rs), "crop": crop, "out_size": (h, w)})
+    if len(net) != 1:
+        raise ValueError(f"the images of a ragged batch must share one network size; {image_prep or resize} gives {sorted(net)}")
+    H, W = net.pop()
+    return H, W, geoms
+
+
 def paired_geometry(H: int, W: int):
     """resize (H, W) of src/inference_paired.py:38-41: LANCZOS to the multiple of 8 below each side."""
     return H - H % 8, W - W % 8
@@ -343,12 +361,15 @@ class TurboBase(torch.nn.Module):
         return cr[2], cr[3], {"resize": rs, "crop": cr, "out_size": out}
 
     def _staged_forward(self, eng, x, text, eps, noise=None, r=1.0, direction=i2it.A2B, u8_mode=None, geometry=None,
-                        variations=False):
+                        variations=False, ragged=None):
         """Run the engine through persistent device staging buffers (per shape/dtype): the captured CUDA graph bakes the IO
         pointers in, so stable addresses mean every call replays the same graph.  Costs two small device-to-device copies;
         the result is returned in a fresh tensor (never aliased across calls).  The text embedding is not an input of the
         graph: its projections are cached on the engine (_bind_text).  `geometry`: forward_u8 resize keywords.
-        variations: x is one image and the eps.shape[0] outputs are its variations (forward_variations)."""
+        variations: x is one image and the eps.shape[0] outputs are its variations (forward_variations).
+        ragged: x is a list of uint8 images of their own sizes and `ragged` their forward_u8 geometries (forward_u8_ragged)."""
+        if ragged is not None:
+            return self._ragged_forward(eng, x, text, eps, noise, r, direction, u8_mode, ragged)
         self._bind_text(eng, text)
         gkey = tuple(sorted(geometry.items())) if geometry else None
         n = eps.shape[0] if variations else x.shape[0]
@@ -373,6 +394,23 @@ class TurboBase(torch.nn.Module):
             fwd(st["x"], u8_mode, None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction, out=st["out"],
                 **(geometry or {}))
         return st["out"].clone()
+
+    def _ragged_forward(self, eng, images, text, eps, noise, r, direction, u8_mode, geometries):
+        """forward_u8_ragged on a list of images.  Only eps and the noise map go through persistent staging: the graph bakes
+        their pointers in.  The images and the fresh outputs sit in the call's descriptors, so they need no copy."""
+        self._bind_text(eng, text)
+        key = ("ragged", tuple(eps.shape), eps.dtype, noise is not None, _cur_dev())
+        st = self.__dict__.setdefault("_stage", {}).get(key)
+        if st is None:
+            st = {"eps": torch.empty_like(eps), "noise": torch.empty_like(eps) if noise is not None else None}
+            if len(self._stage) > 8:
+                self._stage.clear()
+            self._stage[key] = st
+        st["eps"].copy_(eps, non_blocking=True)
+        if noise is not None:
+            st["noise"].copy_(noise, non_blocking=True)
+        return eng.forward_u8_ragged(images, u8_mode, None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction,
+                                     geometries=geometries)
 
     @staticmethod
     def _variation_count(n, text, noise_map, eps) -> int:

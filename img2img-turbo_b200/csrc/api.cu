@@ -213,6 +213,40 @@ int i2it_forward_u8_variations(i2it_handle* h, const void* x_u8_hwc, int in_mode
   API_END
 }
 
+int i2it_forward_u8_ragged(i2it_handle* h, const void* const* x_u8, int in_mode, const i2it_resize_desc* g, int max_side,
+                           const void* text_emb, int text_batch, const void* eps, const void* noise_map, float r,
+                           void* const* out_u8, void* out_latent, int n, int H, int W, int direction, void* stream) {
+  API_BEGIN(h)
+  I2IT_CHECK(n >= 1, "i2it_forward_u8_ragged: n must be >= 1");
+  I2IT_CHECK(in_mode >= 0 && in_mode <= 2, "i2it_forward_u8_ragged: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
+  IO io;
+  std::memset(&io, 0, sizeof io);
+  io.in_mode = in_mode; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r; io.out_latent = out_latent;
+  E.check_device_error();
+  E.forward_ragged(io, x_u8, out_u8, g, max_side, n, H, W, direction, text_batch, static_cast<cudaStream_t>(stream));
+  API_END
+}
+
+int i2it_debug_ragged_tables(const i2it_resize_desc* g, int n, int H, int W, int max_side, long long* used, long long* bound) {
+  try {
+    i2it::rs_check_ragged(g, n, H, W, max_side);
+    i2it::RsTableCache cache;
+    const i2it::RsCall c = i2it::rs_forward_call(g, n, H, W, max_side, cache, nullptr, nullptr, nullptr);   // what the forward uploads
+    if (used) *used = static_cast<long long>(c.tab.size());
+    if (bound) *bound = i2it::rs_forward_bound(n, H, W, max_side);
+    return 0;
+  } catch (...) {
+    return -1;
+  }
+}
+
+int i2it_debug_graph_captures(i2it_handle* h, int* captures) {
+  API_BEGIN(h)
+  I2IT_CHECK(captures != nullptr, "null out pointer");
+  *captures = E.graph_captures;
+  API_END
+}
+
 int i2it_debug_resample_coeffs(int in_size, int out_size, int* bounds, int* coeffs, int cap) {
   try {
     const i2it::ResampleTable t = i2it::lanczos_table(in_size, out_size);   // the host function the plans upload from
@@ -487,6 +521,17 @@ int i2it_debug_tapgemm_override(i2it_handle* h, int bn, int stages, int grid) {
   API_BEGIN(h)
   I2IT_CHECK(bn >= 0 && stages >= 0 && grid >= 0, "i2it_debug_tapgemm_override: values must be >= 0 (0: the engine's choice)");
   E.dbg_bn = bn; E.dbg_stages = stages; E.dbg_grid = grid;
+  API_END
+}
+
+int i2it_op_resize_u8_ragged(i2it_handle* h, const void* const* x, const int* hw_in, void* const* out, const int* hw_out,
+                             int n, int max_side, void* stream) {
+  API_BEGIN(h)
+  {
+    Plan P;
+    E.resize_ragged_op(P, x, hw_in, out, hw_out, n, max_side);
+    run_plan(h, P, static_cast<cudaStream_t>(stream));
+  }
   API_END
 }
 

@@ -280,6 +280,7 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CUDA(cudaStreamCreateWithFlags(&gstream_, cudaStreamNonBlocking));
   I2IT_CUDA(cudaEventCreateWithFlags(&ev_in_, cudaEventDisableTiming));
   I2IT_CUDA(cudaEventCreateWithFlags(&ev_out_, cudaEventDisableTiming));
+  I2IT_CUDA(cudaEventCreateWithFlags(&rs_ev_, cudaEventDisableTiming));
   encode_fn();
   arena_.device = c.device;
 }
@@ -296,6 +297,8 @@ Engine::~Engine() {
   if (gstream_) cudaStreamDestroy(gstream_);
   if (ev_in_) cudaEventDestroy(ev_in_);
   if (ev_out_) cudaEventDestroy(ev_out_);
+  if (rs_ev_) cudaEventDestroy(rs_ev_);
+  if (rs_blob_) cudaFreeHost(rs_blob_);
 }
 
 void Engine::check_device_error() {
@@ -1675,6 +1678,64 @@ void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int te
   }
   Plan* P = plan_for(B, H, W, direction, text_batch, text_cached, io_mode, g, /*evict=*/false);
   if (io_mode & IO_U8_OUT) io.out = P->u8_out_tmp;
+  run(P, io, st);
+}
+
+void Engine::forward_ragged(const IO& io_in, const void* const* x, void* const* out, const i2it_resize_desc* g, int max_side,
+                            int B, int H, int W, int direction, int text_batch, cudaStream_t st) {
+  I2IT_CHECK(H % 8 == 0 && W % 8 == 0 && H > 0 && W > 0, "H and W must be positive multiples of 8 (as the reference CLIs crop them)");
+  I2IT_CHECK(B > 0 && (text_batch == 1 || text_batch == B), "text_batch must be 1 or batch");
+  I2IT_CHECK(x && out && g, "ragged forward: null image or geometry array");
+  rs_check_ragged(g, B, H, W, max_side);      // before the pointers: an empty output (a zero size) has a null one
+  for (int i = 0; i < B; ++i)
+    I2IT_CHECK(x[i] && out[i], "ragged forward: null image pointer (image " + std::to_string(i) + ")");
+  I2IT_CHECK(io_in.eps, "null input/output pointer");
+  const bool text_cached = io_in.text == nullptr;
+  if (text_cached) {
+    auto it = textkv_.find(text_batch);
+    I2IT_CHECK(it != textkv_.end() && it->second->filled,
+               "text_emb == NULL: call i2it_set_text first (and again after every i2it_finalize_weights)");
+  }
+  // the tables first: a size pair the table builder refuses fails here, before a plan is built or anything is enqueued
+  for (int i = 0; i < B; ++i) {
+    const int pairs[4][2] = {{g[i].in_H, g[i].resize_H}, {g[i].in_W, g[i].resize_W}, {H, g[i].out_H}, {W, g[i].out_W}};
+    for (const auto& pr : pairs)
+      if (pr[0] != pr[1]) rs_tables_.get(pr[0], pr[1]);
+  }
+  // the images live in the descriptors, not in the launches: the graph cache key holds no image pointer
+  IO io = io_in;
+  io.x_u8 = nullptr; io.out_u8 = nullptr;
+  Plan* P = plan_for(B, H, W, direction, text_batch, text_cached, IO_U8_IN | IO_U8_OUT | IO_RAGGED, nullptr, /*evict=*/false,
+                     max_side);
+  io.out = P->u8_out_tmp;
+  const RsCall c = rs_forward_call(g, B, H, W, max_side, rs_tables_, x, out, &P->rg);
+  for (int k = 0; k < 4; ++k) P->meta[P->rg.ops[k]].bytes = c.bytes[k];   // i2it_profile: this call's geometries
+  const size_t bytes = stage_ragged(c, P->rg.dev_bytes);
+  char* dev = P->rg.dev;
+  const char* blob = rs_blob_;
+  run(P, io, st, [=](cudaStream_t s) {
+    I2IT_CUDA(cudaMemcpyAsync(dev, blob, bytes, cudaMemcpyHostToDevice, s));
+    I2IT_CUDA(cudaEventRecord(rs_ev_, s));
+  });
+}
+
+size_t Engine::stage_ragged(const RsCall& c, size_t cap) {
+  const size_t dbytes = c.d.size() * sizeof(RsPass), bytes = dbytes + c.tab.size() * sizeof(int);
+  I2IT_CHECK(bytes <= cap, "ragged resize: the call's tables exceed the plan's bound");
+  I2IT_CUDA(cudaEventSynchronize(rs_ev_));      // the previous call's copy has read the blob
+  if (bytes > rs_blob_cap_) {
+    if (rs_blob_) I2IT_CUDA(cudaFreeHost(rs_blob_));
+    rs_blob_ = nullptr;
+    rs_blob_cap_ = 0;
+    I2IT_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&rs_blob_), bytes, cudaHostAllocDefault));
+    rs_blob_cap_ = bytes;
+  }
+  std::memcpy(rs_blob_, c.d.data(), dbytes);
+  std::memcpy(rs_blob_ + dbytes, c.tab.data(), c.tab.size() * sizeof(int));
+  return bytes;
+}
+
+void Engine::run(Plan* P, const IO& io, cudaStream_t st, const std::function<void(cudaStream_t)>& before) {
   P->io = io;
   last_plan_ = P;
   P->last_run = ++tick_;
@@ -1683,6 +1744,7 @@ void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int te
     // replay on the engine's own stream, ordered after/before the caller's stream with events
     I2IT_CUDA(cudaEventRecord(ev_in_, st));
     I2IT_CUDA(cudaStreamWaitEvent(gstream_, ev_in_, 0));
+    if (before) before(gstream_);
     cudaGraphExec_t ge = nullptr;
     for (auto& g : P->graphs) if (g.first == io) ge = g.second;
     if (!ge) {
@@ -1697,6 +1759,7 @@ void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int te
       I2IT_CUDA(cudaGraphInstantiate(&ge, g, 0));
       cudaGraphDestroy(g);
       P->graphs.emplace_back(io, ge);
+      ++graph_captures;
     }
     nvtxRangePushA("i2it:forward(graph)");
     I2IT_CUDA(cudaGraphLaunch(ge, gstream_));
@@ -1704,6 +1767,7 @@ void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int te
     I2IT_CUDA(cudaEventRecord(ev_out_, gstream_));
     I2IT_CUDA(cudaStreamWaitEvent(st, ev_out_, 0));
   } else {
+    if (before) before(st);
     g_pdl.enabled = use_pdl; g_pdl.prev_is_kernel = false;
     size_t next_range = 0;
     bool open = false;

@@ -132,7 +132,8 @@ struct IO {
   bool operator==(const IO& o) const { return std::memcmp(this, &o, sizeof(IO)) == 0; }
 };
 // IO_SHARED_IN: a variations forward, one input image for the whole batch (its encoder runs at batch 1)
-enum IoMode : int { IO_U8_IN = 1, IO_U8_OUT = 2, IO_SHARED_IN = 4 };
+// IO_RAGGED: uint8 images of their own sizes, each resized to and from the one network size (i2it_forward_u8_ragged)
+enum IoMode : int { IO_U8_IN = 1, IO_U8_OUT = 2, IO_SHARED_IN = 4, IO_RAGGED = 8 };
 
 // uint8 HWC images [B][img bytes][w pixels per row][3] an op reads or writes: a caller pointer read from the plan's IO at
 // launch time (slot), or a plan-internal buffer (p); off selects a window's first pixel
@@ -143,6 +144,35 @@ struct U8View {
   int w = 0;
   uint8_t* get() const { return (slot ? static_cast<uint8_t*>(const_cast<void*>(*slot)) : p) + off; }
 };
+
+// Capacity buffers of a ragged plan (or a ragged resize op).  The descriptors and tables live in `dev`: [descs RsPass][tables],
+// rewritten by every call; the horizontal passes write the intermediates, the input side's vertical pass the network image
+// the packing kernel reads, and the output conversion the network image the output side's passes read.
+struct RaggedBufs {
+  int max_side = 0, descs = 0;
+  char* dev = nullptr;
+  size_t dev_bytes = 0;
+  uint8_t* in_mid = nullptr;       // [B][max_side][W][3]
+  uint8_t* in_net = nullptr;       // [B][H][W][3]
+  uint8_t* out_net = nullptr;      // [B][H][W][3]
+  uint8_t* out_mid = nullptr;      // [B][H][max_side][3]
+  size_t ops[4] = {0, 0, 0, 0};    // plan indices of the input side's h / v and the output side's h / v launches
+  const int* tab() const { return reinterpret_cast<const int*>(dev + descs * sizeof(RsPass)); }
+};
+
+// descriptors and tables of one ragged call, built on the host; bytes: algorithmic bytes of the four launches
+struct RsCall {
+  std::vector<RsPass> d;
+  std::vector<int> tab;
+  double bytes[4] = {0, 0, 0, 0};
+};
+// Rejects, with a message, a ragged forward geometry: non-positive sizes, a crop window outside its resized image, a dimension
+// above max_side.  Host only.
+void rs_check_ragged(const i2it_resize_desc* g, int n, int H, int W, int max_side);
+// The call's descriptors (input h, input v, output h, output v; n each) and tables.  x / out / rg may be null (host-only
+// sizing: the descriptors then carry null pointers).
+RsCall rs_forward_call(const i2it_resize_desc* g, int n, int H, int W, int max_side, RsTableCache& cache, const void* const* x,
+                       void* const* out, const RaggedBufs* rg);
 
 struct OpMeta {                  // bookkeeping for i2it_profile / bench roofline accounting
   std::string kind;              // "tapgemm:conv3x3", "gn_apply", ...
@@ -159,12 +189,13 @@ struct Plan {
   struct Trace { unsigned long long* buf; int grid; std::string what; };
   std::vector<Trace> traces;                           // I2IT_TRACE=1 only
   std::vector<std::shared_ptr<void>> keep;
-  std::vector<int> key;                                // (B, H, W, direction, text_batch, text_cached, io_mode[, resize geometry])
+  std::vector<int> key;                                // (B, H, W, direction, text_batch, text_cached, io_mode[, resize geometry | max_side])
   unsigned long long last_run = 0;                     // engine tick of the last forward (or the build): LRU eviction order
   void* u8_out_tmp = nullptr;                          // NCHW image the last conv writes when the caller wants uint8 HWC
   int* gn_counter = nullptr;                           // per-image tickets of the GroupNorm last-block reductions (zero between launches)
   std::vector<std::pair<size_t, const char*>> ranges;  // (first op index, name): NVTX stage ranges of the eager path
   bool debug_tapgemm = false;                          // a diagnostic op plan: its tapgemm launches take the engine's dbg_* override
+  RaggedBufs rg;                                       // IO_RAGGED plans and ragged resize ops
   IO io;
   std::vector<std::pair<IO, cudaGraphExec_t>> graphs;  // small cache: one instantiated graph per distinct IO pointer set
   ~Plan() { for (auto& g : graphs) cudaGraphExecDestroy(g.second); }
@@ -218,11 +249,15 @@ class Engine {
   void finalize(float lw_unet, float lw_vae, float skip_gamma, float twin_r);
   // g: LANCZOS resize geometry of a uint8 forward (i2it_forward_u8_resize); part of the plan key
   // evict: enforce the plan limit once the plan is in (forward() does it itself after the plan becomes the last-run one)
+  // max_side: the capacity of an IO_RAGGED plan (part of its key)
   Plan* plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached = false, int io_mode = 0,
-                 const i2it_resize_desc* g = nullptr, bool evict = true);
+                 const i2it_resize_desc* g = nullptr, bool evict = true, int max_side = 0);
   // shared_input: x / x_u8 hold ONE image that all B outputs start from (i2it_forward_variations); B == 1 is the plain forward
   void forward(const IO& io, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
                const i2it_resize_desc* g = nullptr, bool shared_input = false);
+  // B images of their own sizes (x[i], out[i], g[i]) through one IO_RAGGED plan of capacity max_side on an H x W network
+  void forward_ragged(const IO& io, const void* const* x, void* const* out, const i2it_resize_desc* g, int max_side, int B,
+                      int H, int W, int direction, int text_batch, cudaStream_t st);
   // cross-attention K / V^T of the prompt, computed once per prompt (i2it_set_text) instead of once per forward
   void set_text(const void* text, int text_batch, cudaStream_t st);
   // CLIP text tower (SURVEY 8f #1): tokens [batch, 77] int32 -> last_hidden_state [batch, 77, hidden] in the handle dtype
@@ -256,6 +291,11 @@ class Engine {
   // [B, H, W, 3]: the horizontal pass if the width changes, then the vertical pass if the height changes (at least one must)
   void resample_u8(Plan& P, const U8View& src, int B, int inH, int inW, int rsH, int rsW, int y0, int x0, int H, int W,
                    const U8View& dst);
+  // the ragged resize launches (horizontal, vertical) over descriptors [first, first + B) and [first + B, first + 2B) of P.rg;
+  // ops slot: where their plan indices go in P.rg.ops
+  void resample_ragged(Plan& P, int B, int first, int slot);
+  // i2it_op_resize_u8_ragged: x[i] [hw_in] -> out[i] [hw_out], with tables and intermediates sized by this call
+  void resize_ragged_op(Plan& P, const void* const* x, const int* hw_in, void* const* out, const int* hw_out, int n, int max_side);
   void copy_channels(Plan& P, const Act& src, const Act& dst_slice);
   Act replicate_image(Plan& P, const Act& src, int n);               // [1,H,W,C] -> [n,H,W,C], every image a copy of src
   // V^T[b] = Wv X[b]^T (+ row bias): returns [B][C][ldv] as an Act with N=B,H=1,W=C,ld=ldv (C field = Ntok)
@@ -331,6 +371,7 @@ class Engine {
   cudaStream_t gstream_ = nullptr;          // graphs are captured/replayed here (capture is illegal on the legacy stream)
   cudaEvent_t ev_in_ = nullptr, ev_out_ = nullptr;
   void check_device_error();
+  int graph_captures = 0;                   // CUDA graphs captured since create (i2it_debug_graph_captures)
 
  private:
   std::unordered_map<std::string, WT> w_;
@@ -359,6 +400,16 @@ class Engine {
   void evict_lru(const Plan* also_keep = nullptr, bool keep_last = true);
   void trim_arena(bool keep_last);                          // unmap what no resident plan needs
   std::map<std::vector<int>, std::unique_ptr<Plan>> plans_;
+  // run a forward plan on `st`: replay (or capture) its graph, or launch its ops; `before` is enqueued ahead of the first
+  // launch on the stream they run on
+  void run(Plan* P, const IO& io, cudaStream_t st, const std::function<void(cudaStream_t)>& before = nullptr);
+  // ragged calls: host tables, and the pinned blob one async copy per call moves into the plan's descriptor buffer; the blob
+  // is rewritten only after rs_ev_ says the previous copy has read it
+  RsTableCache rs_tables_;
+  char* rs_blob_ = nullptr;
+  size_t rs_blob_cap_ = 0;
+  cudaEvent_t rs_ev_ = nullptr;
+  size_t stage_ragged(const RsCall& c, size_t cap);     // fills the blob; returns its byte count
   Plan* last_plan_ = nullptr;
   Plan* last_text_plan_ = nullptr;   // the plan of the last encode_text (its stages: i2it_text_stage_names)
   Act text_;                     // staged text embedding while a UNet plan is being built

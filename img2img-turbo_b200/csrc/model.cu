@@ -502,10 +502,108 @@ void Engine::resample_u8(Plan& P, const U8View& src, int B, int inH, int inW, in
   }
 }
 
+void Engine::resample_ragged(Plan& P, int B, int first, int slot) {
+  const RsPass* d = reinterpret_cast<const RsPass*>(P.rg.dev) + first;
+  const int* tab = P.rg.tab();
+  // the grid depends on the device alone: its blocks stride over whatever rows the call has, so a captured launch serves any mix
+  const int grid = num_sms * 8;
+  const std::string shape = std::to_string(B) + " images, max_side " + std::to_string(P.rg.max_side);
+  P.rg.ops[slot] = P.ops.size();
+  add_op(P, [=](cudaStream_t st) {
+    launch_k(resample_h_ragged_kernel, dim3(grid), dim3(256), 0, st, 0, d, B, tab);
+  }, "resample_h_ragged", 0, 0, shape);
+  P.rg.ops[slot + 1] = P.ops.size();
+  add_op(P, [=](cudaStream_t st) {
+    launch_k(resample_v_ragged_kernel, dim3(grid), dim3(256), 0, st, 0, d + B, B, tab);
+  }, "resample_v_ragged", 0, 0, shape);
+}
+
+void Engine::resize_ragged_op(Plan& P, const void* const* x, const int* hw_in, void* const* out, const int* hw_out, int n,
+                              int max_side) {
+  I2IT_CHECK(n >= 1, "i2it_op_resize_u8_ragged: n must be >= 1");
+  I2IT_CHECK(max_side > 0, "i2it_op_resize_u8_ragged: max_side must be positive");
+  I2IT_CHECK(x && out && hw_in && hw_out, "i2it_op_resize_u8_ragged: null array");
+  std::vector<RsImage> im(n);
+  std::vector<size_t> mid_off(n);
+  size_t mid_bytes = 0;
+  for (int i = 0; i < n; ++i) {
+    const std::string at = " (image " + std::to_string(i) + ")";
+    const int H = hw_in[2 * i], W = hw_in[2 * i + 1], H2 = hw_out[2 * i], W2 = hw_out[2 * i + 1];
+    I2IT_CHECK(H > 0 && W > 0 && H2 > 0 && W2 > 0, "i2it_op_resize_u8_ragged: sizes must be positive" + at);
+    I2IT_CHECK(H <= max_side && W <= max_side && H2 <= max_side && W2 <= max_side,
+               "i2it_op_resize_u8_ragged: a dimension exceeds max_side (" + std::to_string(max_side) + ")" + at);
+    I2IT_CHECK(x[i] && out[i], "i2it_op_resize_u8_ragged: null image pointer" + at);
+    im[i] = RsImage{static_cast<const uint8_t*>(x[i]), static_cast<uint8_t*>(out[i]), nullptr, H, W, H2, W2, 0, 0, H2, W2};
+    const std::pair<int, int> rr = rs_rows(im[i], rs_tables_);
+    mid_off[i] = mid_bytes;
+    mid_bytes += static_cast<size_t>(rr.second - rr.first) * W2 * 3;
+  }
+  auto mid = alloc_raw(P, mid_bytes);
+  P.keep.push_back(mid);
+  RsCall c;
+  std::vector<RsPass> v;
+  for (int i = 0; i < n; ++i) {
+    im[i].mid = static_cast<uint8_t*>(mid.get()) + mid_off[i];
+    rs_add_image(im[i], rs_tables_, c.d, v, c.tab, c.bytes);
+  }
+  c.d.insert(c.d.end(), v.begin(), v.end());
+  const size_t dbytes = c.d.size() * sizeof(RsPass);
+  P.rg.max_side = max_side;
+  P.rg.descs = 2 * n;
+  P.rg.dev_bytes = dbytes + c.tab.size() * sizeof(int);
+  P.rg.dev = static_cast<char*>(P.pool.get_fresh(P.rg.dev_bytes));
+  I2IT_CUDA(cudaMemcpy(P.rg.dev, c.d.data(), dbytes, cudaMemcpyHostToDevice));
+  I2IT_CUDA(cudaMemcpy(P.rg.dev + dbytes, c.tab.data(), c.tab.size() * sizeof(int), cudaMemcpyHostToDevice));
+  resample_ragged(P, n, 0, 0);
+  P.meta[P.rg.ops[0]].bytes = c.bytes[0];
+  P.meta[P.rg.ops[1]].bytes = c.bytes[1];
+}
+
+void rs_check_ragged(const i2it_resize_desc* g, int n, int H, int W, int max_side) {
+  I2IT_CHECK(max_side > 0, "ragged forward: max_side must be positive");
+  I2IT_CHECK(g != nullptr && n > 0, "ragged forward: no geometry");
+  for (int i = 0; i < n; ++i) {
+    const i2it_resize_desc& d = g[i];
+    const std::string at = " (image " + std::to_string(i) + ")";
+    I2IT_CHECK(d.in_H > 0 && d.in_W > 0 && d.resize_H > 0 && d.resize_W > 0 && d.out_H > 0 && d.out_W > 0,
+               "resize geometry: sizes must be positive" + at);
+    I2IT_CHECK(d.crop_y >= 0 && d.crop_x >= 0 && d.crop_y + H <= d.resize_H && d.crop_x + W <= d.resize_W,
+               "resize geometry: the H x W crop window lies outside the resized image" + at);
+    I2IT_CHECK(d.in_H <= max_side && d.in_W <= max_side && d.resize_H <= max_side && d.resize_W <= max_side &&
+               d.out_H <= max_side && d.out_W <= max_side,
+               "resize geometry: a dimension exceeds max_side (" + std::to_string(max_side) + ")" + at);
+  }
+}
+
+static uint8_t* rs_at(uint8_t* p, long long off) { return p ? p + off : nullptr; }
+
+RsCall rs_forward_call(const i2it_resize_desc* g, int n, int H, int W, int max_side, RsTableCache& cache, const void* const* x,
+                       void* const* out, const RaggedBufs* rg) {
+  RsCall c;
+  std::vector<RsPass> d[4];
+  const long long net = 3ll * H * W;
+  for (int i = 0; i < n; ++i) {
+    const i2it_resize_desc& e = g[i];
+    const RsImage in{x ? static_cast<const uint8_t*>(x[i]) : nullptr, rg ? rs_at(rg->in_net, i * net) : nullptr,
+                     rg ? rs_at(rg->in_mid, i * 3ll * max_side * W) : nullptr, e.in_H, e.in_W, e.resize_H, e.resize_W,
+                     e.crop_y, e.crop_x, H, W};
+    const RsImage o{rg ? rs_at(rg->out_net, i * net) : nullptr, out ? static_cast<uint8_t*>(out[i]) : nullptr,
+                    rg ? rs_at(rg->out_mid, i * 3ll * H * max_side) : nullptr, H, W, e.out_H, e.out_W, 0, 0, e.out_H, e.out_W};
+    rs_add_image(in, cache, d[0], d[1], c.tab, c.bytes);
+    rs_add_image(o, cache, d[2], d[3], c.tab, c.bytes + 2);
+  }
+  for (auto& v : d) c.d.insert(c.d.end(), v.begin(), v.end());
+  I2IT_CHECK(static_cast<long long>(c.tab.size()) <= rs_forward_bound(n, H, W, max_side),
+             "ragged resize: the call's tables exceed the plan's bound");
+  return c;
+}
+
 Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached, int io_mode,
-                       const i2it_resize_desc* g, bool evict) {
+                       const i2it_resize_desc* g, bool evict, int max_side) {
   std::vector<int> key{B, H, W, direction, text_batch, text_cached ? 1 : 0, io_mode};
   if (g) key.insert(key.end(), {g->in_H, g->in_W, g->resize_H, g->resize_W, g->crop_y, g->crop_x, g->out_H, g->out_W});
+  const bool ragged = (io_mode & IO_RAGGED) != 0;
+  if (ragged) key.push_back(max_side);
   auto it = plans_.find(key);
   if (it != plans_.end()) return it->second.get();
   I2IT_CHECK(finalized_, "i2it_finalize_weights must be called before a forward");
@@ -533,7 +631,24 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
   // what the first kernel reads: the caller's [B, H, W, 3] image, or with a geometry the H x W network window of its resize
   U8View net_in;
   net_in.slot = &P.io.x_u8; net_in.img = 3ll * H * W; net_in.w = W;
-  if (g) {
+  if (ragged) {
+    // capacity buffers: every call's images fit them (rs_check_ragged), so the plan and its graph serve any mix of sizes
+    I2IT_CHECK(max_side > 0, "ragged plan: max_side must be positive");
+    P.rg.max_side = max_side;
+    P.rg.descs = 4 * B;
+    P.rg.dev_bytes = 4 * static_cast<size_t>(B) * sizeof(RsPass) + rs_forward_bound(B, H, W, max_side) * sizeof(int);
+    P.rg.dev = static_cast<char*>(P.pool.get_fresh(P.rg.dev_bytes));
+    auto mid = alloc_raw(P, static_cast<size_t>(B) * max_side * W * 3);
+    auto img = alloc_raw(P, static_cast<size_t>(B) * H * W * 3);
+    P.keep.push_back(mid);
+    P.keep.push_back(img);
+    P.rg.in_mid = static_cast<uint8_t*>(mid.get());
+    P.rg.in_net = static_cast<uint8_t*>(img.get());
+    P.ranges.emplace_back(P.ops.size(), "resize_in");
+    resample_ragged(P, B, 0, 0);
+    net_in = U8View();
+    net_in.p = P.rg.in_net; net_in.img = 3ll * H * W; net_in.w = W;
+  } else if (g) {
     net_in.img = 3ll * g->in_H * g->in_W; net_in.w = g->in_W;
     if (g->in_H == g->resize_H && g->in_W == g->resize_W) {
       net_in.off = 3 * (static_cast<long long>(g->crop_y) * g->in_W + g->crop_x);   // a crop of the input itself: no pass
@@ -584,7 +699,7 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
     Plan* plan = &P;
     U8View out;
     out.slot = &P.io.out_u8; out.img = 3 * HW; out.w = W;
-    const bool resize_out = g && (g->out_H != H || g->out_W != W);
+    const bool resize_out = ragged || (g && (g->out_H != H || g->out_W != W));
     U8View net_out = out;
     if (resize_out) {
       auto buf = alloc_raw(P, static_cast<size_t>(total) * 3);
@@ -596,7 +711,14 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
       DISPATCH_T(dt, (launch_k(nchw_to_u8hwc_kernel<T>, dim3(ceil_div_i(total, 256)), dim3(256), 0, st, 0,
                          reinterpret_cast<const T*>(plan->io.out), net_out.get(), HW, total)));
     }, "unpack_u8", 0, 1.0 * total * (6 + 3));
-    if (resize_out) {
+    if (ragged) {
+      auto mid = alloc_raw(P, static_cast<size_t>(B) * H * max_side * 3);
+      P.keep.push_back(mid);
+      P.rg.out_net = net_out.p;
+      P.rg.out_mid = static_cast<uint8_t*>(mid.get());
+      P.ranges.emplace_back(P.ops.size(), "resize_out");
+      resample_ragged(P, B, 2 * B, 2);
+    } else if (resize_out) {
       out.img = 3ll * g->out_H * g->out_W; out.w = g->out_W;
       P.ranges.emplace_back(P.ops.size(), "resize_out");
       resample_u8(P, net_out, B, H, W, g->out_H, g->out_W, 0, 0, g->out_H, g->out_W, out);

@@ -7,6 +7,9 @@
 // uploaded once per plan: device sin differs in the last bits, and a last-bit difference can move a fixed-point rounding.
 #pragma once
 #include <cmath>
+#include <map>
+#include <memory>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -75,6 +78,21 @@ __device__ __forceinline__ uint8_t rs_clip8(int acc) {
   return static_cast<uint8_t>(v < 0 ? 0 : (v > 255 ? 255 : v));
 }
 
+// One output pixel of a pass: n taps k[0 .. n) over the RGB pixels s, s + step, s + 2 step, ... (step 3 along a row, the row
+// pitch down a column), accumulated in int32 from 2^21, rounded and clipped to uint8.  Every pass, fixed or ragged, runs this.
+__device__ __forceinline__ void rs_taps(const uint8_t* __restrict__ s, long long step, const int* __restrict__ k, int n,
+                                        uint8_t* __restrict__ d) {
+  int a0 = 1 << (RS_PRECISION_BITS - 1), a1 = a0, a2 = a0;
+  for (int t = 0; t < n; ++t) {
+    const int c = __ldg(k + t);
+    const uint8_t* q = s + t * step;
+    a0 += c * q[0];
+    a1 += c * q[1];
+    a2 += c * q[2];
+  }
+  d[0] = rs_clip8(a0); d[1] = rs_clip8(a1); d[2] = rs_clip8(a2);
+}
+
 // Horizontal pass: dst [B, rows, Wo, 3] = src rows row0 .. row0+rows-1 resampled along x, output columns x0 .. x0+Wo-1 of
 // the table (a crop window).  src: [B][img / (src_w*3)][src_w][3], img bytes per image.  One thread per output pixel.
 static __global__ void resample_h_u8_kernel(const uint8_t* __restrict__ src, long long src_img, int src_w, int row0,
@@ -88,17 +106,8 @@ static __global__ void resample_h_u8_kernel(const uint8_t* __restrict__ src, lon
   const int r = static_cast<int>(br % rows);
   const long long b = br / rows;
   const int xo = x0 + j, xmin = bounds[2 * xo], n = bounds[2 * xo + 1];
-  const int* k = coeffs + static_cast<long long>(xo) * ksize;
   const uint8_t* s = src + b * src_img + (static_cast<long long>(row0 + r) * src_w + xmin) * 3;
-  int a0 = 1 << (RS_PRECISION_BITS - 1), a1 = a0, a2 = a0;
-  for (int t = 0; t < n; ++t) {
-    const int c = __ldg(k + t);
-    a0 += c * s[3 * t];
-    a1 += c * s[3 * t + 1];
-    a2 += c * s[3 * t + 2];
-  }
-  uint8_t* d = dst + i * 3;
-  d[0] = rs_clip8(a0); d[1] = rs_clip8(a1); d[2] = rs_clip8(a2);
+  rs_taps(s, 3, coeffs + static_cast<long long>(xo) * ksize, n, dst + i * 3);
 }
 
 // Vertical pass: dst [B, Ho, Wo, 3] = output rows y0 .. y0+Ho-1 of the table, read from src columns col0 .. col0+Wo-1;
@@ -115,19 +124,154 @@ static __global__ void resample_v_u8_kernel(const uint8_t* __restrict__ src, lon
   const int h = static_cast<int>(bh % Ho);
   const long long b = bh / Ho;
   const int yo = y0 + h, ymin = bounds[2 * yo] - row_shift, n = bounds[2 * yo + 1];
-  const int* k = coeffs + static_cast<long long>(yo) * ksize;
   const long long pitch = static_cast<long long>(src_w) * 3;
   const uint8_t* s = src + b * src_img + static_cast<long long>(ymin) * pitch + static_cast<long long>(col0 + j) * 3;
-  int a0 = 1 << (RS_PRECISION_BITS - 1), a1 = a0, a2 = a0;
-  for (int t = 0; t < n; ++t) {
-    const int c = __ldg(k + t);
-    const uint8_t* q = s + t * pitch;
-    a0 += c * q[0];
-    a1 += c * q[1];
-    a2 += c * q[2];
+  rs_taps(s, pitch, coeffs + static_cast<long long>(yo) * ksize, n, dst + i * 3);
+}
+
+// ------------------------------------------------------------------------------------------ ragged passes
+// Every image of a batch with its own sizes, through one horizontal and one vertical launch.  Each image has a descriptor per
+// pass in device memory, written by the host for every call; the grid is fixed by the plan, and its blocks stride over the
+// call's output rows (image by image: item0 counts the rows of the images before), so one captured graph serves any mix.
+//
+// One image of one ragged pass: `rows` output rows of `cols` pixels.  Its table, at `tab` ints into the table area, holds
+// the window's outputs only: bounds [outputs][2] (first source index, taps) then coefficients [outputs][ksize].
+//   horizontal: output row r is source row row0 + r; output column j takes table row j
+//   vertical:   output row r takes table row r and reads source rows from bounds[r].first - row0 (the horizontal pass made
+//               only the rows from row0 on); output column j is source column j
+struct RsPass {
+  const uint8_t* src;
+  uint8_t* dst;
+  long long src_pitch, dst_pitch;   // bytes per row
+  long long tab;
+  long long item0;
+  int rows, cols, ksize, row0;
+};
+
+// the image whose rows hold work item `it`: the last one with item0 <= it (item0 ascends from 0)
+__device__ __forceinline__ int rs_image_of(const RsPass* __restrict__ d, int n, long long it) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (d[mid].item0 <= it) lo = mid; else hi = mid - 1;
   }
-  uint8_t* d = dst + i * 3;
-  d[0] = rs_clip8(a0); d[1] = rs_clip8(a1); d[2] = rs_clip8(a2);
+  return lo;
+}
+
+static __global__ void resample_h_ragged_kernel(const RsPass* __restrict__ d, int n, const int* __restrict__ tab) {
+  pdl_sync();
+  const long long total = d[n - 1].item0 + d[n - 1].rows;
+  for (long long it = blockIdx.x; it < total; it += gridDim.x) {
+    const RsPass p = d[rs_image_of(d, n, it)];
+    const long long r = it - p.item0;
+    const int* bounds = tab + p.tab;
+    const int* coeffs = bounds + 2ll * p.cols;
+    const uint8_t* s = p.src + (p.row0 + r) * p.src_pitch;
+    uint8_t* o = p.dst + r * p.dst_pitch;
+    for (int j = threadIdx.x; j < p.cols; j += blockDim.x)
+      rs_taps(s + 3ll * bounds[2 * j], 3, coeffs + static_cast<long long>(j) * p.ksize, bounds[2 * j + 1], o + 3ll * j);
+  }
+}
+
+static __global__ void resample_v_ragged_kernel(const RsPass* __restrict__ d, int n, const int* __restrict__ tab) {
+  pdl_sync();
+  const long long total = d[n - 1].item0 + d[n - 1].rows;
+  for (long long it = blockIdx.x; it < total; it += gridDim.x) {
+    const RsPass p = d[rs_image_of(d, n, it)];
+    const int r = static_cast<int>(it - p.item0);
+    const int* bounds = tab + p.tab;
+    const int* k = bounds + 2ll * p.rows + static_cast<long long>(r) * p.ksize;
+    const int taps = bounds[2 * r + 1];
+    const uint8_t* s = p.src + static_cast<long long>(bounds[2 * r] - p.row0) * p.src_pitch;
+    uint8_t* o = p.dst + r * p.dst_pitch;
+    for (int j = threadIdx.x; j < p.cols; j += blockDim.x) rs_taps(s + 3ll * j, p.src_pitch, k, taps, o + 3ll * j);
+  }
+}
+
+// ---- host side of the ragged passes ----
+// lanczos_table per (in, out) pair, kept across calls: building one calls sin for every tap
+class RsTableCache {
+ public:
+  std::shared_ptr<const ResampleTable> get(int in, int out) {
+    auto it = m_.find({in, out});
+    if (it != m_.end()) return it->second;
+    if (m_.size() >= 512) m_.clear();
+    auto t = std::make_shared<const ResampleTable>(lanczos_table(in, out));
+    m_[{in, out}] = t;
+    return t;
+  }
+ private:
+  std::map<std::pair<int, int>, std::shared_ptr<const ResampleTable>> m_;
+};
+
+// Table ints of one ragged pass of `win` outputs from `in` samples: 2 bounds per output plus ksize coefficients, where
+// ksize = 2 ceil(3 fs) + 1 with fs = max(in / out, 1) and out >= win the resized size.  Downscaling, ceil(3 fs) <= 3 fs + 1
+// gives ksize <= 6 in / out + 3, so ksize win <= 6 in + 3 win; upscaling, ksize = 7; an identity pass has ksize 1.  Hence
+// at most 2 win + max(6 in + 3 win, 7 win) <= 6 in + 9 win, monotone in both, so capacities bound every call.
+inline long long rs_pass_bound(long long in, long long win) { return 6 * in + 9 * win; }
+
+// table area of a ragged forward plan of B images on an H x W network with capacity max_side: per image, the input side's
+// passes (from at most max_side to W columns and H rows) and the output side's (from W columns and H rows to at most max_side)
+inline long long rs_forward_bound(long long B, long long H, long long W, long long max_side) {
+  return B * (rs_pass_bound(max_side, W) + rs_pass_bound(max_side, H) + rs_pass_bound(W, max_side) + rs_pass_bound(H, max_side));
+}
+
+// One image of a ragged resize: src [inH, inW, 3] resized to rsH x rsW, window (y0, x0, H, W) written densely to
+// dst [H, W, 3]; mid holds its horizontal pass's rows [rows, W, 3].
+struct RsImage {
+  const uint8_t* src;
+  uint8_t* dst;
+  uint8_t* mid;
+  int inH, inW, rsH, rsW, y0, x0, H, W;
+};
+
+// source rows [r0, r1) the vertical pass of `m` reads: what its horizontal pass makes
+inline std::pair<int, int> rs_rows(const RsImage& m, RsTableCache& cache) {
+  if (m.inH == m.rsH) return {m.y0, m.y0 + m.H};
+  const auto t = cache.get(m.inH, m.rsH);
+  const size_t last = 2 * static_cast<size_t>(m.y0 + m.H - 1);
+  return {t->bounds[2 * static_cast<size_t>(m.y0)], t->bounds[last] + t->bounds[last + 1]};
+}
+
+// Appends the window [first, first + count) of the (in -> out) table to `tab`; returns its offset and sets ksize.  With
+// in == out it is the identity: one tap of weight 1 << 22 per output, and (2^21 + v 2^22) >> 22 == v, the bytes PIL keeps
+// when it skips the pass.
+inline long long rs_put_table(std::vector<int>& tab, RsTableCache& cache, int in, int out, int first, int count, int* ksize) {
+  const long long off = static_cast<long long>(tab.size());
+  if (in == out) {
+    *ksize = 1;
+    for (int j = 0; j < count; ++j) { tab.push_back(first + j); tab.push_back(1); }
+    tab.insert(tab.end(), count, 1 << RS_PRECISION_BITS);
+    return off;
+  }
+  const auto t = cache.get(in, out);
+  *ksize = t->ksize;
+  tab.insert(tab.end(), t->bounds.begin() + 2 * static_cast<size_t>(first), t->bounds.begin() + 2 * static_cast<size_t>(first + count));
+  tab.insert(tab.end(), t->coeffs.begin() + static_cast<size_t>(first) * t->ksize,
+             t->coeffs.begin() + static_cast<size_t>(first + count) * t->ksize);
+  return off;
+}
+
+// Appends image m's horizontal pass to h, its vertical pass to v and their tables to tab; bytes[0] / bytes[1] accumulate the
+// passes' algorithmic bytes (pixels read and written, tables read).
+inline void rs_add_image(const RsImage& m, RsTableCache& cache, std::vector<RsPass>& h, std::vector<RsPass>& v,
+                         std::vector<int>& tab, double bytes[2]) {
+  const std::pair<int, int> rr = rs_rows(m, cache);
+  RsPass ph{}, pv{};
+  pv.tab = rs_put_table(tab, cache, m.inH, m.rsH, m.y0, m.H, &pv.ksize);
+  ph.tab = rs_put_table(tab, cache, m.inW, m.rsW, m.x0, m.W, &ph.ksize);
+  const int* hb = tab.data() + ph.tab;
+  const long long span = hb[2 * (m.W - 1)] + hb[2 * (m.W - 1) + 1] - hb[0];
+  ph.src = m.src; ph.src_pitch = 3ll * m.inW; ph.row0 = rr.first; ph.rows = rr.second - rr.first; ph.cols = m.W;
+  ph.dst = m.mid; ph.dst_pitch = 3ll * m.W;
+  ph.item0 = h.empty() ? 0 : h.back().item0 + h.back().rows;
+  pv.src = m.mid; pv.src_pitch = 3ll * m.W; pv.row0 = rr.first; pv.rows = m.H; pv.cols = m.W;
+  pv.dst = m.dst; pv.dst_pitch = 3ll * m.W;
+  pv.item0 = v.empty() ? 0 : v.back().item0 + v.back().rows;
+  h.push_back(ph);
+  v.push_back(pv);
+  bytes[0] += 3.0 * ph.rows * (span + m.W) + 4.0 * m.W * (2 + ph.ksize);
+  bytes[1] += 3.0 * m.W * (ph.rows + m.H) + 4.0 * m.H * (2 + pv.ksize);
 }
 
 }  // namespace i2it

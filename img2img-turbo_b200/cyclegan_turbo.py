@@ -203,3 +203,27 @@ class CycleGAN_Turbo(TurboBase):
         eng = self._finalize(1.0, 1.0, 1.0, -1.0)
         return self._staged_forward(eng, x, text, eps, direction=i2it.A2B if direction == "a2b" else i2it.B2A,
                                     u8_mode=i2it.IN_NORMALIZE, geometry=geom)
+
+    def forward_u8_batch(self, images, direction=None, caption=None, caption_emb=None, *, image_prep="resize_512x512", eps=None):
+        """inference_unpaired.py (:40-53) on a list of uploads of their own sizes in one forward: images[i] [H_i, W_i, 3] uint8
+        -> a list of uint8 CUDA tensors [H_i, W_i, 3].  Each image goes through build_transform(image_prep)
+        (_host.image_prep_geometry: ValueError for the random crops) and comes back at its input size, all on device
+        (i2it.Engine.forward_u8_ragged).  The preps must give every image the same network size; eps is [B,4,H/8,W/8] of it.
+        Output i equals forward_u8(images[i][None], eps=eps[i:i+1], resize=, crop=, out_size=(H_i, W_i)) byte for byte."""
+        if direction is None:
+            assert self.direction is not None
+            direction = self.direction
+        if caption is None and caption_emb is None:
+            assert self.caption is not None
+            caption = self.caption
+        assert direction in ["a2b", "b2a"]
+        dt = self.compute_dtype
+        text = self._prep(caption_emb if caption_emb is not None else self._encode_text(caption), dt)
+        xs = [x.to(device=_host.DEVICE, non_blocking=True).contiguous() for x in images]
+        H, Wd, geoms = _host.ragged_geometries([tuple(x.shape[:2]) for x in xs], image_prep=image_prep)
+        if eps is None:
+            eps = torch.randn((len(xs), 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)
+        eps = self._prep(eps, dt)
+        eng = self._finalize(1.0, 1.0, 1.0, -1.0)
+        return self._staged_forward(eng, xs, text, eps, direction=i2it.A2B if direction == "a2b" else i2it.B2A,
+                                    u8_mode=i2it.IN_NORMALIZE, ragged=geoms)

@@ -34,6 +34,7 @@ SYMBOLS = [
     "i2it_forward_u8_resize", "i2it_op_resize_u8", "i2it_debug_resample_coeffs",
     "i2it_set_max_plans", "i2it_release_plans", "i2it_memory_stats_get", "i2it_debug_poison_workspace",
     "i2it_debug_tapgemm_override", "i2it_forward_variations", "i2it_forward_u8_variations",
+    "i2it_forward_u8_ragged", "i2it_op_resize_u8_ragged", "i2it_debug_ragged_tables", "i2it_debug_graph_captures",
 ]
 TEXT_TOKEN_EMB = "text_encoder.text_model.embeddings.token_embedding.weight"
 TEXT_POS_EMB = "text_encoder.text_model.embeddings.position_embedding.weight"
@@ -80,6 +81,37 @@ def resize_geometry(in_hw, resize=None, crop=None, out_size=None):
     if len(rs) != 2 or len(cr) != 4 or len(out) != 2:
         raise ValueError("resize and out_size are (H, W), crop is (top, left, height, width)")
     return rs, cr, out
+
+
+def ragged_max_side(sizes) -> int:
+    """Default capacity of a ragged forward: the largest of `sizes` rounded up to a multiple of 1024, at least 4096, so an
+    ordinary stream of uploads runs on one plan per batch size."""
+    return max(4096, -(-max(int(v) for v in sizes) // 1024) * 1024)
+
+
+def _ragged_descs(geometries, in_hws):
+    """(H, W, ResizeDesc array) of a ragged call: geometries[i] holds image i's forward_u8 keywords (resize, crop, out_size;
+    each may be absent or None); every crop must have the same size, the network's."""
+    if len(geometries) != len(in_hws):
+        raise ValueError(f"{len(in_hws)} images but {len(geometries)} geometries")
+    descs, net = (ResizeDesc * len(in_hws))(), set()
+    for i, (hw, g) in enumerate(zip(in_hws, geometries)):
+        rs, cr, osz = resize_geometry(hw, g.get("resize"), g.get("crop"), g.get("out_size"))
+        net.add(cr[2:])
+        descs[i] = ResizeDesc(hw[0], hw[1], rs[0], rs[1], cr[0], cr[1], osz[0], osz[1])
+    if len(net) != 1:
+        raise ValueError(f"a ragged batch runs one network size; its geometries give {sorted(net)}")
+    H, W = net.pop()
+    return H, W, descs
+
+
+def ragged_table_ints(geometries, in_hws, max_side: int):
+    """(used, bound): coefficient-table ints a ragged forward on these images uploads, and what its plan reserves (host only)."""
+    H, W, descs = _ragged_descs(geometries, in_hws)
+    used, bound = C.c_longlong(0), C.c_longlong(0)
+    if load_library().i2it_debug_ragged_tables(descs, len(in_hws), H, W, int(max_side), C.byref(used), C.byref(bound)) != 0:
+        raise ValueError("the ragged forward would reject these geometries")
+    return used.value, bound.value
 
 
 def resample_coeffs(in_size: int, out_size: int):
@@ -174,6 +206,12 @@ def load_library(path: Optional[str] = None):
     lib.i2it_forward_variations.argtypes = [vp, vp, vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci, vp]
     lib.i2it_forward_u8_variations.argtypes = [vp, vp, ci, C.POINTER(ResizeDesc), vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci,
                                                vp]
+    lib.i2it_forward_u8_ragged.argtypes = [vp, C.POINTER(vp), ci, C.POINTER(ResizeDesc), ci, vp, ci, vp, vp, cf, C.POINTER(vp),
+                                           vp, ci, ci, ci, ci, vp]
+    lib.i2it_op_resize_u8_ragged.argtypes = [vp, C.POINTER(vp), C.POINTER(ci), C.POINTER(vp), C.POINTER(ci), ci, ci, vp]
+    lib.i2it_debug_ragged_tables.argtypes = [C.POINTER(ResizeDesc), ci, ci, ci, ci, C.POINTER(C.c_longlong),
+                                             C.POINTER(C.c_longlong)]
+    lib.i2it_debug_graph_captures.argtypes = [vp, C.POINTER(ci)]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("i2it_destroy", "i2it_last_error"):
@@ -184,6 +222,17 @@ def load_library(path: Optional[str] = None):
 
 def _ptr(t: Optional[torch.Tensor]):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+
+
+def _ptrs(ts):
+    return (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+
+def _check_u8_images(images, what):
+    for x in images:
+        if not (x.dim() == 3 and x.shape[2] == 3 and x.dtype == torch.uint8 and x.is_cuda and x.is_contiguous()):
+            raise ValueError(f"{what}: every image must be a contiguous uint8 CUDA tensor [H, W, 3], got "
+                             f"{x.dtype} {list(x.shape)}{'' if x.is_cuda else ' on the CPU'}")
 
 
 def _stream():
@@ -388,6 +437,41 @@ class Engine:
                                                         H, W, direction, _stream()), "i2it_forward_u8_variations")
         return out
 
+    def forward_u8_ragged(self, images: Sequence[torch.Tensor], in_mode: int, text_emb: Optional[torch.Tensor],
+                          eps: torch.Tensor, noise_map: Optional[torch.Tensor] = None, r: float = 1.0, direction: int = A2B, *,
+                          geometries, max_side: Optional[int] = None, outs: Optional[Sequence[torch.Tensor]] = None,
+                          out_latent: Optional[torch.Tensor] = None):
+        """forward_u8 on n = len(images) uint8 images of their own sizes ([H_i, W_i, 3] contiguous CUDA tensors) in one forward
+        at batch n.  geometries[i] is image i's forward_u8 keywords as a dict (resize, crop, out_size); every crop has the
+        network size H x W, and eps / noise_map / out_latent are [n, 4, H/8, W/8].  Returns the n outputs [out_H_i, out_W_i, 3]
+        (or fills `outs`).  Output i equals forward_u8(images[i][None], ..., **geometries[i]) with eps[i], byte for byte.
+
+        max_side: the plan's capacity, at least every in / resize / out dimension; None takes ragged_max_side of the call's
+        dimensions, so a stream of calls with the same n reuses one plan and one graph."""
+        n = len(images)
+        _check_u8_images(images, "forward_u8_ragged")
+        H, W, descs = _ragged_descs(geometries, [tuple(x.shape[:2]) for x in images])
+        if eps.shape[0] != n:
+            raise ValueError(f"{n} images but eps has batch {eps.shape[0]}")
+        tb = self._check_operands(n, H, W, text_emb, eps, (noise_map, out_latent))
+        if max_side is None:
+            max_side = ragged_max_side([v for d in descs for v in (d.in_H, d.in_W, d.resize_H, d.resize_W, d.out_H, d.out_W)])
+        if outs is None:
+            outs = [torch.empty(d.out_H, d.out_W, 3, dtype=torch.uint8, device=images[0].device) for d in descs]
+        if len(outs) != n or any(tuple(o.shape) != (d.out_H, d.out_W, 3) or o.dtype != torch.uint8 or not o.is_cuda
+                                 or not o.is_contiguous() for o, d in zip(outs, descs)):
+            raise ValueError("outs must be n contiguous uint8 CUDA tensors [out_H_i, out_W_i, 3]")
+        self._check(self.lib.i2it_forward_u8_ragged(self._h, _ptrs(images), int(in_mode), descs, int(max_side), _ptr(text_emb), tb,
+                                                    _ptr(eps), _ptr(noise_map), float(r), _ptrs(outs), _ptr(out_latent), n, H,
+                                                    W, direction, _stream()), "i2it_forward_u8_ragged")
+        return list(outs)
+
+    def graph_captures(self) -> int:
+        """CUDA graphs this engine has captured (a replayed forward captures none)."""
+        n = C.c_int(0)
+        self._check(self.lib.i2it_debug_graph_captures(self._h, C.byref(n)), "i2it_debug_graph_captures")
+        return n.value
+
     def prep_launch_count(self) -> int:
         n = C.c_int(0)
         self._check(self.lib.i2it_prep_launch_count(self._h, C.byref(n)), "i2it_prep_launch_count")
@@ -589,3 +673,20 @@ class Engine:
         out = torch.empty(B, H2, W2, 3, dtype=torch.uint8, device=x.device)
         self._check(self.lib.i2it_op_resize_u8(self._h, _ptr(x), B, H, W, _ptr(out), H2, W2, _stream()), "i2it_op_resize_u8")
         return out
+
+    def op_resize_u8_ragged(self, images, sizes, max_side: Optional[int] = None):
+        """PIL LANCZOS resize of uint8 HWC CUDA images of their own sizes, images[i] [H_i, W_i, 3] -> [sizes[i][0], sizes[i][1], 3],
+        in the two ragged launches of forward_u8_ragged (synchronous).  max_side None: ragged_max_side of the sizes."""
+        n = len(images)
+        _check_u8_images(images, "op_resize_u8_ragged")
+        if len(sizes) != n:
+            raise ValueError(f"{n} images but {len(sizes)} sizes")
+        hw_in = [int(v) for x in images for v in x.shape[:2]]
+        hw_out = [int(v) for s in sizes for v in s]
+        if max_side is None:
+            max_side = ragged_max_side(hw_in + hw_out)
+        outs = [torch.empty(int(s[0]), int(s[1]), 3, dtype=torch.uint8, device=images[0].device) for s in sizes]
+        self._check(self.lib.i2it_op_resize_u8_ragged(self._h, _ptrs(images), (C.c_int * (2 * n))(*hw_in), _ptrs(outs),
+                                                      (C.c_int * (2 * n))(*hw_out), n, int(max_side), _stream()),
+                    "i2it_op_resize_u8_ragged")
+        return outs

@@ -236,6 +236,21 @@ class Pix2Pix_Turbo(TurboBase):
         mode = i2it.IN_SKETCH if sketch else i2it.IN_UNIT
         return self._fold_and_run(x, caption_enc, eps, B, deterministic, r, noise_map, u8_mode=mode, geometry=geom)
 
+    def forward_u8_batch(self, images, prompt=None, prompt_tokens=None, deterministic=True, r=1.0, noise_map=None, *,
+                         resize=(512, 512), sketch=False, eps=None):
+        """forward_u8 on a list of images of their own sizes in one forward: images[i] [H_i, W_i, 3] uint8 -> a list of uint8
+        CUDA tensors [H_i, W_i, 3].  Every image is LANCZOS-resized to `resize` (H, W), the network size, and its output back
+        to its input size, on device (i2it.Engine.forward_u8_ragged).  eps / noise_map are [B,4,H/8,W/8] of `resize`.
+        Output i equals forward_u8(images[i][None], ..., eps=eps[i:i+1], resize=resize, out_size=(H_i, W_i)) byte for byte."""
+        assert (prompt is None) != (prompt_tokens is None), "Either prompt or prompt_tokens should be provided"
+        caption_enc = self._encode_text(prompt, prompt_tokens)
+        xs = [x.to(device=_host.DEVICE, non_blocking=True).contiguous() for x in images]
+        H, Wd, geoms = _host.ragged_geometries([tuple(x.shape[:2]) for x in xs], resize=resize)
+        B = len(xs)
+        eps = self._draw_eps(eps, B, H, Wd)
+        mode = i2it.IN_SKETCH if sketch else i2it.IN_UNIT
+        return self._fold_and_run(xs, caption_enc, eps, B, deterministic, r, noise_map, u8_mode=mode, ragged=geoms)
+
     def variations_u8(self, images_u8, prompt=None, prompt_tokens=None, deterministic=True, r=1.0, noise_map=None, *, n=None,
                       eps=None, sketch=False, resize=None, crop=None, out_size=None):
         """variations() on the uint8 HWC boundary of forward_u8: ONE image [1,H,W,3] uint8 -> [n,out_H,out_W,3] uint8 CUDA.

@@ -202,6 +202,25 @@ int i2it_forward_u8_variations(i2it_handle* h, const void* x_u8_hwc, int in_mode
                                int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc,
                                void* out_latent, int n, int H, int W, int direction, void* stream);
 
+/* n uint8 images of their own sizes through one forward at batch n on an H x W network:
+ *   x_u8[i]   [g[i].in_H, g[i].in_W, 3]    device pointers, one per image
+ *   out_u8[i] [g[i].out_H, g[i].out_W, 3]  device pointers, one per image
+ *   g[i]      image i's resize geometry (i2it_resize_desc; its crop window is H x W)
+ *   eps / noise_map / out_latent [n, 4, H/8, W/8], text_emb [text_batch, 77, cross] or NULL, as in i2it_forward_u8.
+ * Each image goes through exactly the passes of i2it_forward_u8_resize, so output i is byte-equal to a batch-1
+ * i2it_forward_u8_resize of image i with eps[i] and noise_map[i].  A dimension that does not change is an identity pass,
+ * so every call makes two resize launches per side.
+ * The plan is keyed by (n, H, W, direction, text mode, max_side) and by no image size: max_side is a capacity that
+ * every in_*, resize_* and out_* size of the call must not exceed, and its buffers are sized by it.  Each call
+ * builds its descriptors and coefficient tables on the host (tables cached per size pair) and copies them to the plan with
+ * one asynchronous copy ahead of the first launch.  The image pointers live in those descriptors, not in the captured
+ * graph, so any mix of sizes and pointers replays one graph.
+ * Rejected before any launch: n < 1, a NULL array or image pointer, non-positive sizes, a crop window outside its resized
+ * image, a dimension above max_side (or max_side <= 0), and whatever i2it_forward_u8 rejects. */
+int i2it_forward_u8_ragged(i2it_handle* h, const void* const* x_u8, int in_mode, const i2it_resize_desc* g, int max_side,
+                           const void* text_emb, int text_batch, const void* eps, const void* noise_map, float r,
+                           void* const* out_u8, void* out_latent, int n, int H, int W, int direction, void* stream);
+
 /* Number of kernel launches one forward of this shape issues (for bench accounting): the plan the last forward used if it
  * has this shape, else the plan with the text embedding passed inline. */
 int i2it_launch_count(i2it_handle* h, int batch, int H, int W, int direction, int* launches);
@@ -220,6 +239,14 @@ long long i2it_debug_fast_div(long long max_dividend, int d, int x);
  * the taps).  Either pointer may be NULL; coeffs must hold `cap` ints.  Returns ksize, or -1 for bad sizes or a short buffer.
  * No GPU needed. */
 int i2it_debug_resample_coeffs(int in_size, int out_size, int* bounds, int* coeffs, int cap);
+
+/* Host-side sizing of a ragged forward (i2it_forward_u8_ragged) on n geometries: *used = coefficient-table ints the call
+ * uploads, *bound = the ints its plan reserves for any call with this n, H, W and max_side.  Returns -1 for a geometry the
+ * forward would reject.  No GPU needed. */
+int i2it_debug_ragged_tables(const i2it_resize_desc* g, int n, int H, int W, int max_side, long long* used, long long* bound);
+
+/* CUDA graphs the handle has captured since create (a replay captures none). */
+int i2it_debug_graph_captures(i2it_handle* h, int* captures);
 
 /* Per-launch device timing of the plan the LAST forward used: runs it `reps` more times with CUDA events around
  * every launch and writes a JSON array [{"i","kind","ms","flops","bytes","shape"}...] (algorithmic flops/bytes per
@@ -300,6 +327,11 @@ int i2it_op_upsample_to(i2it_handle* h, const void* x, int N, int H, int W, int 
 /* LANCZOS resize of uint8 HWC images, bit-exact with PIL: x [B, H, W, 3] -> out [B, H2, W2, 3] (device pointers).
  * The same passes as i2it_forward_u8_resize; an unchanged size is a device copy (no launch). */
 int i2it_op_resize_u8(i2it_handle* h, const void* x, int B, int H, int W, void* out, int H2, int W2, void* stream);
+/* Ragged LANCZOS resize, bit-exact with PIL per image: x[i] [hw_in[2i], hw_in[2i+1], 3] -> out[i] [hw_out[2i],
+ * hw_out[2i+1], 3] (device pointers).  Two launches, the passes of i2it_forward_u8_ragged; every dimension must be <= max_side.
+ * Rejected before any launch: n < 1, NULL pointers, non-positive sizes, a dimension above max_side. */
+int i2it_op_resize_u8_ragged(i2it_handle* h, const void* const* x, const int* hw_in, void* const* out, const int* hw_out,
+                             int n, int max_side, void* stream);
 /* Test hook: force tapgemm's tile width, ring depth and persistent grid in the plans of the i2it_op_* calls made after it
  * (forward, encode_text and set_text plans never read it).  0 keeps the engine's choice.  bn replaces pick_bn's width (one of
  * 16, 32, 48, 64, 80, 96, 112, 128, 160, 192, 224, 256, at most round_up(N, 16)); launches that fix their width themselves
