@@ -550,7 +550,7 @@ int i2it_op_resize_u8(i2it_handle* h, const void* x, int B, int H, int W, void* 
     U8View s, d;
     s.slot = &P.io.x_u8; s.img = 3ll * H * W; s.w = W;
     d.slot = &P.io.out_u8; d.img = 3ll * H2 * W2; d.w = W2;
-    E.resample_u8(P, s, B, H, W, H2, W2, 0, 0, H2, W2, d);
+    E.resample_fixed(P, s, B, H, W, H2, W2, 0, 0, H2, W2, d);
     run_plan(h, P, st);
   }
   API_END

@@ -1653,26 +1653,26 @@ void Engine::encode_text(const int* tokens, int batch, void* out, cudaStream_t s
   I2IT_CUDA(cudaGetLastError());
 }
 
-void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
-                     const i2it_resize_desc* g, bool shared_input) {
+bool Engine::check_forward(int B, int H, int W, int text_batch, const void* text) const {
   I2IT_CHECK(H % 8 == 0 && W % 8 == 0 && H > 0 && W > 0, "H and W must be positive multiples of 8 (as the reference CLIs crop them)");
   I2IT_CHECK(B > 0 && (text_batch == 1 || text_batch == B), "text_batch must be 1 or batch");
+  if (text) return false;
+  auto it = textkv_.find(text_batch);
+  I2IT_CHECK(it != textkv_.end() && it->second->filled,
+             "text_emb == NULL: call i2it_set_text first (and again after every i2it_finalize_weights)");
+  return true;
+}
+
+void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
+                     const i2it_resize_desc* g, bool shared_input) {
+  const bool text_cached = check_forward(B, H, W, text_batch, io_in.text);
   IO io = io_in;
   // one variation of one image is the plain batch-1 forward: same plan, same output
   const int io_mode = (io.x_u8 ? IO_U8_IN : 0) | (io.out_u8 ? IO_U8_OUT : 0) | (shared_input && B > 1 ? IO_SHARED_IN : 0);
   I2IT_CHECK((io.x || io.x_u8) && io.eps && (io.out || io.out_u8), "null input/output pointer");
-  const bool text_cached = io.text == nullptr;
-  if (text_cached) {
-    auto it = textkv_.find(text_batch);
-    I2IT_CHECK(it != textkv_.end() && it->second->filled,
-               "text_emb == NULL: call i2it_set_text first (and again after every i2it_finalize_weights)");
-  }
   if (g) {
     I2IT_CHECK(io.x_u8 && io.out_u8, "a resize geometry needs the uint8 boundary");
-    I2IT_CHECK(g->in_H > 0 && g->in_W > 0 && g->resize_H > 0 && g->resize_W > 0 && g->out_H > 0 && g->out_W > 0,
-               "resize geometry: sizes must be positive");
-    I2IT_CHECK(g->crop_y >= 0 && g->crop_x >= 0 && g->crop_y + H <= g->resize_H && g->crop_x + W <= g->resize_W,
-               "resize geometry: the H x W crop window lies outside the resized image");
+    rs_check_geometry(*g, H, W);
     // nothing to resize or crop: the plan (and its key) of the plain uint8 forward
     if (g->in_H == H && g->in_W == W && g->resize_H == H && g->resize_W == W && g->out_H == H && g->out_W == W) g = nullptr;
   }
@@ -1683,19 +1683,12 @@ void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int te
 
 void Engine::forward_ragged(const IO& io_in, const void* const* x, void* const* out, const i2it_resize_desc* g, int max_side,
                             int B, int H, int W, int direction, int text_batch, cudaStream_t st) {
-  I2IT_CHECK(H % 8 == 0 && W % 8 == 0 && H > 0 && W > 0, "H and W must be positive multiples of 8 (as the reference CLIs crop them)");
-  I2IT_CHECK(B > 0 && (text_batch == 1 || text_batch == B), "text_batch must be 1 or batch");
+  const bool text_cached = check_forward(B, H, W, text_batch, io_in.text);
   I2IT_CHECK(x && out && g, "ragged forward: null image or geometry array");
   rs_check_ragged(g, B, H, W, max_side);      // before the pointers: an empty output (a zero size) has a null one
   for (int i = 0; i < B; ++i)
     I2IT_CHECK(x[i] && out[i], "ragged forward: null image pointer (image " + std::to_string(i) + ")");
   I2IT_CHECK(io_in.eps, "null input/output pointer");
-  const bool text_cached = io_in.text == nullptr;
-  if (text_cached) {
-    auto it = textkv_.find(text_batch);
-    I2IT_CHECK(it != textkv_.end() && it->second->filled,
-               "text_emb == NULL: call i2it_set_text first (and again after every i2it_finalize_weights)");
-  }
   // the tables first: a size pair the table builder refuses fails here, before a plan is built or anything is enqueued
   for (int i = 0; i < B; ++i) {
     const int pairs[4][2] = {{g[i].in_H, g[i].resize_H}, {g[i].in_W, g[i].resize_W}, {H, g[i].out_H}, {W, g[i].out_W}};

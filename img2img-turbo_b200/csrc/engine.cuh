@@ -166,8 +166,11 @@ struct RsCall {
   std::vector<int> tab;
   double bytes[4] = {0, 0, 0, 0};
 };
-// Rejects, with a message, a ragged forward geometry: non-positive sizes, a crop window outside its resized image, a dimension
-// above max_side.  Host only.
+// Rejects, with a message ending in `at`, a resize geometry with a non-positive size or an H x W crop window outside its
+// resized image.  Host only.
+void rs_check_geometry(const i2it_resize_desc& d, int H, int W, const std::string& at = "");
+// Rejects, with a message, a ragged forward geometry: rs_check_geometry's rejections of each image, a dimension above
+// max_side.  Host only.
 void rs_check_ragged(const i2it_resize_desc* g, int n, int H, int W, int max_side);
 // The call's descriptors (input h, input v, output h, output v; n each) and tables.  x / out / rg may be null (host-only
 // sizing: the descriptors then carry null pointers).
@@ -258,6 +261,9 @@ class Engine {
   // B images of their own sizes (x[i], out[i], g[i]) through one IO_RAGGED plan of capacity max_side on an H x W network
   void forward_ragged(const IO& io, const void* const* x, void* const* out, const i2it_resize_desc* g, int max_side, int B,
                       int H, int W, int direction, int text_batch, cudaStream_t st);
+  // the checks every image forward starts with (network size, text batch, a cached text when text is null); returns
+  // whether the text is the cached one
+  bool check_forward(int B, int H, int W, int text_batch, const void* text) const;
   // cross-attention K / V^T of the prompt, computed once per prompt (i2it_set_text) instead of once per forward
   void set_text(const void* text, int text_batch, cudaStream_t st);
   // CLIP text tower (SURVEY 8f #1): tokens [batch, 77] int32 -> last_hidden_state [batch, 77, hidden] in the handle dtype
@@ -288,9 +294,14 @@ class Engine {
   Act upsample_to(Plan& P, const Act& x, int Ho, int Wo);          // F.interpolate(size=(Ho,Wo), mode="nearest")
   Act pad_even(Plan& P, const Act& x);                               // zero-padded copy with even H and W
   // PIL LANCZOS resize of src [B, inH, inW, 3] to rsH x rsW, window [y0, y0+H) x [x0, x0+W) written densely to dst
-  // [B, H, W, 3]: the horizontal pass if the width changes, then the vertical pass if the height changes (at least one must)
-  void resample_u8(Plan& P, const U8View& src, int B, int inH, int inW, int rsH, int rsW, int y0, int x0, int H, int W,
-                   const U8View& dst);
+  // [B, H, W, 3]: the horizontal pass if the width changes, then the vertical pass if the height changes (at least one must).
+  // Descriptors and tables are uploaded here, once.
+  void resample_fixed(Plan& P, const U8View& src, int B, int inH, int inW, int rsH, int rsW, int y0, int x0, int H, int W,
+                      const U8View& dst);
+  // one resize launch of `grid` blocks over descriptors d[0, n); a caller's view (slot) is the base its side's descriptor
+  // addresses are relative to, read at launch; a plan buffer's or an empty view's base is 0
+  void resample_pass(Plan& P, bool vertical, const RsPass* d, int n, const int* tab, const U8View& src, const U8View& dst,
+                     int grid, const char* kind, double bytes, const std::string& shape);
   // the ragged resize launches (horizontal, vertical) over descriptors [first, first + B) and [first + B, first + 2B) of P.rg;
   // ops slot: where their plan indices go in P.rg.ops
   void resample_ragged(Plan& P, int B, int first, int slot);

@@ -442,64 +442,47 @@ Act Engine::build_unet(Plan& P, const Act& z, int text_batch, bool text_cached) 
 }
 
 // ------------------------------------------------------------------------------------------ whole path
-void Engine::resample_u8(Plan& P, const U8View& src, int B, int inH, int inW, int rsH, int rsW, int y0, int x0, int H, int W,
-                         const U8View& dst) {
+void Engine::resample_fixed(Plan& P, const U8View& src, int B, int inH, int inW, int rsH, int rsW, int y0, int x0, int H, int W,
+                            const U8View& dst) {
   const bool need_h = inW != rsW, need_v = inH != rsH;
-  I2IT_CHECK(need_h || need_v, "resample_u8: the size does not change");
-  I2IT_CHECK(y0 >= 0 && x0 >= 0 && y0 + H <= rsH && x0 + W <= rsW, "resample_u8: window outside the resized image");
-  // [bounds | coefficients] on the device, written once here: a fresh block, never recycled by later ops of the plan
-  auto upload = [&P](const ResampleTable& t) {
-    int* d = static_cast<int*>(P.pool.get_fresh((t.bounds.size() + t.coeffs.size()) * sizeof(int)));
-    I2IT_CUDA(cudaMemcpy(d, t.bounds.data(), t.bounds.size() * sizeof(int), cudaMemcpyHostToDevice));
-    I2IT_CUDA(cudaMemcpy(d + t.bounds.size(), t.coeffs.data(), t.coeffs.size() * sizeof(int), cudaMemcpyHostToDevice));
-    return d;
-  };
+  I2IT_CHECK(need_h || need_v, "resample_fixed: the size does not change");
+  I2IT_CHECK(y0 >= 0 && x0 >= 0 && y0 + H <= rsH && x0 + W <= rsW, "resample_fixed: window outside the resized image");
+  // a caller's images are offsets from the pointer each launch reads (one graph per IO set); a plan buffer's are addresses
+  auto addr = [](const U8View& v) { return v.slot ? 0 : reinterpret_cast<uintptr_t>(v.get()); };
+  RsImage m{addr(src), addr(dst), 0, inH, inW, rsH, rsW, y0, x0, H, W};
+  if (need_h && need_v) {
+    const std::pair<int, int> rr = rs_rows(m, rs_tables_);
+    auto mid = alloc_raw(P, static_cast<size_t>(B) * (rr.second - rr.first) * W * 3);
+    P.keep.push_back(mid);
+    m.mid = reinterpret_cast<uintptr_t>(mid.get());
+  }
+  std::vector<RsPass> d, v;
+  std::vector<int> tab;
+  double bytes[2] = {0, 0};
+  rs_add_images(m, B, src.img, dst.img, /*skip_identity=*/true, rs_tables_, d, v, tab, bytes);
+  const size_t nh = d.size();
+  d.insert(d.end(), v.begin(), v.end());
+  // [descriptors | tables] on the device, written once here: a fresh block, never recycled by later ops of the plan
+  const size_t dbytes = d.size() * sizeof(RsPass);
+  char* dev = static_cast<char*>(P.pool.get_fresh(dbytes + tab.size() * sizeof(int)));
+  I2IT_CUDA(cudaMemcpy(dev, d.data(), dbytes, cudaMemcpyHostToDevice));
+  I2IT_CUDA(cudaMemcpy(dev + dbytes, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice));
+  const RsPass* dd = reinterpret_cast<const RsPass*>(dev);
+  const int* dtab = reinterpret_cast<const int*>(dev + dbytes);
   const std::string geo = std::to_string(B) + "x" + std::to_string(inH) + "x" + std::to_string(inW) + "->" + std::to_string(rsH) +
                           "x" + std::to_string(rsW) + "@" + std::to_string(y0) + "," + std::to_string(x0) + ":" +
                           std::to_string(H) + "x" + std::to_string(W);
-  // source rows the vertical pass reads (the window's rows when only the width changes); the horizontal pass makes only these
-  ResampleTable tv;
-  int r0 = y0, r1 = y0 + H;
-  if (need_v) {
-    tv = lanczos_table(inH, rsH);
-    r0 = tv.bounds[2 * static_cast<size_t>(y0)];
-    r1 = tv.bounds[2 * static_cast<size_t>(y0 + H - 1)] + tv.bounds[2 * static_cast<size_t>(y0 + H - 1) + 1];
-  }
-  U8View vsrc = src;
-  int col0 = x0, shift = 0;
-  if (need_h) {
-    const ResampleTable th = lanczos_table(inW, rsW);
-    const int* tab = upload(th);
-    const int rows = r1 - r0, ks = th.ksize;
-    U8View hd = dst;
-    if (need_v) {
-      auto buf = alloc_raw(P, static_cast<size_t>(B) * rows * W * 3);
-      P.keep.push_back(buf);
-      hd = U8View();
-      hd.p = static_cast<uint8_t*>(buf.get()); hd.img = static_cast<long long>(rows) * W * 3; hd.w = W;
-    }
-    const long long total = static_cast<long long>(B) * rows * W;
-    const int span = th.bounds[2 * static_cast<size_t>(x0 + W - 1)] + th.bounds[2 * static_cast<size_t>(x0 + W - 1) + 1] -
-                     th.bounds[2 * static_cast<size_t>(x0)];
-    const double bytes = 3.0 * B * rows * (span + W) + 4.0 * W * (2 + ks);
-    const int* coef = tab + 2 * static_cast<size_t>(rsW);
-    add_op(P, [=](cudaStream_t st) {
-      launch_k(resample_h_u8_kernel, dim3(ceil_div_i(total, 256)), dim3(256), 0, st, 0, src.get(), src.img, src.w, r0,
-               hd.get(), rows, W, x0, tab, coef, ks, total);
-    }, "resample_h", 0, bytes, geo);
-    vsrc = hd; col0 = 0; shift = r0;
-  }
-  if (need_v) {
-    const int* tab = upload(tv);
-    const int* coef = tab + 2 * static_cast<size_t>(rsH);
-    const int ks = tv.ksize;
-    const long long total = static_cast<long long>(B) * H * W;
-    const double bytes = 3.0 * B * W * ((r1 - r0) + H) + 4.0 * H * (2 + ks);
-    add_op(P, [=](cudaStream_t st) {
-      launch_k(resample_v_u8_kernel, dim3(ceil_div_i(total, 256)), dim3(256), 0, st, 0, vsrc.get(), vsrc.img, vsrc.w, col0,
-               shift, dst.get(), H, W, y0, tab, coef, ks, total);
-    }, "resample_v", 0, bytes, geo);
-  }
+  // one block per output row: the rows are known here, and no block strides or exits early
+  if (need_h) resample_pass(P, false, dd, B, dtab, src, need_v ? U8View() : dst, B * d[0].rows, "resample_h", bytes[0], geo);
+  if (need_v) resample_pass(P, true, dd + nh, B, dtab, need_h ? U8View() : src, dst, B * H, "resample_v", bytes[1], geo);
+}
+
+void Engine::resample_pass(Plan& P, bool vertical, const RsPass* d, int n, const int* tab, const U8View& src, const U8View& dst,
+                           int grid, const char* kind, double bytes, const std::string& shape) {
+  add_op(P, [=](cudaStream_t st) {
+    auto base = [](const U8View& v) { return v.slot ? reinterpret_cast<uintptr_t>(v.get()) : uintptr_t(0); };
+    launch_k(vertical ? resample_v_kernel : resample_h_kernel, dim3(grid), dim3(256), 0, st, 0, d, n, tab, base(src), base(dst));
+  }, kind, 0, bytes, shape);
 }
 
 void Engine::resample_ragged(Plan& P, int B, int first, int slot) {
@@ -509,13 +492,9 @@ void Engine::resample_ragged(Plan& P, int B, int first, int slot) {
   const int grid = num_sms * 8;
   const std::string shape = std::to_string(B) + " images, max_side " + std::to_string(P.rg.max_side);
   P.rg.ops[slot] = P.ops.size();
-  add_op(P, [=](cudaStream_t st) {
-    launch_k(resample_h_ragged_kernel, dim3(grid), dim3(256), 0, st, 0, d, B, tab);
-  }, "resample_h_ragged", 0, 0, shape);
+  resample_pass(P, false, d, B, tab, U8View(), U8View(), grid, "resample_h_ragged", 0, shape);
   P.rg.ops[slot + 1] = P.ops.size();
-  add_op(P, [=](cudaStream_t st) {
-    launch_k(resample_v_ragged_kernel, dim3(grid), dim3(256), 0, st, 0, d + B, B, tab);
-  }, "resample_v_ragged", 0, 0, shape);
+  resample_pass(P, true, d + B, B, tab, U8View(), U8View(), grid, "resample_v_ragged", 0, shape);
 }
 
 void Engine::resize_ragged_op(Plan& P, const void* const* x, const int* hw_in, void* const* out, const int* hw_out, int n,
@@ -533,7 +512,7 @@ void Engine::resize_ragged_op(Plan& P, const void* const* x, const int* hw_in, v
     I2IT_CHECK(H <= max_side && W <= max_side && H2 <= max_side && W2 <= max_side,
                "i2it_op_resize_u8_ragged: a dimension exceeds max_side (" + std::to_string(max_side) + ")" + at);
     I2IT_CHECK(x[i] && out[i], "i2it_op_resize_u8_ragged: null image pointer" + at);
-    im[i] = RsImage{static_cast<const uint8_t*>(x[i]), static_cast<uint8_t*>(out[i]), nullptr, H, W, H2, W2, 0, 0, H2, W2};
+    im[i] = RsImage{reinterpret_cast<uintptr_t>(x[i]), reinterpret_cast<uintptr_t>(out[i]), 0, H, W, H2, W2, 0, 0, H2, W2};
     const std::pair<int, int> rr = rs_rows(im[i], rs_tables_);
     mid_off[i] = mid_bytes;
     mid_bytes += static_cast<size_t>(rr.second - rr.first) * W2 * 3;
@@ -543,8 +522,8 @@ void Engine::resize_ragged_op(Plan& P, const void* const* x, const int* hw_in, v
   RsCall c;
   std::vector<RsPass> v;
   for (int i = 0; i < n; ++i) {
-    im[i].mid = static_cast<uint8_t*>(mid.get()) + mid_off[i];
-    rs_add_image(im[i], rs_tables_, c.d, v, c.tab, c.bytes);
+    im[i].mid = reinterpret_cast<uintptr_t>(mid.get()) + mid_off[i];
+    rs_add_images(im[i], 1, 0, 0, /*skip_identity=*/false, rs_tables_, c.d, v, c.tab, c.bytes);
   }
   c.d.insert(c.d.end(), v.begin(), v.end());
   const size_t dbytes = c.d.size() * sizeof(RsPass);
@@ -559,23 +538,27 @@ void Engine::resize_ragged_op(Plan& P, const void* const* x, const int* hw_in, v
   P.meta[P.rg.ops[1]].bytes = c.bytes[1];
 }
 
+void rs_check_geometry(const i2it_resize_desc& d, int H, int W, const std::string& at) {
+  I2IT_CHECK(d.in_H > 0 && d.in_W > 0 && d.resize_H > 0 && d.resize_W > 0 && d.out_H > 0 && d.out_W > 0,
+             "resize geometry: sizes must be positive" + at);
+  I2IT_CHECK(d.crop_y >= 0 && d.crop_x >= 0 && d.crop_y + H <= d.resize_H && d.crop_x + W <= d.resize_W,
+             "resize geometry: the H x W crop window lies outside the resized image" + at);
+}
+
 void rs_check_ragged(const i2it_resize_desc* g, int n, int H, int W, int max_side) {
   I2IT_CHECK(max_side > 0, "ragged forward: max_side must be positive");
   I2IT_CHECK(g != nullptr && n > 0, "ragged forward: no geometry");
   for (int i = 0; i < n; ++i) {
     const i2it_resize_desc& d = g[i];
     const std::string at = " (image " + std::to_string(i) + ")";
-    I2IT_CHECK(d.in_H > 0 && d.in_W > 0 && d.resize_H > 0 && d.resize_W > 0 && d.out_H > 0 && d.out_W > 0,
-               "resize geometry: sizes must be positive" + at);
-    I2IT_CHECK(d.crop_y >= 0 && d.crop_x >= 0 && d.crop_y + H <= d.resize_H && d.crop_x + W <= d.resize_W,
-               "resize geometry: the H x W crop window lies outside the resized image" + at);
+    rs_check_geometry(d, H, W, at);
     I2IT_CHECK(d.in_H <= max_side && d.in_W <= max_side && d.resize_H <= max_side && d.resize_W <= max_side &&
                d.out_H <= max_side && d.out_W <= max_side,
                "resize geometry: a dimension exceeds max_side (" + std::to_string(max_side) + ")" + at);
   }
 }
 
-static uint8_t* rs_at(uint8_t* p, long long off) { return p ? p + off : nullptr; }
+static uintptr_t rs_at(const void* p, long long off = 0) { return p ? reinterpret_cast<uintptr_t>(p) + off : 0; }
 
 RsCall rs_forward_call(const i2it_resize_desc* g, int n, int H, int W, int max_side, RsTableCache& cache, const void* const* x,
                        void* const* out, const RaggedBufs* rg) {
@@ -584,13 +567,12 @@ RsCall rs_forward_call(const i2it_resize_desc* g, int n, int H, int W, int max_s
   const long long net = 3ll * H * W;
   for (int i = 0; i < n; ++i) {
     const i2it_resize_desc& e = g[i];
-    const RsImage in{x ? static_cast<const uint8_t*>(x[i]) : nullptr, rg ? rs_at(rg->in_net, i * net) : nullptr,
-                     rg ? rs_at(rg->in_mid, i * 3ll * max_side * W) : nullptr, e.in_H, e.in_W, e.resize_H, e.resize_W,
-                     e.crop_y, e.crop_x, H, W};
-    const RsImage o{rg ? rs_at(rg->out_net, i * net) : nullptr, out ? static_cast<uint8_t*>(out[i]) : nullptr,
-                    rg ? rs_at(rg->out_mid, i * 3ll * H * max_side) : nullptr, H, W, e.out_H, e.out_W, 0, 0, e.out_H, e.out_W};
-    rs_add_image(in, cache, d[0], d[1], c.tab, c.bytes);
-    rs_add_image(o, cache, d[2], d[3], c.tab, c.bytes + 2);
+    const RsImage in{x ? rs_at(x[i]) : 0, rg ? rs_at(rg->in_net, i * net) : 0, rg ? rs_at(rg->in_mid, i * 3ll * max_side * W) : 0,
+                     e.in_H, e.in_W, e.resize_H, e.resize_W, e.crop_y, e.crop_x, H, W};
+    const RsImage o{rg ? rs_at(rg->out_net, i * net) : 0, out ? rs_at(out[i]) : 0, rg ? rs_at(rg->out_mid, i * 3ll * H * max_side) : 0,
+                    H, W, e.out_H, e.out_W, 0, 0, e.out_H, e.out_W};
+    rs_add_images(in, 1, 0, 0, /*skip_identity=*/false, cache, d[0], d[1], c.tab, c.bytes);
+    rs_add_images(o, 1, 0, 0, /*skip_identity=*/false, cache, d[2], d[3], c.tab, c.bytes + 2);
   }
   for (auto& v : d) c.d.insert(c.d.end(), v.begin(), v.end());
   I2IT_CHECK(static_cast<long long>(c.tab.size()) <= rs_forward_bound(n, H, W, max_side),
@@ -658,7 +640,7 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
       U8View d;
       d.p = static_cast<uint8_t*>(buf.get()); d.img = 3ll * H * W; d.w = W;
       P.ranges.emplace_back(P.ops.size(), "resize_in");
-      resample_u8(P, net_in, B_in, g->in_H, g->in_W, g->resize_H, g->resize_W, g->crop_y, g->crop_x, H, W, d);
+      resample_fixed(P, net_in, B_in, g->in_H, g->in_W, g->resize_H, g->resize_W, g->crop_y, g->crop_x, H, W, d);
       net_in = d;
     }
   }
@@ -721,7 +703,7 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
     } else if (resize_out) {
       out.img = 3ll * g->out_H * g->out_W; out.w = g->out_W;
       P.ranges.emplace_back(P.ops.size(), "resize_out");
-      resample_u8(P, net_out, B, H, W, g->out_H, g->out_W, 0, 0, g->out_H, g->out_W, out);
+      resample_fixed(P, net_out, B, H, W, g->out_H, g->out_W, 0, 0, g->out_H, g->out_W, out);
     }
   }
   flush_prep();                             // every weight of the plan: one fold/re-layout launch (+ the time-embedding GEMVs)

@@ -93,55 +93,21 @@ __device__ __forceinline__ void rs_taps(const uint8_t* __restrict__ s, long long
   d[0] = rs_clip8(a0); d[1] = rs_clip8(a1); d[2] = rs_clip8(a2);
 }
 
-// Horizontal pass: dst [B, rows, Wo, 3] = src rows row0 .. row0+rows-1 resampled along x, output columns x0 .. x0+Wo-1 of
-// the table (a crop window).  src: [B][img / (src_w*3)][src_w][3], img bytes per image.  One thread per output pixel.
-static __global__ void resample_h_u8_kernel(const uint8_t* __restrict__ src, long long src_img, int src_w, int row0,
-                                            uint8_t* __restrict__ dst, int rows, int Wo, int x0, const int* __restrict__ bounds,
-                                            const int* __restrict__ coeffs, int ksize, long long total) {
-  pdl_sync();
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;   // over B*rows*Wo
-  if (i >= total) return;
-  const int j = static_cast<int>(i % Wo);
-  const long long br = i / Wo;
-  const int r = static_cast<int>(br % rows);
-  const long long b = br / rows;
-  const int xo = x0 + j, xmin = bounds[2 * xo], n = bounds[2 * xo + 1];
-  const uint8_t* s = src + b * src_img + (static_cast<long long>(row0 + r) * src_w + xmin) * 3;
-  rs_taps(s, 3, coeffs + static_cast<long long>(xo) * ksize, n, dst + i * 3);
-}
-
-// Vertical pass: dst [B, Ho, Wo, 3] = output rows y0 .. y0+Ho-1 of the table, read from src columns col0 .. col0+Wo-1;
-// src row index = table row index - row_shift (the horizontal pass computed only the rows from row_shift on).
-static __global__ void resample_v_u8_kernel(const uint8_t* __restrict__ src, long long src_img, int src_w, int col0,
-                                            int row_shift, uint8_t* __restrict__ dst, int Ho, int Wo, int y0,
-                                            const int* __restrict__ bounds, const int* __restrict__ coeffs, int ksize,
-                                            long long total) {
-  pdl_sync();
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;   // over B*Ho*Wo
-  if (i >= total) return;
-  const int j = static_cast<int>(i % Wo);
-  const long long bh = i / Wo;
-  const int h = static_cast<int>(bh % Ho);
-  const long long b = bh / Ho;
-  const int yo = y0 + h, ymin = bounds[2 * yo] - row_shift, n = bounds[2 * yo + 1];
-  const long long pitch = static_cast<long long>(src_w) * 3;
-  const uint8_t* s = src + b * src_img + static_cast<long long>(ymin) * pitch + static_cast<long long>(col0 + j) * 3;
-  rs_taps(s, pitch, coeffs + static_cast<long long>(yo) * ksize, n, dst + i * 3);
-}
-
-// ------------------------------------------------------------------------------------------ ragged passes
-// Every image of a batch with its own sizes, through one horizontal and one vertical launch.  Each image has a descriptor per
-// pass in device memory, written by the host for every call; the grid is fixed by the plan, and its blocks stride over the
-// call's output rows (image by image: item0 counts the rows of the images before), so one captured graph serves any mix.
+// ------------------------------------------------------------------------------------------ the passes
+// A launch runs one pass over a list of images, each with its own descriptor in device memory.  Its blocks stride over the
+// launch's output rows (image by image: item0 counts the rows of the images before), so the grid need not depend on the
+// images and a ragged plan's one captured graph serves any mix of sizes.
 //
-// One image of one ragged pass: `rows` output rows of `cols` pixels.  Its table, at `tab` ints into the table area, holds
-// the window's outputs only: bounds [outputs][2] (first source index, taps) then coefficients [outputs][ksize].
+// One image of one pass: `rows` output rows of `cols` pixels.  Its table, at `tab` ints into the table area, holds the
+// window's outputs only: bounds [outputs][2] (first source index, taps) then coefficients [outputs][ksize].
 //   horizontal: output row r is source row row0 + r; output column j takes table row j
 //   vertical:   output row r takes table row r and reads source rows from bounds[r].first - row0 (the horizontal pass made
 //               only the rows from row0 on); output column j is source column j
+// src and dst are relative to the launch's src_base / dst_base.  A ragged launch passes 0: its descriptors, uploaded with
+// every call, hold the images' addresses.  A fixed plan passes the caller's pointer, read at launch: its descriptors,
+// uploaded once, hold each image's offset from it.
 struct RsPass {
-  const uint8_t* src;
-  uint8_t* dst;
+  uintptr_t src, dst;
   long long src_pitch, dst_pitch;   // bytes per row
   long long tab;
   long long item0;
@@ -158,7 +124,8 @@ __device__ __forceinline__ int rs_image_of(const RsPass* __restrict__ d, int n, 
   return lo;
 }
 
-static __global__ void resample_h_ragged_kernel(const RsPass* __restrict__ d, int n, const int* __restrict__ tab) {
+static __global__ void resample_h_kernel(const RsPass* __restrict__ d, int n, const int* __restrict__ tab, uintptr_t src_base,
+                                         uintptr_t dst_base) {
   pdl_sync();
   const long long total = d[n - 1].item0 + d[n - 1].rows;
   for (long long it = blockIdx.x; it < total; it += gridDim.x) {
@@ -166,14 +133,15 @@ static __global__ void resample_h_ragged_kernel(const RsPass* __restrict__ d, in
     const long long r = it - p.item0;
     const int* bounds = tab + p.tab;
     const int* coeffs = bounds + 2ll * p.cols;
-    const uint8_t* s = p.src + (p.row0 + r) * p.src_pitch;
-    uint8_t* o = p.dst + r * p.dst_pitch;
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(src_base + p.src) + (p.row0 + r) * p.src_pitch;
+    uint8_t* o = reinterpret_cast<uint8_t*>(dst_base + p.dst) + r * p.dst_pitch;
     for (int j = threadIdx.x; j < p.cols; j += blockDim.x)
       rs_taps(s + 3ll * bounds[2 * j], 3, coeffs + static_cast<long long>(j) * p.ksize, bounds[2 * j + 1], o + 3ll * j);
   }
 }
 
-static __global__ void resample_v_ragged_kernel(const RsPass* __restrict__ d, int n, const int* __restrict__ tab) {
+static __global__ void resample_v_kernel(const RsPass* __restrict__ d, int n, const int* __restrict__ tab, uintptr_t src_base,
+                                         uintptr_t dst_base) {
   pdl_sync();
   const long long total = d[n - 1].item0 + d[n - 1].rows;
   for (long long it = blockIdx.x; it < total; it += gridDim.x) {
@@ -182,13 +150,13 @@ static __global__ void resample_v_ragged_kernel(const RsPass* __restrict__ d, in
     const int* bounds = tab + p.tab;
     const int* k = bounds + 2ll * p.rows + static_cast<long long>(r) * p.ksize;
     const int taps = bounds[2 * r + 1];
-    const uint8_t* s = p.src + static_cast<long long>(bounds[2 * r] - p.row0) * p.src_pitch;
-    uint8_t* o = p.dst + r * p.dst_pitch;
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(src_base + p.src) + static_cast<long long>(bounds[2 * r] - p.row0) * p.src_pitch;
+    uint8_t* o = reinterpret_cast<uint8_t*>(dst_base + p.dst) + r * p.dst_pitch;
     for (int j = threadIdx.x; j < p.cols; j += blockDim.x) rs_taps(s + 3ll * j, p.src_pitch, k, taps, o + 3ll * j);
   }
 }
 
-// ---- host side of the ragged passes ----
+// ---- host side ----
 // lanczos_table per (in, out) pair, kept across calls: building one calls sin for every tap
 class RsTableCache {
  public:
@@ -216,12 +184,10 @@ inline long long rs_forward_bound(long long B, long long H, long long W, long lo
   return B * (rs_pass_bound(max_side, W) + rs_pass_bound(max_side, H) + rs_pass_bound(W, max_side) + rs_pass_bound(H, max_side));
 }
 
-// One image of a ragged resize: src [inH, inW, 3] resized to rsH x rsW, window (y0, x0, H, W) written densely to
-// dst [H, W, 3]; mid holds its horizontal pass's rows [rows, W, 3].
+// One image of a resize: src [inH, inW, 3] resized to rsH x rsW, window (y0, x0, H, W) written densely to dst [H, W, 3];
+// mid holds its horizontal pass's rows [rows, W, 3].  Addresses, or offsets from a launch's base (RsPass).
 struct RsImage {
-  const uint8_t* src;
-  uint8_t* dst;
-  uint8_t* mid;
+  uintptr_t src, dst, mid;
   int inH, inW, rsH, rsW, y0, x0, H, W;
 };
 
@@ -252,26 +218,47 @@ inline long long rs_put_table(std::vector<int>& tab, RsTableCache& cache, int in
   return off;
 }
 
-// Appends image m's horizontal pass to h, its vertical pass to v and their tables to tab; bytes[0] / bytes[1] accumulate the
-// passes' algorithmic bytes (pixels read and written, tables read).
-inline void rs_add_image(const RsImage& m, RsTableCache& cache, std::vector<RsPass>& h, std::vector<RsPass>& v,
-                         std::vector<int>& tab, double bytes[2]) {
+// Appends the passes of n images of geometry m to h and v, and their tables, once, to tab.  Image b reads m.src + b src_img,
+// writes m.dst + b dst_img and keeps its horizontal pass's rows at m.mid + b times their bytes.  bytes[0] / bytes[1] accumulate
+// the passes' algorithmic bytes (pixels read and written, tables read once).  A ragged launch runs both passes for every
+// image, an unchanged dimension as the identity.  With skip_identity a pass whose dimension does not change is left out, as
+// PIL leaves it out: the other pass then reads the source (at column x0) or writes the destination itself.
+inline void rs_add_images(const RsImage& m, int n, long long src_img, long long dst_img, bool skip_identity, RsTableCache& cache,
+                          std::vector<RsPass>& h, std::vector<RsPass>& v, std::vector<int>& tab, double bytes[2]) {
   const std::pair<int, int> rr = rs_rows(m, cache);
+  const bool need_h = !skip_identity || m.inW != m.rsW, need_v = !skip_identity || m.inH != m.rsH;
+  const int rows = rr.second - rr.first;
+  const long long mid_img = 3ll * rows * m.W;
   RsPass ph{}, pv{};
-  pv.tab = rs_put_table(tab, cache, m.inH, m.rsH, m.y0, m.H, &pv.ksize);
-  ph.tab = rs_put_table(tab, cache, m.inW, m.rsW, m.x0, m.W, &ph.ksize);
-  const int* hb = tab.data() + ph.tab;
-  const long long span = hb[2 * (m.W - 1)] + hb[2 * (m.W - 1) + 1] - hb[0];
-  ph.src = m.src; ph.src_pitch = 3ll * m.inW; ph.row0 = rr.first; ph.rows = rr.second - rr.first; ph.cols = m.W;
-  ph.dst = m.mid; ph.dst_pitch = 3ll * m.W;
-  ph.item0 = h.empty() ? 0 : h.back().item0 + h.back().rows;
-  pv.src = m.mid; pv.src_pitch = 3ll * m.W; pv.row0 = rr.first; pv.rows = m.H; pv.cols = m.W;
-  pv.dst = m.dst; pv.dst_pitch = 3ll * m.W;
-  pv.item0 = v.empty() ? 0 : v.back().item0 + v.back().rows;
-  h.push_back(ph);
-  v.push_back(pv);
-  bytes[0] += 3.0 * ph.rows * (span + m.W) + 4.0 * m.W * (2 + ph.ksize);
-  bytes[1] += 3.0 * m.W * (ph.rows + m.H) + 4.0 * m.H * (2 + pv.ksize);
+  if (need_v) pv.tab = rs_put_table(tab, cache, m.inH, m.rsH, m.y0, m.H, &pv.ksize);
+  if (need_h) {
+    ph.tab = rs_put_table(tab, cache, m.inW, m.rsW, m.x0, m.W, &ph.ksize);
+    const int* hb = tab.data() + ph.tab;
+    const long long span = hb[2 * (m.W - 1)] + hb[2 * (m.W - 1) + 1] - hb[0];
+    ph.src = m.src; ph.src_pitch = 3ll * m.inW; ph.row0 = rr.first; ph.rows = rows; ph.cols = m.W;
+    ph.dst = need_v ? m.mid : m.dst; ph.dst_pitch = 3ll * m.W;
+    bytes[0] += 3.0 * n * rows * (span + m.W) + 4.0 * m.W * (2 + ph.ksize);
+  }
+  if (need_v) {
+    pv.src = need_h ? m.mid : m.src + 3ll * m.x0; pv.src_pitch = need_h ? 3ll * m.W : 3ll * m.inW;
+    pv.row0 = need_h ? rr.first : 0; pv.rows = m.H; pv.cols = m.W;
+    pv.dst = m.dst; pv.dst_pitch = 3ll * m.W;
+    bytes[1] += 3.0 * n * m.W * (rows + m.H) + 4.0 * m.H * (2 + pv.ksize);
+  }
+  for (long long b = 0; b < n; ++b) {
+    if (need_h) {
+      RsPass p = ph;
+      p.src += b * src_img; p.dst += b * (need_v ? mid_img : dst_img);
+      p.item0 = h.empty() ? 0 : h.back().item0 + h.back().rows;
+      h.push_back(p);
+    }
+    if (need_v) {
+      RsPass p = pv;
+      p.src += b * (need_h ? mid_img : src_img); p.dst += b * dst_img;
+      p.item0 = v.empty() ? 0 : v.back().item0 + v.back().rows;
+      v.push_back(p);
+    }
+  }
 }
 
 }  // namespace i2it

@@ -191,3 +191,29 @@ def test_wrapper_resize_at_sd_turbo_width():
     ref = _pil(m.forward_u8(_pil(img, rs), eps=eps), (720, 1280))
     assert got.shape == (2, 720, 1280, 3)
     assert int((got.cpu() != ref).sum()) == 0
+
+
+@pytest.mark.parametrize("graph", [True, False])
+@pytest.mark.parametrize("size", [(90, 160), (64, 100), (75, 64)], ids=["both-passes", "width-only", "height-only"])
+def test_fixed_geometry_on_many_tensors(size, graph, tiny_sd_cyc):
+    """A fixed plan's descriptors hold offsets from the caller's pointers, read at every launch: one geometry (resized to the
+    64x64 network and back) alternates over more input / output pairs than the plan keeps graphs for, and every output equals
+    the host pipeline (a pointer kept from an earlier call, or a stale graph, writes the wrong tensor)."""
+    import i2it
+    import weights as W
+    from test_gpu_plans import _engine as _plans_engine
+    e = _plans_engine("cyclegan", torch.float16, tiny_sd_cyc, W.TINY, use_cuda_graph=graph)
+    g = torch.Generator().manual_seed(12)
+    text = torch.randn(1, 77, W.TINY["cross_dim"], generator=g).half().cuda()
+    eps = torch.randn(2, 4, 8, 8, generator=g).half().cuda()
+    imgs = [_stripes(2, *size, seed=20 + i) for i in range(10)]
+    refs = [_host_pipeline(e, x, i2it.IN_NORMALIZE, text, eps, (64, 64), None, size) for x in imgs]
+    xs = [x.cuda() for x in imgs]
+    outs = [torch.empty(2, *size, 3, dtype=torch.uint8, device="cuda") for _ in imgs]
+    for rnd in range(2):
+        for i, (x, o) in enumerate(zip(xs, outs)):
+            o.zero_()
+            e.forward_u8(x, i2it.IN_NORMALIZE, text, eps, out=o, resize=(64, 64), out_size=size)
+            assert torch.equal(o.cpu(), refs[i]), (rnd, i)
+        for i, o in enumerate(outs):
+            assert torch.equal(o.cpu(), refs[i]), (rnd, i)
