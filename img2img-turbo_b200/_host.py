@@ -143,6 +143,40 @@ def paired_geometry(H: int, W: int):
 # ------------------------------------------------------------------------------------------------
 # light-weight stand-ins for the diffusers module objects the reference exposes as .unet / .vae
 # ------------------------------------------------------------------------------------------------
+def weight_record(sd: Dict[str, torch.Tensor]) -> Dict[str, tuple]:
+    """What weight_update compares against: key -> (the tensor registered on the engine, its version counter then)."""
+    return {k: (v, v._version) for k, v in sd.items()}
+
+
+def _shares_storage(a: torch.Tensor, b: torch.Tensor) -> bool:
+    return a.untyped_storage().data_ptr() == b.untyped_storage().data_ptr()
+
+
+def weight_update(loaded: Optional[Dict[str, tuple]], sd: Dict[str, torch.Tensor]) -> Optional[List[str]]:
+    """How a live engine that holds `loaded` (weight_record of the tensors registered on it) takes the state dict `sd`: the
+    keys whose tensors changed, to register again in place before a refold, or None when it needs a new engine (no engine
+    yet, a key added or removed, a shape changed).  A TwinConv added or removed changes the keys.
+
+    A recorded tensor may alias what the caller holds (state_dict() hands out the stored tensors, and an fp32 CPU tensor is
+    stored as is), so its values are not a record of what was registered: a tensor modified in place since (its version
+    moved) counts as changed, and so does any other tensor on its storage.  Only a different tensor on other storage is
+    compared by value with an unmodified record."""
+    if loaded is None or loaded.keys() != sd.keys():
+        return None
+    changed = []
+    for k, v in sd.items():
+        old, version = loaded[k]
+        if tuple(v.shape) != tuple(old.shape):
+            return None
+        if old._version != version:
+            changed.append(k)
+        elif v is old:
+            continue
+        elif _shares_storage(v, old) or v.dtype != old.dtype or not torch.equal(v, old):
+            changed.append(k)
+    return changed
+
+
 class NetHandle:
     """What `model.unet` / `model.vae` are here: a view of the state dict plus the handful of methods the
     reference's callers use (.eval(), .train(), .requires_grad_(), .to(), .cuda(), .state_dict(),
@@ -159,7 +193,7 @@ class NetHandle:
     def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
         for k, v in sd.items():
             self._owner._sd[self._prefix + k] = v.detach().float().cpu()
-        self._owner._invalidate()
+        self._owner._reload()
 
     def named_parameters(self):
         return iter(self.state_dict().items())
@@ -259,6 +293,26 @@ class TurboBase(torch.nn.Module):
         self._final_key = None
         self.__dict__["_text_bound"] = None
 
+    def _reload(self):
+        """Take the state dict's new tensors.  A live engine that holds the same keys and shapes registers only the tensors
+        that changed and refolds in place, keeping its plans and CUDA graphs; anything else builds a new engine."""
+        live = self._engine is not None and self._engine_key is not None
+        changed = weight_update(self.__dict__.get("_loaded"), self._sd) if live else None
+        if changed is None:
+            self._invalidate()
+            return
+        if not changed:
+            return
+        try:
+            self._engine.load_state_dict({k: self._sd[k] for k in changed})
+            self._loaded = weight_record(self._sd)
+            if self._final_key is not None:
+                self._engine.refold(*self._final_key)
+                self.__dict__["_text_bound"] = None
+        except Exception:
+            self._invalidate()
+            raise
+
     # ---- engine lifecycle -------------------------------------------------------------------------
     def _get_engine(self) -> i2it.Engine:
         key = (self.compute_dtype, _cur_dev())
@@ -270,6 +324,7 @@ class TurboBase(torch.nn.Module):
                               use_cuda_graph=self._use_graph, max_plans=self.MAX_PLANS,
                               **({"text_heads": te["heads"], "text_act": te["act"]} if te else {}))
             eng.load_state_dict(self._sd)
+            self._loaded = weight_record(self._sd)
             if te:      # the CLIP text tower runs on the engine too (SURVEY 8f #1): same tensors, transformers key names
                 eng.load_state_dict({"text_encoder." + k: v for k, v in self.text_encoder.state_dict().items()})
             self._text_on_engine = bool(te)
@@ -288,7 +343,11 @@ class TurboBase(torch.nn.Module):
         eng = self._get_engine()
         key = (float(lw_unet), float(lw_vae), float(gamma), float(twin_r))
         if self._final_key != key:
-            eng.finalize(*key)
+            prev = self._final_key
+            if prev is not None and (prev[3] < 0) == (key[3] < 0):
+                eng.refold(*key)          # the same weights in the same buffers: plans and CUDA graphs stay
+            else:
+                eng.finalize(*key)
             self._final_key = key
             self.__dict__["_text_bound"] = None
         return eng

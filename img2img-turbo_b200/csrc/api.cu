@@ -91,6 +91,12 @@ int i2it_finalize_weights(i2it_handle* h, float lw_unet, float lw_vae, float ski
   API_END
 }
 
+int i2it_refold_weights(i2it_handle* h, float lw_unet, float lw_vae, float skip_gamma, float twin_r) {
+  API_BEGIN(h)
+  E.refold(lw_unet, lw_vae, skip_gamma, twin_r);
+  API_END
+}
+
 int i2it_workspace_bytes(i2it_handle* h, int batch, int H, int W, size_t* bytes) {
   API_BEGIN(h)
   I2IT_CHECK(bytes != nullptr, "null out pointer");
@@ -326,6 +332,12 @@ int i2it_read_prepared(i2it_handle* h, const char* key, void* w, size_t w_elems,
   API_BEGIN(h)
   I2IT_CHECK(key != nullptr && dims != nullptr, "i2it_read_prepared: null argument");
   E.read_prepared(key, w, w_elems, bias, b_elems, dims);
+  API_END
+}
+
+int i2it_debug_refold_info(i2it_handle* h, char* json, size_t cap) {
+  API_BEGIN(h)
+  copy_json(E.refold_info_json(), json, cap, "i2it_debug_refold_info");
   API_END
 }
 

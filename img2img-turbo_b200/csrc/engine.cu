@@ -293,6 +293,8 @@ Engine::~Engine() {
   textenc_.clear();
   free_prepared();
   for (auto& kv : w_) cudaFree(kv.second.d);
+  for (void* p : retired_) cudaFree(p);
+  for (auto& t : job_tables_) cudaFree(t.p);
   if (err_host_) cudaFreeHost(err_host_);
   if (gstream_) cudaStreamDestroy(gstream_);
   if (ev_in_) cudaEventDestroy(ev_in_);
@@ -392,6 +394,7 @@ void Engine::free_prepared() {
   prep_allocs_.clear();
   prepared_.clear();
   prepared_f32_.clear();
+  recipes_.clear();
   emb_act_ = nullptr;
   pending_jobs_.clear();
   pending_blocks_ = 0;
@@ -403,25 +406,40 @@ void Engine::set_weight(const std::string& key_in, const void* data, const int64
   const std::string bl = ".base_layer.";
   const size_t pos = key.find(bl);
   if (pos != std::string::npos) key = key.substr(0, pos) + "." + key.substr(pos + bl.size());
-  WT t;
-  t.numel = 1;
-  for (int i = 0; i < ndim; ++i) { t.shape.push_back(shape[i]); t.numel *= shape[i]; }
-  I2IT_CHECK(t.numel > 0, "empty tensor for key " + key);
-  I2IT_CUDA(cudaMalloc(&t.d, t.numel * sizeof(float)));
-  if (dt == DT_F32) {
-    I2IT_CUDA(cudaMemcpy(t.d, data, t.numel * sizeof(float), is_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+  std::vector<int64_t> shp(shape, shape + ndim);
+  long long numel = 1;
+  for (int i = 0; i < ndim; ++i) numel *= shape[i];
+  I2IT_CHECK(numel > 0, "empty tensor for key " + key);
+  I2IT_CHECK(dt == DT_F32 || dt == DT_F16 || dt == DT_BF16, "unsupported weight dtype");
+  auto it = w_.find(key);
+  // the same shape: copy into the existing master, whose address the prepared weights' recipes and the plans (norm scales,
+  // text embeddings) hold; no forward may be reading it meanwhile
+  const bool in_place = it != w_.end() && it->second.shape == shp;
+  float* dst = nullptr;
+  if (in_place) {
+    sync_plans();
+    dst = it->second.d;
   } else {
-    I2IT_CHECK(dt == DT_F16 || dt == DT_BF16, "unsupported weight dtype");
+    I2IT_CUDA(cudaMalloc(&dst, numel * sizeof(float)));
+  }
+  if (dt == DT_F32) {
+    I2IT_CUDA(cudaMemcpy(dst, data, numel * sizeof(float), is_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+  } else {
     uint16_t* tmp = nullptr;
-    I2IT_CUDA(cudaMalloc(&tmp, t.numel * 2));
-    I2IT_CUDA(cudaMemcpy(tmp, data, t.numel * 2, is_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
-    cvt16_to_f32_kernel<<<ceil_div(t.numel, 256), 256>>>(tmp, t.d, t.numel, dt == DT_BF16);
+    I2IT_CUDA(cudaMalloc(&tmp, numel * 2));
+    I2IT_CUDA(cudaMemcpy(tmp, data, numel * 2, is_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+    cvt16_to_f32_kernel<<<ceil_div(numel, 256), 256>>>(tmp, dst, numel, dt == DT_BF16);
     I2IT_CUDA(cudaDeviceSynchronize());
     cudaFree(tmp);
   }
-  auto it = w_.find(key);
-  if (it != w_.end()) { cudaFree(it->second.d); w_.erase(it); }
-  w_.emplace(key, std::move(t));
+  if (!in_place) {
+    // resident plans may still read the old master (a norm scale): it lives until the next finalize drops them
+    if (it != w_.end()) { retired_.push_back(it->second.d); w_.erase(it); }
+    WT t;
+    t.d = dst; t.shape = shp; t.numel = numel;
+    w_.emplace(key, std::move(t));
+  }
+  dirty_w_.insert(key);
   finalized_ = false;
 }
 
@@ -433,11 +451,77 @@ const WT& Engine::raw(const std::string& name, const char* what) const {
   return it->second;
 }
 
-float Engine::adapter_weight(const std::string& name, const std::string& adapter) const {
+const WT& Engine::src(const std::string& name, const char* what) {
+  const WT& w = raw(name, what);
+  if (recording_ >= 0) recipes_[recording_].reads.push_back(name + "." + what);
+  return w;
+}
+
+const float* Engine::f32_input(const std::string& key) {
+  auto it = prepared_f32_.find(key);
+  if (it != prepared_f32_.end()) {
+    if (recording_ >= 0) recipes_[recording_].after.push_back(key);
+    return it->second;
+  }
+  auto w = w_.find(key);
+  I2IT_CHECK(w != w_.end(), "missing weight '" + key + "'");
+  if (recording_ >= 0) recipes_[recording_].reads.push_back(key);
+  return w->second.d;
+}
+
+float Engine::fold_input(FoldInput which) {
+  I2IT_CHECK(which == FOLD_GAMMA || which == FOLD_TWIN_R, "fold_input: the LoRA weights are read through adapter_weight");
+  if (recording_ >= 0) recipes_[recording_].uses |= which;
+  return which == FOLD_GAMMA ? skip_gamma_ : twin_r_;
+}
+
+float Engine::adapter_weight(const std::string& name, const std::string& adapter) {
   auto it = adapter_scale_.find(adapter);
   I2IT_CHECK(it != adapter_scale_.end(), "no scale registered for LoRA adapter '" + adapter + "' (layer " + name + ")");
   const bool is_unet = name.rfind("unet.", 0) == 0;
+  if (recording_ >= 0) recipes_[recording_].uses |= (is_unet ? FOLD_LW_UNET : FOLD_LW_VAE) | FOLD_ADAPTER_SCALE;
   return it->second * (is_unet ? lw_unet_ : lw_vae_);
+}
+
+void Engine::add_recipe(const std::string& key, std::function<void()> emit) {
+  Recipe r;
+  r.key = key;
+  r.emit = std::move(emit);
+  recipes_.push_back(std::move(r));
+  try {
+    run_recipe(recipes_.size() - 1);
+  } catch (...) {
+    recipes_.pop_back();
+    throw;
+  }
+}
+
+void Engine::run_recipe(size_t i) {
+  Recipe& r = recipes_[i];
+  // a run that throws pushes no launch: its buffers keep the last fold, and so must what the recipe says that fold read
+  const unsigned uses = r.uses;
+  std::vector<std::string> reads = std::move(r.reads), after = std::move(r.after);
+  r.uses = 0;
+  r.reads.clear();
+  r.after.clear();
+  recording_ = static_cast<long long>(i);
+  try {
+    r.emit();
+  } catch (...) {
+    recording_ = -1;
+    r.uses = uses;
+    r.reads = std::move(reads);
+    r.after = std::move(after);
+    throw;
+  }
+  recording_ = -1;
+}
+
+void Engine::snapshot_fold() {
+  fold_shapes_.clear();
+  for (const auto& kv : w_) fold_shapes_[kv.first] = kv.second.shape;
+  fold_adapter_scale_ = adapter_scale_;
+  dirty_w_.clear();
 }
 
 void Engine::finalize(float lw_unet, float lw_vae, float skip_gamma, float twin_r) {
@@ -449,15 +533,107 @@ void Engine::finalize(float lw_unet, float lw_vae, float skip_gamma, float twin_
   last_plan_ = nullptr;
   last_text_plan_ = nullptr;
   free_prepared();
+  for (void* p : retired_) cudaFree(p);
+  retired_.clear();
+  snapshot_fold();
   finalized_ = true;
+  folded_ = true;
+}
+
+// algorithmic bytes a preparation job reads and writes (each source element once)
+static double prep_job_bytes(const PrepJob& j) {
+  if (j.mode == PREP_IDENTITY) return 2.0 * j.n;
+  if (j.mode == PREP_BIAS) return 4.0 * j.cout * (1 + (j.bias != nullptr) + (j.w1 != nullptr) + (j.bias_add != nullptr));
+  const double inner = 1.0 * j.cin * j.taps;
+  double b = 4.0 * j.cout * inner * (j.w1 ? 2 : 1) + 2.0 * j.n;
+  for (int a = 0; a < j.n_adapters; ++a) b += 4.0 * j.rank[a] * (inner + j.cout);
+  return b;
+}
+
+static double gemv_job_bytes(const GemvJob& j) {
+  double b = 4.0 * (1.0 * j.out * j.in + j.in + j.out * (j.b ? 2 : 1));
+  for (int a = 0; a < j.n_adapters; ++a) b += 4.0 * j.rank[a] * (1.0 * j.in + j.out);
+  return b;
+}
+
+void Engine::refold(float lw_unet, float lw_vae, float skip_gamma, float twin_r) {
+  sync_plans();
+  I2IT_CHECK(folded_, "i2it_refold_weights: the weights were never folded; call i2it_finalize_weights first");
+  I2IT_CHECK((twin_r < 0.f) == (twin_r_ < 0.f),
+             std::string("i2it_refold_weights: twin_r ") + (twin_r < 0.f ? "< 0 turns the TwinConv blend off" : ">= 0 turns the TwinConv blend on") +
+             " since the last fold; call i2it_finalize_weights");
+  // every master a recipe or a plan reads keeps its address and shape (set_weight copies same-shape tensors in place)
+  for (const auto& kv : w_) {
+    auto it = fold_shapes_.find(kv.first);
+    I2IT_CHECK(it != fold_shapes_.end(), "i2it_refold_weights: tensor '" + kv.first + "' was added since the last fold; "
+                                         "call i2it_finalize_weights");
+    I2IT_CHECK(it->second == kv.second.shape, "i2it_refold_weights: tensor '" + kv.first + "' changed shape since the last "
+                                              "fold; call i2it_finalize_weights");
+  }
+  I2IT_CHECK(w_.size() == fold_shapes_.size(), "i2it_refold_weights: a tensor has gone since the last fold; call i2it_finalize_weights");
+  float* cur[4] = {&lw_unet_, &lw_vae_, &skip_gamma_, &twin_r_};
+  const float next[4] = {lw_unet, lw_vae, skip_gamma, twin_r};
+  const unsigned bit[4] = {FOLD_LW_UNET, FOLD_LW_VAE, FOLD_GAMMA, FOLD_TWIN_R};
+  float prev[4];
+  unsigned changed = adapter_scale_ != fold_adapter_scale_ ? FOLD_ADAPTER_SCALE : 0u;
+  for (int i = 0; i < 4; ++i) {
+    prev[i] = *cur[i];
+    if (std::memcmp(&next[i], cur[i], sizeof(float)) != 0) changed |= bit[i];   // bitwise: 0 and -0 fold to different bits
+    *cur[i] = next[i];
+  }
+  // the recipes in creation order: a recipe runs after those whose outputs it reads, and its jobs are the ones a fresh
+  // finalize would push for it
+  std::vector<std::string> touched;
+  std::set<std::string> rebuilt;
+  try {
+    for (size_t i = 0; i < recipes_.size(); ++i) {
+      const Recipe& r = recipes_[i];
+      bool dirty = (r.uses & changed) != 0;
+      for (const auto& k : r.reads) dirty = dirty || dirty_w_.count(k) != 0;
+      for (const auto& k : r.after) dirty = dirty || rebuilt.count(k) != 0;
+      if (!dirty) continue;
+      run_recipe(i);
+      rebuilt.insert(recipes_[i].key);
+      touched.push_back(recipes_[i].key);
+    }
+  } catch (...) {
+    for (int i = 0; i < 4; ++i) *cur[i] = prev[i];
+    pending_jobs_.clear();
+    pending_blocks_ = 0;
+    for (auto& g : pending_gemv_) g.clear();
+    throw;
+  }
+  refold_touched_ = std::move(touched);
+  refold_jobs_ = static_cast<long long>(pending_jobs_.size());
+  refold_gemv_jobs_ = 0;
+  refold_bytes_ = 0;
+  for (const auto& j : pending_jobs_) refold_bytes_ += prep_job_bytes(j);
+  for (const auto& g : pending_gemv_) {
+    refold_gemv_jobs_ += static_cast<long long>(g.size());
+    for (const auto& j : g) refold_bytes_ += gemv_job_bytes(j);
+  }
+  flush_prep();
+  I2IT_CUDA(cudaDeviceSynchronize());
+  I2IT_CUDA(cudaGetLastError());
+  // cached cross-attention operands were projected with the old weights; their buffers stay (cached-text plans read them)
+  for (auto& kv : textkv_) kv.second->filled = false;
+  snapshot_fold();
+  finalized_ = true;
+}
+
+std::string Engine::refold_info_json() const {
+  std::string js = "{\"recipes\":[";
+  for (size_t i = 0; i < refold_touched_.size(); ++i) js += std::string(i ? "," : "") + "\"" + refold_touched_[i] + "\"";
+  return js + "],\"jobs\":" + std::to_string(refold_jobs_) + ",\"gemv_jobs\":" + std::to_string(refold_gemv_jobs_) +
+         ",\"bytes\":" + std::to_string(static_cast<long long>(refold_bytes_)) + "}";
 }
 
 // Fold recipe of a layer: c0*W (+ c1*W_other) + sum_adapters s_a * B_a @ A_a — filled into a job, evaluated on device
 void Engine::fill_fold(PrepJob& j, const std::string& name, float c0, const std::string& other, float c1) {
-  const WT& w = raw(name, "weight");
+  const WT& w = src(name, "weight");
   j.w0 = w.d; j.c0 = c0; j.w1 = nullptr; j.c1 = 0.f; j.n_adapters = 0;
   if (!other.empty()) {
-    const WT& o = raw(other, "weight");
+    const WT& o = src(other, "weight");
     I2IT_CHECK(o.numel == w.numel, "TwinConv shapes differ");
     j.w1 = o.d; j.c1 = c1;
   }
@@ -472,10 +648,9 @@ void Engine::fill_fold(PrepJob& j, const std::string& name, float c0, const std:
   for (const auto& adapter : adapters) {
     const float s = adapter_weight(name, adapter);
     if (s == 0.f) continue;
-    const WT& A = w_.at(pre + adapter + ".weight");
-    auto itb = w_.find(name + ".lora_B." + adapter + ".weight");
-    I2IT_CHECK(itb != w_.end(), "lora_A without lora_B for " + name);
-    const WT& Bm = itb->second;
+    const WT& A = src(name + ".lora_A." + adapter, "weight");
+    I2IT_CHECK(has(name + ".lora_B." + adapter + ".weight"), "lora_A without lora_B for " + name);
+    const WT& Bm = src(name + ".lora_B." + adapter, "weight");
     const int rank = static_cast<int>(A.shape[0]);
     const long long inner = A.numel / rank;
     I2IT_CHECK(Bm.shape[0] * inner == w.numel && Bm.shape[1] == rank, "LoRA shape mismatch at " + name);
@@ -502,6 +677,21 @@ void Engine::push_bias_job(float* out, const float* b, const float* add, int cou
   push_job(j);
 }
 
+void* Engine::upload_jobs(int table, const void* jobs, size_t bytes) {
+  JobTable& t = job_tables_[table];
+  if (t.cap < bytes) {
+    I2IT_CUDA(cudaDeviceSynchronize());   // an earlier flush's launch may still read the old table
+    cudaFree(t.p);
+    t.p = nullptr;
+    t.cap = 0;
+    I2IT_CUDA(cudaMalloc(&t.p, bytes));
+    t.cap = bytes;
+  }
+  // on the default stream, as the launches that read the table: ordered after the previous flush's launch
+  I2IT_CUDA(cudaMemcpy(t.p, jobs, bytes, cudaMemcpyHostToDevice));
+  return t.p;
+}
+
 // Runs every pending preparation job: <= 3 GEMV launches (time embedding chain) + ONE fold/re-layout launch.
 void Engine::flush_prep() {
   for (int st = 0; st < 3; ++st) {
@@ -509,16 +699,14 @@ void Engine::flush_prep() {
     if (g.empty()) continue;
     int warps = 0;
     for (auto& j : g) { j.warp0 = warps; warps += j.out; }
-    GemvJob* d = static_cast<GemvJob*>(dmalloc(g.size() * sizeof(GemvJob)));
-    I2IT_CUDA(cudaMemcpy(d, g.data(), g.size() * sizeof(GemvJob), cudaMemcpyHostToDevice));
+    GemvJob* d = static_cast<GemvJob*>(upload_jobs(st, g.data(), g.size() * sizeof(GemvJob)));
     gemv_jobs_kernel<<<ceil_div(warps * 32ll, 256), 256>>>(d, static_cast<int>(g.size()));
     I2IT_CUDA(cudaGetLastError());
     prep_launches_ += 1;
     g.clear();
   }
   if (!pending_jobs_.empty()) {
-    PrepJob* d = static_cast<PrepJob*>(dmalloc(pending_jobs_.size() * sizeof(PrepJob)));
-    I2IT_CUDA(cudaMemcpy(d, pending_jobs_.data(), pending_jobs_.size() * sizeof(PrepJob), cudaMemcpyHostToDevice));
+    PrepJob* d = static_cast<PrepJob*>(upload_jobs(3, pending_jobs_.data(), pending_jobs_.size() * sizeof(PrepJob)));
     I2IT_CHECK(pending_blocks_ < (1ll << 31), "weight preparation: too many blocks for one launch");
     DISPATCH_T(dtype, (prep_jobs_kernel<T><<<static_cast<unsigned>(pending_blocks_), 256>>>(d, static_cast<int>(pending_jobs_.size()))));
     I2IT_CUDA(cudaGetLastError());
@@ -528,8 +716,8 @@ void Engine::flush_prep() {
   }
 }
 
-PW Engine::prep(const std::string& cache_key, const std::vector<std::string>& names, bool geglu, float scale,
-                const float* bias_add) {
+PW Engine::prep(const std::string& cache_key, const std::vector<std::string>& names, bool geglu, bool skip_scale,
+                const std::string& bias_add) {
   auto it = prepared_.find(cache_key);
   if (it != prepared_.end()) return it->second;
   I2IT_CHECK(finalized_, "i2it_finalize_weights must be called before a forward");
@@ -538,7 +726,7 @@ PW Engine::prep(const std::string& cache_key, const std::vector<std::string>& na
   pw.cin = static_cast<int>(w0.shape[1]);
   pw.taps = (w0.shape.size() == 4) ? static_cast<int>(w0.shape[2] * w0.shape[3]) : 1;
   pw.cin_pad = round_up(pw.cin, 8);
-  bool any_bias = bias_add != nullptr;
+  bool any_bias = !bias_add.empty();
   for (const auto& n : names) {
     const WT& w = raw(n, "weight");
     I2IT_CHECK(static_cast<int>(w.shape[1]) == pw.cin, "fused projection with different input widths: " + n);
@@ -549,30 +737,34 @@ PW Engine::prep(const std::string& cache_key, const std::vector<std::string>& na
   const size_t wbytes = static_cast<size_t>(pw.taps) * pw.rows * pw.cin_pad * 2;
   pw.w = static_cast<uint16_t*>(dmalloc(wbytes));
   if (any_bias) pw.bias = static_cast<float*>(dmalloc(pw.rows * sizeof(float)));
-  int row_off = 0;
-  for (const auto& n : names) {
-    const int cout = static_cast<int>(raw(n, "weight").shape[0]);
-    const int half = geglu ? cout / 2 : 0;
-    PrepJob j;
-    std::memset(&j, 0, sizeof j);
-    fill_fold(j, n);
-    j.mode = PREP_STORE; j.out = pw.w; j.cout = cout; j.cin = pw.cin; j.taps = pw.taps; j.cin_pad = pw.cin_pad;
-    j.rows_total = pw.rows; j.row_off = row_off; j.interleave_half = half; j.scale = scale;
-    j.n = static_cast<long long>(cout) * pw.cin_pad * pw.taps;
-    push_job(j);
-    if (pw.bias) push_bias_job(pw.bias, has(n + ".bias") ? raw(n, "bias").d : nullptr, bias_add, cout, row_off, half);
-    row_off += cout;
-  }
+  add_recipe(cache_key, [this, pw, names, geglu, skip_scale, bias_add]() {
+    const float scale = skip_scale ? fold_input(FOLD_GAMMA) : 1.f;
+    const float* add = bias_add.empty() ? nullptr : f32_input(bias_add);
+    int row_off = 0;
+    for (const auto& n : names) {
+      const int cout = static_cast<int>(raw(n, "weight").shape[0]);
+      const int half = geglu ? cout / 2 : 0;
+      PrepJob j;
+      std::memset(&j, 0, sizeof j);
+      fill_fold(j, n);
+      j.mode = PREP_STORE; j.out = pw.w; j.cout = cout; j.cin = pw.cin; j.taps = pw.taps; j.cin_pad = pw.cin_pad;
+      j.rows_total = pw.rows; j.row_off = row_off; j.interleave_half = half; j.scale = scale;
+      j.n = static_cast<long long>(cout) * pw.cin_pad * pw.taps;
+      push_job(j);
+      if (pw.bias) push_bias_job(pw.bias, has(n + ".bias") ? src(n, "bias").d : nullptr, add, cout, row_off, half);
+      row_off += cout;
+    }
+  });
   prepared_[cache_key] = pw;
   return pw;
 }
 
-PW Engine::prep_twin(const std::string& pre, const std::string& cur, float r) {
+PW Engine::prep_twin(const std::string& pre, const std::string& cur) {
   const std::string key = pre + "|twin";
   auto it = prepared_.find(key);
   if (it != prepared_.end()) return it->second;
-  I2IT_CHECK(r >= 0.f, "the state dict has a TwinConv conv_in but no blend ratio r was given (deterministic forward on a "
-                       "sketch_to_image_stochastic model is undefined in the reference too)");
+  I2IT_CHECK(twin_r_ >= 0.f, "the state dict has a TwinConv conv_in but no blend ratio r was given (deterministic forward on a "
+                             "sketch_to_image_stochastic model is undefined in the reference too)");
   PW pw;
   const WT& w0 = raw(pre, "weight");
   pw.rows = static_cast<int>(w0.shape[0]);
@@ -581,14 +773,17 @@ PW Engine::prep_twin(const std::string& pre, const std::string& cur, float r) {
   pw.cin_pad = round_up(pw.cin, 8);
   pw.w = static_cast<uint16_t*>(dmalloc(static_cast<size_t>(pw.taps) * pw.rows * pw.cin_pad * 2));
   pw.bias = static_cast<float*>(dmalloc(pw.rows * sizeof(float)));
-  PrepJob j;
-  std::memset(&j, 0, sizeof j);
-  fill_fold(j, pre, 1.f - r, cur, r);                       // W = (1-r) W_pre + r W_cur   (pix2pix_turbo.py:23-26)
-  j.mode = PREP_STORE; j.out = pw.w; j.cout = pw.rows; j.cin = pw.cin; j.taps = pw.taps; j.cin_pad = pw.cin_pad;
-  j.rows_total = pw.rows; j.scale = 1.f;
-  j.n = static_cast<long long>(pw.rows) * pw.cin_pad * pw.taps;
-  push_job(j);
-  push_bias_job(pw.bias, raw(pre, "bias").d, nullptr, pw.rows, 0, 0, 1.f - r, raw(cur, "bias").d, r);   // (1-r) b_pre + r b_cur
+  add_recipe(key, [this, pw, pre, cur]() {
+    const float r = fold_input(FOLD_TWIN_R);
+    PrepJob j;
+    std::memset(&j, 0, sizeof j);
+    fill_fold(j, pre, 1.f - r, cur, r);                       // W = (1-r) W_pre + r W_cur   (pix2pix_turbo.py:23-26)
+    j.mode = PREP_STORE; j.out = pw.w; j.cout = pw.rows; j.cin = pw.cin; j.taps = pw.taps; j.cin_pad = pw.cin_pad;
+    j.rows_total = pw.rows; j.scale = 1.f;
+    j.n = static_cast<long long>(pw.rows) * pw.cin_pad * pw.taps;
+    push_job(j);
+    push_bias_job(pw.bias, src(pre, "bias").d, nullptr, pw.rows, 0, 0, 1.f - r, src(cur, "bias").d, r);   // (1-r) b_pre + r b_cur
+  });
   prepared_[key] = pw;
   return pw;
 }
@@ -603,13 +798,15 @@ PW Engine::prep_im2col3(const std::string& name) {
   pw.rows = static_cast<int>(w0.shape[0]); pw.cin = 32; pw.cin_pad = 32; pw.taps = 1;
   pw.w = static_cast<uint16_t*>(dmalloc(static_cast<size_t>(pw.rows) * 32 * 2));
   pw.bias = static_cast<float*>(dmalloc(pw.rows * sizeof(float)));
-  PrepJob j;
-  std::memset(&j, 0, sizeof j);
-  fill_fold(j, name);
-  j.mode = PREP_IM2COL3; j.out = pw.w; j.cout = pw.rows; j.cin = 3; j.taps = 9; j.scale = 1.f;
-  j.n = static_cast<long long>(pw.rows) * 32;
-  push_job(j);
-  push_bias_job(pw.bias, raw(name, "bias").d, nullptr, pw.rows, 0, 0);
+  add_recipe(key, [this, pw, name]() {
+    PrepJob j;
+    std::memset(&j, 0, sizeof j);
+    fill_fold(j, name);
+    j.mode = PREP_IM2COL3; j.out = pw.w; j.cout = pw.rows; j.cin = 3; j.taps = 9; j.scale = 1.f;
+    j.n = static_cast<long long>(pw.rows) * 32;
+    push_job(j);
+    push_bias_job(pw.bias, src(name, "bias").d, nullptr, pw.rows, 0, 0);
+  });
   prepared_[key] = pw;
   return pw;
 }
@@ -621,10 +818,12 @@ PW Engine::prep_identity(int n) {
   PW pw;
   pw.rows = n; pw.cin = n; pw.cin_pad = n; pw.taps = 1;
   pw.w = static_cast<uint16_t*>(dmalloc(static_cast<size_t>(n) * n * 2));
-  PrepJob j;
-  std::memset(&j, 0, sizeof j);
-  j.mode = PREP_IDENTITY; j.out = pw.w; j.cout = n; j.n = static_cast<long long>(n) * n;
-  push_job(j);
+  add_recipe(key, [this, pw, n]() {
+    PrepJob j;
+    std::memset(&j, 0, sizeof j);
+    j.mode = PREP_IDENTITY; j.out = pw.w; j.cout = n; j.n = static_cast<long long>(n) * n;
+    push_job(j);
+  });
   prepared_[key] = pw;
   return pw;
 }
@@ -640,13 +839,15 @@ PW Engine::prep_subpixel(const std::string& name) {
   const long long total = 16ll * pw.rows * pw.cin_pad;
   pw.w = static_cast<uint16_t*>(dmalloc(static_cast<size_t>(total) * 2));
   pw.bias = static_cast<float*>(dmalloc(pw.rows * sizeof(float)));
-  PrepJob j;
-  std::memset(&j, 0, sizeof j);
-  fill_fold(j, name);
-  j.mode = PREP_SUBPIXEL; j.out = pw.w; j.cout = pw.rows; j.cin = pw.cin; j.taps = 9; j.cin_pad = pw.cin_pad; j.scale = 1.f;
-  j.n = total;
-  push_job(j);
-  push_bias_job(pw.bias, raw(name, "bias").d, nullptr, pw.rows, 0, 0);
+  add_recipe(key, [this, pw, name, total]() {
+    PrepJob j;
+    std::memset(&j, 0, sizeof j);
+    fill_fold(j, name);
+    j.mode = PREP_SUBPIXEL; j.out = pw.w; j.cout = pw.rows; j.cin = pw.cin; j.taps = 9; j.cin_pad = pw.cin_pad; j.scale = 1.f;
+    j.n = total;
+    push_job(j);
+    push_bias_job(pw.bias, src(name, "bias").d, nullptr, pw.rows, 0, 0);
+  });
   prepared_[key] = pw;
   return pw;
 }
@@ -676,22 +877,22 @@ NormW Engine::norm(const std::string& name) {
   return n;
 }
 
-const float* Engine::temb_bias(const std::string& p) {
+std::string Engine::temb_bias(const std::string& p) {
   const std::string key = p + "|temb";
-  auto it = prepared_f32_.find(key);
-  if (it != prepared_f32_.end()) return it->second;
+  if (prepared_f32_.count(key)) return key;
   const int T = cfg.temb_dim, C0 = cfg.unet_channels[0];
-  auto gemv = [&](int stage, const std::string& name, const float* x, float* y, int out, int in, int silu) {
+  auto gemv = [this](int stage, const std::string& name, const float* x, float* y, int out, int in, int silu) {
     PrepJob f;
     std::memset(&f, 0, sizeof f);
     fill_fold(f, name);
     GemvJob g;
     std::memset(&g, 0, sizeof g);
-    g.w = f.w0; g.b = raw(name, "bias").d; g.x = x; g.y = y; g.out = out; g.in = in; g.silu_out = silu;
+    g.w = f.w0; g.b = src(name, "bias").d; g.x = x; g.y = y; g.out = out; g.in = in; g.silu_out = silu;
     g.n_adapters = f.n_adapters;
     for (int a = 0; a < f.n_adapters; ++a) { g.A[a] = f.A[a]; g.B[a] = f.B[a]; g.s[a] = f.s[a]; g.rank[a] = f.rank[a]; }
     pending_gemv_[stage].push_back(g);
   };
+  static const std::string emb = "unet.time_embedding|emb";   // the shared embedding: a recipe of its own, in no cache
   if (!emb_act_) {
     // Timesteps(flip_sin_to_cos=True, freq_shift=0) at t = 999, then TimestepEmbedding, then the SiLU every resnet applies
     std::vector<float> te(C0);
@@ -703,17 +904,24 @@ const float* Engine::temb_bias(const std::string& p) {
     }
     float* d_te = static_cast<float*>(dmalloc(C0 * sizeof(float)));
     float* d_h = static_cast<float*>(dmalloc(T * sizeof(float)));
-    emb_act_ = static_cast<float*>(dmalloc(T * sizeof(float)));
+    float* e = static_cast<float*>(dmalloc(T * sizeof(float)));
     I2IT_CUDA(cudaMemcpy(d_te, te.data(), C0 * sizeof(float), cudaMemcpyHostToDevice));
-    gemv(0, "unet.time_embedding.linear_1", d_te, d_h, T, C0, 1);
-    gemv(1, "unet.time_embedding.linear_2", d_h, emb_act_, T, T, 1);
+    add_recipe(emb, [=]() {
+      gemv(0, "unet.time_embedding.linear_1", d_te, d_h, T, C0, 1);
+      gemv(1, "unet.time_embedding.linear_2", d_h, e, T, T, 1);
+    });
+    emb_act_ = e;
   }
   const WT& w = raw(p + ".time_emb_proj", "weight");
   const int cout = static_cast<int>(w.shape[0]);
   float* out = static_cast<float*>(dmalloc(cout * sizeof(float)));
-  gemv(2, p + ".time_emb_proj", emb_act_, out, cout, T, 0);
+  float* e = emb_act_;
+  add_recipe(key, [=]() {
+    recipes_[recording_].after.push_back(emb);
+    gemv(2, p + ".time_emb_proj", e, out, cout, T, 0);
+  });
   prepared_f32_[key] = out;
-  return out;
+  return key;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1659,7 +1867,7 @@ bool Engine::check_forward(int B, int H, int W, int text_batch, const void* text
   if (text) return false;
   auto it = textkv_.find(text_batch);
   I2IT_CHECK(it != textkv_.end() && it->second->filled,
-             "text_emb == NULL: call i2it_set_text first (and again after every i2it_finalize_weights)");
+             "text_emb == NULL: call i2it_set_text first (and again after every i2it_finalize_weights or i2it_refold_weights)");
   return true;
 }
 

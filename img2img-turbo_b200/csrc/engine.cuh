@@ -5,6 +5,7 @@
 #include <functional>
 #include <map>
 #include <memory>
+#include <set>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -230,6 +231,20 @@ struct WT {                      // raw fp32 tensor of the state dict, on device
   long long numel = 0;
 };
 
+// The fold inputs a prepared weight's coefficients read (Recipe::uses)
+enum FoldInput : unsigned { FOLD_LW_UNET = 1, FOLD_LW_VAE = 2, FOLD_GAMMA = 4, FOLD_TWIN_R = 8, FOLD_ADAPTER_SCALE = 16 };
+
+// How a prepared weight was made, so Engine::refold can push its jobs again into the same buffers: `emit` is the prep_*
+// or temb_bias call that made it (with its arguments), and reads the engine's fold inputs when it runs.  uses / reads /
+// after are recorded by each run.
+struct Recipe {
+  std::string key;                   // its prepared_ / prepared_f32_ key
+  std::function<void()> emit;
+  unsigned uses = 0;                 // FoldInput bits
+  std::vector<std::string> reads;    // master tensors its jobs read
+  std::vector<std::string> after;    // recipes whose outputs its jobs read (a UNet conv1 bias reads its time-embedding GEMV)
+};
+
 // cached cross-attention operands of one prompt batch: K [tb*77, C] and V^T [tb][C][80] per transformer block
 struct TextKV {
   Plan plan;                                   // declared first: its pool outlives the Acts below
@@ -250,6 +265,9 @@ class Engine {
   void set_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dt, bool is_dev);
   void set_adapter_scale(const std::string& a, float s) { adapter_scale_[a] = s; }
   void finalize(float lw_unet, float lw_vae, float skip_gamma, float twin_r);
+  // i2it_refold_weights: rewrite, in place, the prepared weights whose fold inputs changed since the last fold
+  void refold(float lw_unet, float lw_vae, float skip_gamma, float twin_r);
+  std::string refold_info_json() const;                               // i2it_debug_refold_info
   // g: LANCZOS resize geometry of a uint8 forward (i2it_forward_u8_resize); part of the plan key
   // evict: enforce the plan limit once the plan is in (forward() does it itself after the plan becomes the last-run one)
   // max_side: the capacity of an IO_RAGGED plan (part of its key)
@@ -322,15 +340,17 @@ class Engine {
   // ---- weights ----
   bool has(const std::string& key) const;
   const WT& raw(const std::string& name, const char* what) const;   // accepts X.what or X.base_layer.what
+  // skip_scale: scaled by the skip-conv gamma; bias_add: key of an fp32 vector added to the bias (a master tensor, or a
+  // temb_bias output)
   PW prep(const std::string& cache_key, const std::vector<std::string>& names, bool geglu = false,
-          float scale = 1.f, const float* bias_add = nullptr);
-  PW prep_twin(const std::string& pre, const std::string& cur, float r);
+          bool skip_scale = false, const std::string& bias_add = "");
+  PW prep_twin(const std::string& pre, const std::string& cur);     // blended at the fold's twin_r
   PW prep_im2col3(const std::string& name);
   PW prep_identity(int n);                                          // [n][n] identity as a 1x1 'weight'
   PW prep_subpixel(const std::string& name);                       // 16 pre-summed 2x2 taps for upsample2x+conv3x3
   Act conv_up2x(Plan& P, const Act& x, const PW& wsub, const Act* x2, const PW* w2, bool gn_out = false);                        // 3x3 conv over 3 channels as a K=32 single-tap GEMM
   NormW norm(const std::string& name);
-  const float* temb_bias(const std::string& resnet_prefix);          // time_emb_proj(silu(emb)) at t=999
+  std::string temb_bias(const std::string& resnet_prefix);          // time_emb_proj(silu(emb)) at t=999: its prepared_f32_ key
   void free_prepared();
   void flush_prep();                                                // run all pending preparation jobs (4-5 launches)
   int prep_launches_ = 0;
@@ -389,6 +409,7 @@ class Engine {
   std::unordered_map<std::string, float> adapter_scale_;
   float lw_unet_ = 1.f, lw_vae_ = 1.f, skip_gamma_ = 1.f, twin_r_ = -1.f;
   bool finalized_ = false;
+  bool folded_ = false;                                     // finalized at least once
   std::unordered_map<std::string, PW> prepared_;
   std::unordered_map<std::string, float*> prepared_f32_;
   std::vector<void*> prep_allocs_;
@@ -396,6 +417,26 @@ class Engine {
   std::vector<PrepJob> pending_jobs_;
   std::vector<GemvJob> pending_gemv_[3];
   long long pending_blocks_ = 0;
+  // device job tables of flush_prep (three GEMV stages, the preparation jobs): reused, grown when a flush needs more
+  struct JobTable { void* p = nullptr; size_t cap = 0; };
+  JobTable job_tables_[4];
+  void* upload_jobs(int table, const void* jobs, size_t bytes);
+  // ---- refold state ----
+  std::vector<Recipe> recipes_;                             // every prepared weight's recipe, in creation order
+  long long recording_ = -1;                                // index of the recipe being run: fill_fold & co. record into it
+  std::set<std::string> dirty_w_;                           // masters registered since the last fold
+  std::map<std::string, std::vector<int64_t>> fold_shapes_; // every master's shape at the last fold
+  std::unordered_map<std::string, float> fold_adapter_scale_;
+  std::vector<void*> retired_;                              // replaced masters plans may still read: freed by finalize
+  std::vector<std::string> refold_touched_;                 // the last refold's rebuilt recipes
+  long long refold_jobs_ = 0, refold_gemv_jobs_ = 0;
+  double refold_bytes_ = 0;
+  void add_recipe(const std::string& key, std::function<void()> emit);
+  void run_recipe(size_t i);
+  const WT& src(const std::string& name, const char* what);   // raw() that records the read in the running recipe
+  const float* f32_input(const std::string& key);             // a master tensor or a prepared fp32 vector, recorded
+  float fold_input(FoldInput which);                          // a fold scalar, recorded
+  void snapshot_fold();
   void fill_fold(PrepJob& j, const std::string& name, float c0 = 1.f, const std::string& other = "", float c1 = 0.f);
   void push_job(PrepJob& j);
   void push_bias_job(float* out, const float* b, const float* add, int cout, int row_off, int half, float c0 = 1.f,
@@ -426,7 +467,7 @@ class Engine {
   Act text_;                     // staged text embedding while a UNet plan is being built
   TextKV* text_kv_ = nullptr;    // ... or the cached cross-attention operands (text_emb == NULL forwards)
 
-  float adapter_weight(const std::string& name, const std::string& adapter) const;
+  float adapter_weight(const std::string& name, const std::string& adapter);
   void* dmalloc(size_t bytes);
 };
 

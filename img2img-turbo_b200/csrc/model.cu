@@ -35,7 +35,7 @@ Act Engine::vae_resnet(Plan& P, const std::string& p, const Act& x, const Act* s
     // pre-added to conv2's, so there is no separate launch and no residual read
     I2IT_CHECK(skip == nullptr, "vae_resnet: shortcut and skip source at once");
     PW wsc = prep(p + ".conv_shortcut", {p + ".conv_shortcut"});
-    PW w2 = prep(p + ".conv2+sc", {p + ".conv2"}, false, 1.f, raw(p + ".conv_shortcut", "bias").d);
+    PW w2 = prep(p + ".conv2+sc", {p + ".conv2"}, false, false, p + ".conv_shortcut.bias");
     o.x2 = &x; o.w2 = &wsc;
     Act y = conv(P, h, w2, o);
     mark_layer(P, p + ".conv2", y);
@@ -150,7 +150,7 @@ void Engine::build_vae_decoder(Plan& P, const std::string& vp, const Act& dec_in
   // `sample = sample + skip_conv_i(skip_i * gamma)` (src/model.py:40-42) is folded into whichever conv PRODUCES `sample`
   // for up-block i: mid_block.resnets.1.conv2 for i = 0, the previous block's upsampler conv for i >= 1.  gamma is folded
   // into the bias-free 1x1 weights.
-  auto skip_w = [&](int i) { const std::string sk = d + ".skip_conv_" + std::to_string(i + 1); return prep(sk, {sk}, false, skip_gamma_); };
+  auto skip_w = [&](int i) { const std::string sk = d + ".skip_conv_" + std::to_string(i + 1); return prep(sk, {sk}, false, true); };
   // the skip that skip_conv_(k+1) reads.  A variations forward encoded one image: its batch-1 skip is replicated to the
   // decoder's batch right before the block that reads it, so a batch-n copy lives for one layer, not across the UNet
   auto skip_in = [&](int i, int k) {
@@ -200,7 +200,7 @@ Act Engine::unet_resnet(Plan& P, const std::string& p, const Act& x, bool gn_nex
   mark_layer(P, p + ".norm1", h);
   // t == 999 always: time_emb_proj(silu(emb)) is a per-channel constant -> part of conv1's bias
   ConvOpts o1; o1.gn_out = true;
-  h = conv(P, h, prep(p + ".conv1", {p + ".conv1"}, false, 1.f, temb_bias(p)), o1);
+  h = conv(P, h, prep(p + ".conv1", {p + ".conv1"}, false, false, temb_bias(p)), o1);
   mark_layer(P, p + ".conv1", h);
   h = group_norm(P, h, norm(p + ".norm2"), 1e-5f, true);
   mark_layer(P, p + ".norm2", h);
@@ -209,7 +209,7 @@ Act Engine::unet_resnet(Plan& P, const std::string& p, const Act& x, bool gn_nex
   o.out = out;
   if (has(p + ".conv_shortcut.weight")) {
     PW wsc = prep(p + ".conv_shortcut", {p + ".conv_shortcut"});
-    PW w2 = prep(p + ".conv2+sc", {p + ".conv2"}, false, 1.f, raw(p + ".conv_shortcut", "bias").d);
+    PW w2 = prep(p + ".conv2+sc", {p + ".conv2"}, false, false, p + ".conv_shortcut.bias");
     o.x2 = &x; o.w2 = &wsc;
     Act y = conv(P, h, w2, o);
     mark_layer(P, p + ".conv2", y);
@@ -357,7 +357,7 @@ Act Engine::build_unet(Plan& P, const Act& z, int text_batch, bool text_cached) 
     ConvOpts oc; oc.gn_out = true;
     if (fuse) oc.out = &t.skip;
     if (has(u + ".conv_in.conv_in_pretrained.weight"))
-      s = conv(P, z, prep_twin(u + ".conv_in.conv_in_pretrained", u + ".conv_in.conv_in_curr", twin_r_), oc);
+      s = conv(P, z, prep_twin(u + ".conv_in.conv_in_pretrained", u + ".conv_in.conv_in_curr"), oc);
     else
       s = conv(P, z, prep(u + ".conv_in", {u + ".conv_in"}), oc);
     mark_layer(P, u + ".conv_in", s);

@@ -122,7 +122,7 @@ class CycleGAN_Turbo(TurboBase):
         for part in ("sd_vae_enc", "sd_vae_dec"):
             for k, v in sd[part].items():          # keys already carry "vae." / "vae_b2a." (VAE_encode/VAE_decode state dicts)
                 self._sd[k.replace(".base_layer.", ".")] = v.detach().float().cpu()
-        self._invalidate()
+        self._reload()
 
     def load_ckpt_from_url(self, url, ckpt_folder):
         os.makedirs(ckpt_folder, exist_ok=True)

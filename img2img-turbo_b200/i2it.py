@@ -35,6 +35,7 @@ SYMBOLS = [
     "i2it_set_max_plans", "i2it_release_plans", "i2it_memory_stats_get", "i2it_debug_poison_workspace",
     "i2it_debug_tapgemm_override", "i2it_forward_variations", "i2it_forward_u8_variations",
     "i2it_forward_u8_ragged", "i2it_op_resize_u8_ragged", "i2it_debug_ragged_tables", "i2it_debug_graph_captures",
+    "i2it_refold_weights", "i2it_debug_refold_info",
 ]
 TEXT_TOKEN_EMB = "text_encoder.text_model.embeddings.token_embedding.weight"
 TEXT_POS_EMB = "text_encoder.text_model.embeddings.position_embedding.weight"
@@ -212,6 +213,8 @@ def load_library(path: Optional[str] = None):
     lib.i2it_debug_ragged_tables.argtypes = [C.POINTER(ResizeDesc), ci, ci, ci, ci, C.POINTER(C.c_longlong),
                                              C.POINTER(C.c_longlong)]
     lib.i2it_debug_graph_captures.argtypes = [vp, C.POINTER(ci)]
+    lib.i2it_refold_weights.argtypes = [vp, cf, cf, cf, cf]
+    lib.i2it_debug_refold_info.argtypes = [vp, C.c_char_p, C.c_size_t]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("i2it_destroy", "i2it_last_error"):
@@ -313,6 +316,14 @@ class Engine:
         self._text_batch = None          # cached text projections die with the folded weights
         self._check(self.lib.i2it_finalize_weights(self._h, lora_weight_unet, lora_weight_vae, skip_gamma, twin_r),
                     "i2it_finalize_weights")
+
+    def refold(self, lora_weight_unet: float = 1.0, lora_weight_vae: float = 1.0, skip_gamma: float = 1.0,
+               twin_r: float = -1.0):
+        """Fold again in place (i2it_refold_weights): new scalars, or tensors re-registered with their shapes since the last
+        fold.  Plans and their CUDA graphs stay; the set_text cache is dropped, as after finalize."""
+        self._check(self.lib.i2it_refold_weights(self._h, lora_weight_unet, lora_weight_vae, skip_gamma, twin_r),
+                    "i2it_refold_weights")
+        self._text_batch = None          # a refused refold keeps the cache, as the engine does
 
     # ---- the hot path ----------------------------------------------------------------------------
     def set_text(self, text_emb: torch.Tensor):
@@ -545,6 +556,11 @@ class Engine:
     def text_stage_names(self):
         """[(name, (N, C, H, W))] of every stage the last encode_text kept, in build order (read them with read_stage)."""
         return [(s["name"], tuple(s["dims"])) for s in self._json(self.lib.i2it_text_stage_names, "i2it_text_stage_names")]
+
+    def _debug_refold_info(self) -> dict:
+        """What the last refold rebuilt: {"recipes": prepared-weight keys in fold order, "jobs", "gemv_jobs", "bytes": the
+        algorithmic bytes those jobs read and write}."""
+        return self._json(self.lib.i2it_debug_refold_info, "i2it_debug_refold_info")
 
     def prepared_keys(self):
         """Cache keys of every prepared weight (plain layer names, "+sc", ".qk", "|twin", "|im2col", "|subpixel", "identity|n")."""

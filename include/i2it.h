@@ -69,7 +69,11 @@ const char* i2it_last_error(const i2it_handle* h);   /* h may be NULL: last erro
 /* Register one tensor of the state dict.  `key` is "<model>.<diffusers key>" with model in
  * {unet, vae, vae_b2a}; peft spellings ("X.base_layer.weight", "X.lora_A.<adapter>.weight",
  * "X.lora_B.<adapter>.weight") are accepted as-is.  `data` may be a host or device pointer
- * (is_device); dtype is I2IT_F32/F16/BF16.  The engine keeps an fp32 device copy (synchronous).
+ * (is_device); dtype is I2IT_F32/F16/BF16.  The engine keeps an fp32 device copy (synchronous).  A key registered again
+ * with the same shape is copied into its existing copy after the handle's work drains (plans read some tensors, such as
+ * the norm scales, directly), so i2it_refold_weights can fold it in place.  A key registered again with another shape gets
+ * a new copy; the old one stays allocated until the next i2it_finalize_weights or i2it_destroy, because resident plans may
+ * still read it.
  * Replaces load_state_dict at src/pix2pix_turbo.py:66-78, cyclegan_turbo.py:162-190. */
 int i2it_set_weight(i2it_handle* h, const char* key, const void* data, const int64_t* shape, int ndim,
                     int dtype, int is_device);
@@ -87,6 +91,18 @@ int i2it_set_adapter_scale(i2it_handle* h, const char* adapter, float alpha_over
  * requested" (error if the state dict has a TwinConv). */
 int i2it_finalize_weights(i2it_handle* h, float lora_weight_unet, float lora_weight_vae, float skip_gamma,
                           float twin_r);
+
+/* Fold again with new scalars, or after i2it_set_weight re-registered tensors of an unchanged shape, writing the prepared
+ * weights in place.  Synchronous: it waits for the handle's work, rebuilds only the prepared weights whose fold inputs
+ * changed (a scalar they read, or a tensor re-registered since the last fold) in one preparation launch plus at most three
+ * time-embedding GEMV launches, and waits for them.  Every prepared weight is then bit-identical to what
+ * i2it_finalize_weights with the same arguments would write.
+ * Kept: every forward plan and its CUDA graphs, the workspace arena, the text-tower plans.  Dropped: the i2it_set_text
+ * cache (the projections carry the LoRA scale), with the same error as after i2it_finalize_weights.
+ * Refused, with nothing changed, when the handle was never finalized, when twin_r < 0 differs from twin_r < 0 at the last
+ * fold, or when a tensor was added, or re-registered with another shape, since the last fold: those need
+ * i2it_finalize_weights. */
+int i2it_refold_weights(i2it_handle* h, float lora_weight_unet, float lora_weight_vae, float skip_gamma, float twin_r);
 
 /* Bytes of device workspace the engine holds for a (batch, H, W) forward: the last forward's plan when it has this shape,
  * else the plan is built.  Every buffer grows linearly in H*W (the VAE attention runs fused above 8192 tokens).
@@ -141,7 +157,8 @@ int i2it_forward(i2it_handle* h, const void* x, const void* text_emb, int text_b
 /* Project and cache the cross-attention operands of a prompt: K = to_k(text_emb), V^T = to_v(text_emb)^T for every
  * transformer block (32 small launches, enqueued on `stream`).  text_emb [text_batch, 77, cross] device pointer in the
  * handle dtype; it is consumed before the call returns control to the stream order (the caller may reuse the buffer after
- * the stream reaches this point).  Must be called again after i2it_finalize_weights (the projections carry the LoRA scale).
+ * the stream reaches this point).  Must be called again after i2it_finalize_weights or i2it_refold_weights (the projections carry the LoRA
+ * scale).
  * Replaces the per-forward `attn2.to_k / attn2.to_v` calls under unet(...) at src/pix2pix_turbo.py:199. */
 int i2it_set_text(i2it_handle* h, const void* text_emb, int text_batch, void* stream);
 
@@ -247,6 +264,10 @@ int i2it_debug_ragged_tables(const i2it_resize_desc* g, int n, int H, int W, int
 
 /* CUDA graphs the handle has captured since create (a replay captures none). */
 int i2it_debug_graph_captures(i2it_handle* h, int* captures);
+
+/* What the last i2it_refold_weights rebuilt, as JSON: {"recipes": [prepared-weight keys, in fold order], "jobs": preparation
+ * jobs, "gemv_jobs": time-embedding GEMV jobs, "bytes": algorithmic bytes those jobs read and write}. */
+int i2it_debug_refold_info(i2it_handle* h, char* json, size_t cap);
 
 /* Per-launch device timing of the plan the LAST forward used: runs it `reps` more times with CUDA events around
  * every launch and writes a JSON array [{"i","kind","ms","flops","bytes","shape"}...] (algorithmic flops/bytes per
