@@ -445,7 +445,9 @@ class TurboBase(torch.nn.Module):
         st["eps"].copy_(eps, non_blocking=True)
         if noise is not None:
             st["noise"].copy_(noise, non_blocking=True)
-        if u8_mode is None:
+        if isinstance(direction, list):          # one direction per image: CycleGAN's mixed-direction forward
+            eng.forward_mixed(st["x"], None, st["eps"], direction, out=st["out"])
+        elif u8_mode is None:
             fwd = eng.forward_variations if variations else eng.forward
             fwd(st["x"], None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction, out=st["out"])
         else:
@@ -468,6 +470,8 @@ class TurboBase(torch.nn.Module):
         st["eps"].copy_(eps, non_blocking=True)
         if noise is not None:
             st["noise"].copy_(noise, non_blocking=True)
+        if isinstance(direction, list):
+            return eng.forward_u8_ragged_mixed(images, u8_mode, None, st["eps"], direction, geometries=geometries)
         return eng.forward_u8_ragged(images, u8_mode, None, st["eps"], noise_map=st["noise"], r=float(r), direction=direction,
                                      geometries=geometries)
 

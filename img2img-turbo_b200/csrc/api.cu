@@ -233,6 +233,42 @@ int i2it_forward_u8_ragged(i2it_handle* h, const void* const* x_u8, int in_mode,
   API_END
 }
 
+int i2it_forward_mixed(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps, void* out,
+                       void* out_latent, int batch, int H, int W, const int* directions, void* stream) {
+  API_BEGIN(h)
+  IO io;
+  std::memset(&io, 0, sizeof io);
+  io.x = x; io.text = text_emb; io.eps = eps; io.out = out; io.out_latent = out_latent;
+  E.check_device_error();
+  E.forward_mixed(io, directions, batch, H, W, text_batch, static_cast<cudaStream_t>(stream));
+  API_END
+}
+
+int i2it_forward_u8_ragged_mixed(i2it_handle* h, const void* const* x_u8, int in_mode, const i2it_resize_desc* g, int max_side,
+                                 const void* text_emb, int text_batch, const void* eps, void* const* out_u8, void* out_latent,
+                                 int n, int H, int W, const int* directions, void* stream) {
+  API_BEGIN(h)
+  I2IT_CHECK(n >= 1, "i2it_forward_u8_ragged_mixed: n must be >= 1");
+  I2IT_CHECK(in_mode >= 0 && in_mode <= 2, "i2it_forward_u8_ragged_mixed: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
+  E.check_mixed(directions, n, H, W);
+  IO io;
+  std::memset(&io, 0, sizeof io);
+  io.in_mode = in_mode; io.text = text_emb; io.eps = eps; io.out_latent = out_latent;
+  E.check_device_error();
+  E.forward_ragged(io, x_u8, out_u8, g, max_side, n, H, W, I2IT_A2B, text_batch, static_cast<cudaStream_t>(stream), directions);
+  API_END
+}
+
+int i2it_mixed_size_check(int H, int W, char* msg, size_t cap) {
+  const std::string why = i2it::mixed_size_rule(H, W);
+  if (msg && cap > 0) {
+    const size_t n = std::min(cap - 1, why.size());
+    std::memcpy(msg, why.data(), n);
+    msg[n] = 0;
+  }
+  return why.empty() ? 0 : 1;
+}
+
 int i2it_debug_ragged_tables(const i2it_resize_desc* g, int n, int H, int W, int max_side, long long* used, long long* bound) {
   try {
     i2it::rs_check_ragged(g, n, H, W, max_side);
@@ -363,7 +399,10 @@ static Act view(const void* p, int N, int H, int W, int C, int ld) {
   return a;
 }
 
-int i2it_op_conv2d_ex(i2it_handle* h, const i2it_conv_desc* d, void* stream) {
+// the b2a weight set and directions of i2it_op_conv2d_sel
+struct OpSel { const float* w; const float* bias; const float* w2; const int* dirs; };
+
+static int op_conv(i2it_handle* h, const i2it_conv_desc* d, const OpSel* sel, void* stream) {
   API_BEGIN(h)
   I2IT_CHECK(d && d->x && d->w && d->out, "i2it_op_conv2d_ex: null operand");
   const int stride = d->stride > 0 ? d->stride : 1, k = d->ksize, oc = (d->act == TG_ACT_GEGLU) ? d->Cout / 2 : d->Cout;
@@ -380,10 +419,33 @@ int i2it_op_conv2d_ex(i2it_handle* h, const i2it_conv_desc* d, void* stream) {
     const int64_t w2shape[4] = {d->Cout, d->C2, 1, 1};
     E.set_weight("__op.conv2.weight", d->w2, w2shape, 4, I2IT_F32, true);
   }
+  if (sel) {
+    I2IT_CHECK(sel->w && !sel->bias == !d->bias, "i2it_op_conv2d_sel: w_alt is required, and bias_alt iff bias");
+    I2IT_CHECK(sel->dirs, "i2it_op_conv2d_sel: null direction array");
+    for (int i = 0; i < d->N; ++i)
+      I2IT_CHECK(sel->dirs[i] == 0 || sel->dirs[i] == 1, "i2it_op_conv2d_sel: direction " + std::to_string(sel->dirs[i]) +
+                                                             " of image " + std::to_string(i) + " is neither 0 nor 1");
+    E.set_weight("__op.convb.weight", sel->w, wshape, 4, I2IT_F32, true);
+    if (d->bias) { const int64_t bshape[1] = {d->Cout}; E.set_weight("__op.convb.bias", sel->bias, bshape, 1, I2IT_F32, true); }
+    if (d->x2 && sel->w2) {
+      const int64_t w2shape[4] = {d->Cout, d->C2, 1, 1};
+      E.set_weight("__op.conv2b.weight", sel->w2, w2shape, 4, I2IT_F32, true);
+    }
+  }
   E.finalize(1.f, 1.f, 1.f, -1.f);
   {
     Plan P;
     P.debug_tapgemm = true;
+    if (sel) {
+      P.dir = static_cast<int*>(P.pool.get_fresh(static_cast<size_t>(d->N) * sizeof(int)));
+      I2IT_CUDA(cudaMemcpy(P.dir, sel->dirs, static_cast<size_t>(d->N) * sizeof(int), cudaMemcpyHostToDevice));
+    }
+    // the selecting op: each weight carries its b2a twin and the directions (a shared second-source weight without w2_alt)
+    auto paired = [&](PW a, const PW& b) {
+      if (!sel) return a;
+      a.w_alt = b.w; a.bias_alt = b.bias; a.dir = P.dir;
+      return a;
+    };
     // Ho = ceil(H / stride): Engine::conv pads an odd map to even before a stride-2 conv
     const int Ho = d->up2x ? 2 * d->H : (d->H + stride - 1) / stride, Wo = d->up2x ? 2 * d->W : (d->W + stride - 1) / stride;
     Act xin = view(d->x, d->N, d->H, d->W, d->Cin, d->ldx);
@@ -392,13 +454,15 @@ int i2it_op_conv2d_ex(i2it_handle* h, const i2it_conv_desc* d, void* stream) {
     Act x2 = view(d->x2, d->N, Ho, Wo, d->C2, d->ld2);
     PW pw2;
     if (d->x2) pw2 = E.prep("__op.conv2", {"__op.conv2"});
+    if (d->x2 && sel && sel->w2) pw2 = paired(pw2, E.prep("__op.conv2b", {"__op.conv2b"}));
     Act y;
     if (d->up2x) {
-      const PW pw = E.prep_subpixel("__op.conv");
+      const PW pw = paired(E.prep_subpixel("__op.conv"), sel ? E.prep_subpixel("__op.convb") : PW());
       y = E.conv_up2x(P, xin, pw, d->x2 ? &x2 : nullptr, d->x2 ? &pw2 : nullptr, d->gn_y != nullptr);
       E.copy_channels(P, y, ov);
     } else {
-      const PW pw = E.prep("__op.conv", {"__op.conv"}, d->act == TG_ACT_GEGLU);
+      const PW pw = paired(E.prep("__op.conv", {"__op.conv"}, d->act == TG_ACT_GEGLU),
+                           sel ? E.prep("__op.convb", {"__op.convb"}, d->act == TG_ACT_GEGLU) : PW());
       ConvOpts o;
       o.ksize = k; o.stride = stride; o.asym = d->asym_pad != 0; o.act = d->act; o.out_fp32 = d->out_fp32 != 0;
       o.gn_out = d->gn_y != nullptr;
@@ -420,6 +484,14 @@ int i2it_op_conv2d_ex(i2it_handle* h, const i2it_conv_desc* d, void* stream) {
     run_plan(h, P, static_cast<cudaStream_t>(stream));
   }
   API_END
+}
+
+int i2it_op_conv2d_ex(i2it_handle* h, const i2it_conv_desc* d, void* stream) { return op_conv(h, d, nullptr, stream); }
+
+int i2it_op_conv2d_sel(i2it_handle* h, const i2it_conv_desc* d, const float* w_alt, const float* bias_alt, const float* w2_alt,
+                       const int* directions, void* stream) {
+  const OpSel sel{w_alt, bias_alt, w2_alt, directions};
+  return op_conv(h, d, &sel, stream);
 }
 
 int i2it_op_conv2d(i2it_handle* h, const void* x, int N, int H, int W, int Cin, int ldx, const float* w,

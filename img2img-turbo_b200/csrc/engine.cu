@@ -239,6 +239,17 @@ template <typename T> static TgKernel<T> tapgemm_for(bool lean, int bn) {   // n
 #undef TG_CASE_FULL
   return nullptr;
 }
+template <typename T> using TgSelKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TapGemmParams,
+                                                   CUtensorMap, CUtensorMap, TapGemmSel);
+template <typename T> static TgSelKernel<T> tapgemm_sel_for(bool lean, int bn) {   // the same widths as tapgemm_for
+#define TG_CASE_LEAN(n) if (lean && bn == n) return tapgemm_sel_kernel<T, true, n>;
+#define TG_CASE_FULL(n) if (!lean && bn == n) return tapgemm_sel_kernel<T, false, n>;
+  TG_BN_LEAN(TG_CASE_LEAN)
+  TG_BN_FULL(TG_CASE_FULL)
+#undef TG_CASE_LEAN
+#undef TG_CASE_FULL
+  return nullptr;
+}
 
 Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CHECK(c.dtype == DT_F16 || c.dtype == DT_BF16, "dtype must be I2IT_F16 or I2IT_BF16");
@@ -252,6 +263,9 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
     for (int bn = 16; bn <= 256; bn += 16) {
       if (auto k = tapgemm_for<__half>(lean, bn)) I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
       if (auto k = tapgemm_for<__nv_bfloat16>(lean, bn))
+        I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
+      if (auto k = tapgemm_sel_for<__half>(lean, bn)) I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
+      if (auto k = tapgemm_sel_for<__nv_bfloat16>(lean, bn))
         I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
     }
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
@@ -281,6 +295,7 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CUDA(cudaEventCreateWithFlags(&ev_in_, cudaEventDisableTiming));
   I2IT_CUDA(cudaEventCreateWithFlags(&ev_out_, cudaEventDisableTiming));
   I2IT_CUDA(cudaEventCreateWithFlags(&rs_ev_, cudaEventDisableTiming));
+  I2IT_CUDA(cudaEventCreateWithFlags(&dir_ev_, cudaEventDisableTiming));
   encode_fn();
   arena_.device = c.device;
 }
@@ -301,6 +316,8 @@ Engine::~Engine() {
   if (ev_out_) cudaEventDestroy(ev_out_);
   if (rs_ev_) cudaEventDestroy(rs_ev_);
   if (rs_blob_) cudaFreeHost(rs_blob_);
+  if (dir_ev_) cudaEventDestroy(dir_ev_);
+  if (dir_blob_) cudaFreeHost(dir_blob_);
 }
 
 void Engine::check_device_error() {
@@ -716,8 +733,32 @@ void Engine::flush_prep() {
   }
 }
 
+// Mixed-direction plans: a vae. weight is prepared (through its usual cache key) together with its vae_b2a. twin, and the
+// pair goes to the launch, which selects per image.  While the twins are prepared the pairing is paused.
+static bool is_a2b_vae(const std::string& key) { return key.compare(0, 4, "vae.") == 0; }
+static std::string b2a_key(const std::string& key) { return is_a2b_vae(key) ? "vae_b2a." + key.substr(4) : key; }
+struct MixedPause {
+  const int*& slot;
+  const int* dir;
+  explicit MixedPause(const int*& s) : slot(s), dir(s) { slot = nullptr; }
+  ~MixedPause() { slot = dir; }
+};
+static PW pair_pw(PW a, const PW& b, const int* dir, const std::string& key) {
+  I2IT_CHECK(a.rows == b.rows && a.cin == b.cin && a.cin_pad == b.cin_pad && a.taps == b.taps && !a.bias == !b.bias,
+             "mixed-direction plan: " + key + " and its vae_b2a twin differ in shape");
+  a.w_alt = b.w; a.bias_alt = b.bias; a.dir = dir;
+  return a;
+}
+
 PW Engine::prep(const std::string& cache_key, const std::vector<std::string>& names, bool geglu, bool skip_scale,
                 const std::string& bias_add) {
+  if (mixed_dir_ && is_a2b_vae(cache_key)) {
+    MixedPause pause(mixed_dir_);
+    std::vector<std::string> nb;
+    for (const auto& n : names) nb.push_back(b2a_key(n));
+    const PW a = prep(cache_key, names, geglu, skip_scale, bias_add);
+    return pair_pw(a, prep(b2a_key(cache_key), nb, geglu, skip_scale, b2a_key(bias_add)), pause.dir, cache_key);
+  }
   auto it = prepared_.find(cache_key);
   if (it != prepared_.end()) return it->second;
   I2IT_CHECK(finalized_, "i2it_finalize_weights must be called before a forward");
@@ -789,6 +830,11 @@ PW Engine::prep_twin(const std::string& pre, const std::string& cur) {
 }
 
 PW Engine::prep_im2col3(const std::string& name) {
+  if (mixed_dir_ && is_a2b_vae(name)) {
+    MixedPause pause(mixed_dir_);
+    const PW a = prep_im2col3(name);
+    return pair_pw(a, prep_im2col3(b2a_key(name)), pause.dir, name);
+  }
   const std::string key = name + "|im2col";
   auto it = prepared_.find(key);
   if (it != prepared_.end()) return it->second;
@@ -829,6 +875,11 @@ PW Engine::prep_identity(int n) {
 }
 
 PW Engine::prep_subpixel(const std::string& name) {
+  if (mixed_dir_ && is_a2b_vae(name)) {
+    MixedPause pause(mixed_dir_);
+    const PW a = prep_subpixel(name);
+    return pair_pw(a, prep_subpixel(b2a_key(name)), pause.dir, name);
+  }
   const std::string key = name + "|subpixel";
   auto it = prepared_.find(key);
   if (it != prepared_.end()) return it->second;
@@ -874,6 +925,13 @@ NormW Engine::norm(const std::string& name) {
   n.g = g.d;
   n.b = raw(name, "bias").d;
   n.C = static_cast<int>(g.numel);
+  if (mixed_dir_ && is_a2b_vae(name)) {
+    const WT& g2 = raw(b2a_key(name), "weight");
+    I2IT_CHECK(g2.numel == g.numel, "mixed-direction plan: " + name + " and its vae_b2a twin differ in shape");
+    n.g_alt = g2.d;
+    n.b_alt = raw(b2a_key(name), "bias").d;
+    n.dir = mixed_dir_;
+  }
   return n;
 }
 
@@ -1005,8 +1063,16 @@ bool Engine::tma_eligible(const TapGemmParams& p, bool out_from_io) const {
 
 static void fill_strides(TmapSpec& s);
 
+void conv_box(bool stride1, int Ho, int Wo, bool nchw, int& tw, int& th, int& tn) {
+  if (stride1) tw = (Ho == 1) ? std::min(128, pow2ceil(Wo)) : std::min(nchw ? 32 : 16, pow2ceil(Wo));
+  else tw = std::min(16, pow2ceil(Wo));
+  th = std::min(128 / tw, pow2ceil(Ho));
+  tn = 128 / (tw * th);
+}
+
 void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemmParams& p_in, bool out_from_io,
-                         const char* kind, double k_valid, double bytes, const TmapSpec* sa2p, const TmapSpec* sb2p) {
+                         const char* kind, double k_valid, double bytes, const TmapSpec* sa2p, const TmapSpec* sb2p,
+                         const SelSpec* sel) {
   TapGemmParams p = p_in;
   for (int t = 0; t < p.num_taps; ++t)
     if (p.tap_kc[t] == 0) p.tap_kc[t] = p.kchunks;          // single-source callers only set kchunks
@@ -1049,9 +1115,9 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
   }
   const bool lean = use_lean && p.tma_out && p.act == TG_ACT_NONE;      // the epilogue variant without activation / direct-store code
   char shp[168];
-  snprintf(shp, sizeof shp, "M=%.0f N=%d K=%.0f taps=%d BN=%d tiles=%lld grid=%d st=%d%s%s%s", m_valid, p.N, k_valid, p.num_taps,
+  snprintf(shp, sizeof shp, "M=%.0f N=%d K=%.0f taps=%d BN=%d tiles=%lld grid=%d st=%d%s%s%s%s", m_valid, p.N, k_valid, p.num_taps,
            p.BN, total_tiles, grid, p.stages, p.tma_out ? (p.ostg2 ? " tma2" : " tma") : "",
-           (p.gn_part && p.tma_out) ? " gn" : "", lean ? " lean" : "");
+           (p.gn_part && p.tma_out) ? " gn" : "", lean ? " lean" : "", sel ? " sel" : "");
   // TMA-store epilogue: the output tensor map has the tile's row dims (extents = logical extents, so ragged edges are clipped
   // by the hardware) and a box of 64 columns x the 32 rows one epilogue warp owns
   if (!p.tma_out) p.gn_part = nullptr;
@@ -1088,6 +1154,23 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
     while ((1 << p.gn_shift) < p.gn_red) ++p.gn_shift;
   }
   I2IT_CHECK(tapgemm_for<__half>(lean, p.BN) != nullptr, "tapgemm: no kernel instantiated for BN=" + std::to_string(p.BN));
+  if (sel) {
+    // the alternative maps have the geometry (and boxes) of the ones they replace; only the base differs
+    I2IT_CHECK(p.ksplit <= 1, "tapgemm: a selecting launch cannot split K");
+    I2IT_CHECK(sel->s.dir && (sel->s.dim == 0 || sel->s.dim == 2 || sel->s.dim == 3) && sel->s.div >= 1 &&
+               (!sel->s.bias == !p.bias), "tapgemm: bad selecting launch");
+    const CUtensorMap tx = encode_tmap(sel->x, dtype), tx2 = sb2p ? encode_tmap(sel->x2, dtype) : tx;
+    TapGemmSel s = sel->s;
+    s.magic = make_magic(static_cast<long long>(p.tdim[s.dim]) + 1, s.div);
+    I2IT_CHECK(s.magic != 0, "tapgemm: tile space too large for the division-free image decode");
+    add_op(P, [ta, tb, ta2, tb2, to, p, grid, dt, out_from_io, plan, lean, tx, tx2, s](cudaStream_t st) {
+      TapGemmParams q = p;
+      if (out_from_io) q.out = plan->io.out;
+      DISPATCH_T(dt, (launch_k(tapgemm_sel_for<T>(lean, q.BN), dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q,
+                               tx, tx2, s)));
+    }, kind, 2.0 * m_valid * p.N * k_valid, bytes, shp);
+    return;
+  }
   add_op(P, [ta, tb, ta2, tb2, to, p, grid, dt, out_from_io, plan, lean](cudaStream_t st) {
     TapGemmParams q = p;
     if (out_from_io) q.out = plan->io.out;
@@ -1145,9 +1228,7 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
   int tw, th, tn;
   const long long ldo = o.to_io_out_nchw ? 0 : out.ld;
   if (o.stride == 1) {
-    tw = (x.H == 1) ? std::min(128, pow2ceil(x.W)) : std::min(o.to_io_out_nchw ? 32 : 16, pow2ceil(x.W));
-    th = std::min(128 / tw, pow2ceil(x.H));
-    tn = 128 / (tw * th);
+    conv_box(true, x.H, x.W, o.to_io_out_nchw, tw, th, tn);
     sa.base = x.p;
     sa.dim[0] = x.C; sa.dim[1] = x.W; sa.dim[2] = x.H; sa.dim[3] = x.N; sa.dim[4] = 1;
     sa.stride[0] = x.ld * 2ull; sa.stride[1] = 2ull * x.W * x.ld; sa.stride[2] = 2ull * x.H * x.W * x.ld;
@@ -1183,9 +1264,7 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
   } else {
     I2IT_CHECK(o.stride == 2 && k == 3, "conv: only 3x3 stride-2 is on the path");
     I2IT_CHECK(x.ld % 8 == 0 && x.C % 64 == 0 && x.H % 2 == 0 && x.W % 2 == 0, "conv s2: needs NHWC with ld%8==0, C%64==0, even H/W");
-    tw = std::min(16, pow2ceil(Wo));
-    th = std::min(128 / tw, pow2ceil(Ho));
-    tn = 128 / (tw * th);
+    conv_box(false, Ho, Wo, false, tw, th, tn);
     const unsigned long long C = x.C, LD = x.ld;
     // 5-D view (px*ld + c, xo, py, yo, n) of the NHWC input (pixel pitch ld >= C: the input may be a channel slice of a concat
     // buffer): a stride-2 tap is a plain box in this view.  dim 0 spans the C channels of the even pixel, the gap, and the C
@@ -1353,12 +1432,30 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
     p.num_taps = taps + 1;
     k2 = o.x2_identity ? 0 : o.w2->cin;
   }
+  SelSpec sel{};
+  if (w.dir) {
+    // mixed-direction plan: each tile takes its image's weight set, so no tile may hold rows of two images
+    const std::string why = " would hold rows of two images (mixed-direction forwards need one image per tile)";
+    sel.x = sb; sel.x.base = w.w_alt;
+    sel.s.dir = w.dir; sel.s.bias = (p.bias_mode == TG_BIAS_NONE) ? nullptr : w.bias_alt; sel.s.div = 1;
+    if (p.bias_mode == TG_BIAS_NONE) p.bias = nullptr;
+    if (o.gn_rows_per_image > 0) {                 // flattened token rows: image = 128-row tile / (tiles per image)
+      I2IT_CHECK(o.gn_rows_per_image % 128 == 0 && tw == 128 && x.rows() % o.gn_rows_per_image == 0,
+                 "conv: a token tile of " + std::to_string(o.gn_rows_per_image) + " rows per image" + why);
+      sel.s.dim = 0; sel.s.div = static_cast<int>(o.gn_rows_per_image / 128);
+    } else {
+      I2IT_CHECK(tn == 1, "conv: a " + std::to_string(x.H) + "x" + std::to_string(x.W) + " tile box" + why);
+      sel.s.dim = (o.stride == 1) ? 2 : 3;
+    }
+    if (o.x2) { sel.x2 = sb2; if (o.w2->w_alt) sel.x2.base = o.w2->w_alt; }   // an identity second source is shared
+  }
   {
     const double m_valid = 1.0 * x.N * Ho * Wo, k_valid = 1.0 * taps * w.cin + k2;
     const double bytes = 2.0 * (1.0 * x.N * x.H * x.W * w.cin + m_valid * outc * (o.out_fp32 ? 2 : 1) + 1.0 * gemm_n * k_valid +
                                 (o.res ? m_valid * outc : 0) + m_valid * k2);
     const char* kind = sub ? "tapgemm:conv_up2x" : (k == 3) ? (o.stride == 2 ? "tapgemm:conv3x3s2" : "tapgemm:conv3x3") : "tapgemm:linear";
-    launch_gemm(P, sa, sb, p, o.to_io_out_nchw, kind, k_valid, bytes, o.x2 ? &sa2 : nullptr, o.x2 ? &sb2 : nullptr);
+    launch_gemm(P, sa, sb, p, o.to_io_out_nchw, kind, k_valid, bytes, o.x2 ? &sa2 : nullptr, o.x2 ? &sb2 : nullptr,
+                w.dir ? &sel : nullptr);
   }
   if (splitk) {
     const float* part = static_cast<const float*>(sk_hold.get());
@@ -1444,6 +1541,17 @@ Act Engine::group_norm(Plan& P, const Act& x, const NormW& nw, float eps, bool s
       DISPATCH_T(dt, (launch_k(gn_stats_kernel<T>, dim3(schunks, N), dim3(threads), static_cast<size_t>(rows) * 2 * C * sizeof(float), st, 0,
                                reinterpret_cast<const T*>(xp), ximg, ldx, C, HW, cg, spix, d_part, d_counter, inv_count, eps, d_stats)));
     }, "gn_stats", 0, 2.0 * N * HW * C);
+  }
+  if (nw.dir) {   // mixed-direction plan: image n takes its direction's gamma / beta
+    const int* dir = nw.dir;
+    const float* g2 = nw.g_alt;
+    const float* b2 = nw.b_alt;
+    add_op(P, [=](cudaStream_t st) {
+      DISPATCH_T(dt, (launch_k(gn_apply_sel_kernel<T>, dim3(chunks, N), dim3(threads), 0, st, 0,
+                         reinterpret_cast<const T*>(xp), ximg, ldx, reinterpret_cast<T*>(yp), yimg, ldy, C, HW, cg, pix,
+                         d_stats, g, b, isilu, dir, g2, b2)));
+    }, "gn_apply_sel", 0, 4.0 * N * HW * C);
+    return y;
   }
   add_op(P, [=](cudaStream_t st) {
     DISPATCH_T(dt, (launch_k(gn_apply_kernel<T>, dim3(chunks, N), dim3(threads), 0, st, 0,
@@ -1565,8 +1673,14 @@ Act Engine::vt_proj(Plan& P, const Act& x, int B, int ntok, const PW& wv) {
   p.bias_mode = wv.bias ? TG_BIAS_ROW : TG_BIAS_NONE;
   p.alpha = 1.f;
   p.err = d_err;
+  SelSpec sel{};
+  if (wv.dir) {   // mixed-direction plan: the weight is the row operand, so the selection takes A and the row bias; t[2] = image
+    sel.x = sa; sel.x.base = wv.w_alt;
+    sel.s.dir = wv.dir; sel.s.bias = wv.bias_alt; sel.s.dim = 2; sel.s.div = 1; sel.s.sel_a = 1;
+  }
   launch_gemm(P, sa, sb, p, false, "tapgemm:vt",
-              wv.cin, 2.0 * (1.0 * C * wv.cin + 1.0 * B * ntok * wv.cin + 1.0 * B * C * ntok));
+              wv.cin, 2.0 * (1.0 * C * wv.cin + 1.0 * B * ntok * wv.cin + 1.0 * B * C * ntok), nullptr, nullptr,
+              wv.dir ? &sel : nullptr);
   return vt;
 }
 
@@ -1890,7 +2004,8 @@ void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int te
 }
 
 void Engine::forward_ragged(const IO& io_in, const void* const* x, void* const* out, const i2it_resize_desc* g, int max_side,
-                            int B, int H, int W, int direction, int text_batch, cudaStream_t st) {
+                            int B, int H, int W, int direction, int text_batch, cudaStream_t st, const int* dirs) {
+  if (dirs) { check_mixed(dirs, B, H, W); direction = DIR_MIXED; }
   const bool text_cached = check_forward(B, H, W, text_batch, io_in.text);
   I2IT_CHECK(x && out && g, "ragged forward: null image or geometry array");
   rs_check_ragged(g, B, H, W, max_side);      // before the pointers: an empty output (a zero size) has a null one
@@ -1914,10 +2029,76 @@ void Engine::forward_ragged(const IO& io_in, const void* const* x, void* const* 
   const size_t bytes = stage_ragged(c, P->rg.dev_bytes);
   char* dev = P->rg.dev;
   const char* blob = rs_blob_;
+  const std::function<void(cudaStream_t)> dir_copy = dirs ? stage_dirs(P, dirs, B) : nullptr;
   run(P, io, st, [=](cudaStream_t s) {
     I2IT_CUDA(cudaMemcpyAsync(dev, blob, bytes, cudaMemcpyHostToDevice, s));
     I2IT_CUDA(cudaEventRecord(rs_ev_, s));
+    if (dir_copy) dir_copy(s);
   });
+}
+
+std::string mixed_size_rule(int H, int W) {
+  const std::string hw = std::to_string(H) + "x" + std::to_string(W);
+  if (H <= 0 || W <= 0 || H % 8 || W % 8) return "H and W must be positive multiples of 8";
+  const long long tok = 1ll * (H / 8) * (W / 8);
+  if (tok % 128 != 0)
+    return hw + " is refused: the VAE attention's token launches need (H/8)*(W/8) = " + std::to_string(tok) +
+           " latent pixels per image to be a multiple of 128, so that no 128-row tile holds rows of two images";
+  // the VAE's convs: stride 1 on every level H/2^k x W/2^k (k = 0..3; the final image's launch on level 0), stride 2 into
+  // levels 1..3.  The box shrinks with the map, but every level is checked as the picker sees it.
+  for (int k = 0; k < 4; ++k) {
+    const int h = H >> k, w = W >> k;
+    int tw, th, tn;
+    const bool kinds[3][2] = {{true, false}, {true, k == 0}, {false, false}};
+    for (int i = 0; i < 3; ++i) {
+      if (i == 2 && k == 0) continue;       // no stride-2 conv writes level 0
+      conv_box(kinds[i][0], h, w, kinds[i][1], tw, th, tn);
+      if (tn != 1)
+        return hw + " is refused: a VAE conv on its " + std::to_string(h) + "x" + std::to_string(w) + " map has a " +
+               std::to_string(tw) + "x" + std::to_string(th) + "-pixel tile box that spans " + std::to_string(tn) +
+               " images (one image per 128-row tile needs the box to fill 128 pixels of one image)";
+    }
+  }
+  return "";
+}
+
+void Engine::check_mixed(const int* dirs, int B, int H, int W) const {
+  I2IT_CHECK(cfg.model_kind == I2IT_CYCLEGAN, "mixed-direction forward: a pix2pix handle has one VAE; directions are CycleGAN's");
+  I2IT_CHECK(dirs != nullptr, "mixed-direction forward: null direction array");
+  I2IT_CHECK(B >= 1, "mixed-direction forward: batch must be >= 1");
+  for (int i = 0; i < B; ++i)
+    I2IT_CHECK(dirs[i] == I2IT_A2B || dirs[i] == I2IT_B2A, "mixed-direction forward: direction " + std::to_string(dirs[i]) +
+                                                                " of image " + std::to_string(i) + " is neither I2IT_A2B (0) nor I2IT_B2A (1)");
+  const std::string why = mixed_size_rule(H, W);
+  I2IT_CHECK(why.empty(), "mixed-direction forward: " + why);
+}
+
+std::function<void(cudaStream_t)> Engine::stage_dirs(Plan* P, const int* dirs, int B) {
+  I2IT_CHECK(P->dir != nullptr, "mixed-direction forward: the plan has no direction array");
+  I2IT_CUDA(cudaEventSynchronize(dir_ev_));     // the previous call's copy has read the blob
+  if (B > dir_blob_cap_) {
+    if (dir_blob_) I2IT_CUDA(cudaFreeHost(dir_blob_));
+    dir_blob_ = nullptr;
+    dir_blob_cap_ = 0;
+    I2IT_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&dir_blob_), static_cast<size_t>(B) * sizeof(int), cudaHostAllocDefault));
+    dir_blob_cap_ = B;
+  }
+  std::memcpy(dir_blob_, dirs, static_cast<size_t>(B) * sizeof(int));
+  int* dev = P->dir;
+  const int* blob = dir_blob_;
+  cudaEvent_t ev = dir_ev_;
+  return [=](cudaStream_t s) {
+    I2IT_CUDA(cudaMemcpyAsync(dev, blob, static_cast<size_t>(B) * sizeof(int), cudaMemcpyHostToDevice, s));
+    I2IT_CUDA(cudaEventRecord(ev, s));
+  };
+}
+
+void Engine::forward_mixed(const IO& io, const int* dirs, int B, int H, int W, int text_batch, cudaStream_t st) {
+  check_mixed(dirs, B, H, W);
+  const bool text_cached = check_forward(B, H, W, text_batch, io.text);
+  I2IT_CHECK(io.x && io.eps && io.out, "null input/output pointer");
+  Plan* P = plan_for(B, H, W, DIR_MIXED, text_batch, text_cached, 0, nullptr, /*evict=*/false);
+  run(P, io, st, stage_dirs(P, dirs, B));
 }
 
 size_t Engine::stage_ragged(const RsCall& c, size_t cap) {

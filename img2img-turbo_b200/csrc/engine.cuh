@@ -95,6 +95,10 @@ struct PW {                        // prepared (folded, re-laid-out) weight: [ta
   uint16_t* w = nullptr;
   float* bias = nullptr;
   int rows = 0, cin = 0, cin_pad = 0, taps = 1;
+  // a mixed-direction plan's VAE weight: the b2a twin (same shape), taken by the images whose dir[] entry is 1
+  uint16_t* w_alt = nullptr;
+  float* bias_alt = nullptr;
+  const int* dir = nullptr;        // non-null: the launches that use this weight select per image
 };
 // ---- kernel launch for plan ops: programmatic dependent launch (see pdl_sync in common.cuh) when the previous op of the
 // plan was also a kernel; `cluster` > 0 adds a (cluster,1,1) cluster dimension.  Executor state, one engine call per thread.
@@ -122,7 +126,10 @@ inline void launch_k(void (*kern)(KA...), dim3 grid, dim3 block, size_t smem, cu
   g_pdl.prev_is_kernel = true;
 }
 
-struct NormW { const float* g = nullptr; const float* b = nullptr; int C = 0; };
+struct NormW {
+  const float* g = nullptr; const float* b = nullptr; int C = 0;
+  const float* g_alt = nullptr; const float* b_alt = nullptr; const int* dir = nullptr;   // as PW's alternative set
+};
 
 struct IO {
   const void* x = nullptr; const void* text = nullptr; const void* eps = nullptr; const void* noise = nullptr;
@@ -135,6 +142,10 @@ struct IO {
 // IO_SHARED_IN: a variations forward, one input image for the whole batch (its encoder runs at batch 1)
 // IO_RAGGED: uint8 images of their own sizes, each resized to and from the one network size (i2it_forward_u8_ragged)
 enum IoMode : int { IO_U8_IN = 1, IO_U8_OUT = 2, IO_SHARED_IN = 4, IO_RAGGED = 8 };
+// the plan-key direction of a mixed-direction CycleGAN plan (I2IT_A2B = 0 and I2IT_B2A = 1 are the single-direction ones)
+constexpr int DIR_MIXED = 2;
+// the 128-row tile box (tw x th pixels of tn images) Engine::conv picks for an Ho x Wo output; nchw: the final image's launch
+void conv_box(bool stride1, int Ho, int Wo, bool nchw, int& tw, int& th, int& tn);
 
 // uint8 HWC images [B][img bytes][w pixels per row][3] an op reads or writes: a caller pointer read from the plan's IO at
 // launch time (slot), or a plan-internal buffer (p); off selects a window's first pixel
@@ -160,6 +171,11 @@ struct RaggedBufs {
   size_t ops[4] = {0, 0, 0, 0};    // plan indices of the input side's h / v and the output side's h / v launches
   const int* tab() const { return reinterpret_cast<const int*>(dev + descs * sizeof(RsPass)); }
 };
+
+// The sizes a mixed-direction forward accepts: every tile of every VAE launch must hold rows of one image (conv boxes of one
+// image: Engine::conv's box picker gives tn == 1; the attention's token launches: (H/8)(W/8) a multiple of 128).  Returns
+// "" when H x W is accepted, else the reason.  Host only.
+std::string mixed_size_rule(int H, int W);
 
 // descriptors and tables of one ragged call, built on the host; bytes: algorithmic bytes of the four launches
 struct RsCall {
@@ -200,6 +216,7 @@ struct Plan {
   std::vector<std::pair<size_t, const char*>> ranges;  // (first op index, name): NVTX stage ranges of the eager path
   bool debug_tapgemm = false;                          // a diagnostic op plan: its tapgemm launches take the engine's dbg_* override
   RaggedBufs rg;                                       // IO_RAGGED plans and ragged resize ops
+  int* dir = nullptr;                                  // mixed-direction plans: [B] directions, written before every run
   IO io;
   std::vector<std::pair<IO, cudaGraphExec_t>> graphs;  // small cache: one instantiated graph per distinct IO pointer set
   ~Plan() { for (auto& g : graphs) cudaGraphExecDestroy(g.second); }
@@ -278,7 +295,12 @@ class Engine {
                const i2it_resize_desc* g = nullptr, bool shared_input = false);
   // B images of their own sizes (x[i], out[i], g[i]) through one IO_RAGGED plan of capacity max_side on an H x W network
   void forward_ragged(const IO& io, const void* const* x, void* const* out, const i2it_resize_desc* g, int max_side, int B,
-                      int H, int W, int direction, int text_batch, cudaStream_t st);
+                      int H, int W, int direction, int text_batch, cudaStream_t st, const int* dirs = nullptr);
+  // mixed-direction CycleGAN forward: image i through vae (dirs[i] == I2IT_A2B) or vae_b2a (I2IT_B2A), one plan for every mix
+  void forward_mixed(const IO& io, const int* dirs, int B, int H, int W, int text_batch, cudaStream_t st);
+  // rejects, with a message, what a mixed forward refuses before building anything: a pix2pix handle, a direction array
+  // that is null or holds a value other than 0 / 1, and a size whose VAE tiles would hold rows of two images
+  void check_mixed(const int* dirs, int B, int H, int W) const;
   // the checks every image forward starts with (network size, text batch, a cached text when text is null); returns
   // whether the text is the cached one
   bool check_forward(int B, int H, int W, int text_batch, const void* text) const;
@@ -386,8 +408,12 @@ class Engine {
     P.meta.push_back(m);
   }
   // encodes the tensor maps and appends the launch
+  // sel: a selecting launch (tapgemm_sel_kernel); x / x2 are the alternative maps of B and the second source's B (of A when
+  // sel->sel_a), and sel's dir / bias / dim / div are set by the caller
+  struct SelSpec { TmapSpec x, x2; TapGemmSel s; };
   void launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemmParams& p, bool out_from_io, const char* kind,
-                   double k_valid, double bytes, const TmapSpec* sa2 = nullptr, const TmapSpec* sb2 = nullptr);
+                   double k_valid, double bytes, const TmapSpec* sa2 = nullptr, const TmapSpec* sb2 = nullptr,
+                   const SelSpec* sel = nullptr);
   bool use_idres = true, use_pdl = false, trace_on = false, use_tmaout = true, use_gnepi = true, use_splitk = true, use_catfuse = true, use_ostg2 = true, use_lean = true, sync_each = false;
   bool tma_eligible(const TapGemmParams& p, bool out_from_io) const;
   std::string profile_json(int reps, cudaStream_t st);
@@ -462,6 +488,14 @@ class Engine {
   size_t rs_blob_cap_ = 0;
   cudaEvent_t rs_ev_ = nullptr;
   size_t stage_ragged(const RsCall& c, size_t cap);     // fills the blob; returns its byte count
+  // mixed-direction forwards: the pinned copy of the call's directions one async copy moves into Plan::dir (dir_ev_ says
+  // the previous copy has read it); mixed_dir_ is the plan's array while a mixed plan is being built (prep / norm pair the
+  // vae. weights with their vae_b2a. twins then)
+  int* dir_blob_ = nullptr;
+  int dir_blob_cap_ = 0;
+  cudaEvent_t dir_ev_ = nullptr;
+  const int* mixed_dir_ = nullptr;
+  std::function<void(cudaStream_t)> stage_dirs(Plan* P, const int* dirs, int B);
   Plan* last_plan_ = nullptr;
   Plan* last_text_plan_ = nullptr;   // the plan of the last encode_text (its stages: i2it_text_stage_names)
   Act text_;                     // staged text embedding while a UNet plan is being built

@@ -167,15 +167,21 @@ static __global__ void gn_part_reduce_kernel(const float* __restrict__ part, int
   if (t == 0) counter[n] = 0;
 }
 
-template <typename T>
-__global__ void gn_apply_kernel(const T* __restrict__ x, long long ximg, int ldx, T* __restrict__ y, long long yimg,
-                                int ldy, int C, int HW, int cg, int pix_per_cta, const float* __restrict__ stats,
-                                const float* __restrict__ gamma, const float* __restrict__ beta, int silu) {
+// SEL: gamma / beta of image n are (gamma2, beta2) where dir[n] != 0 (gn_apply_sel_kernel); the arithmetic is the same
+template <typename T, bool SEL>
+__device__ __forceinline__ void gn_apply_body(const T* __restrict__ x, long long ximg, int ldx, T* __restrict__ y, long long yimg,
+                                              int ldy, int C, int HW, int cg, int pix_per_cta, const float* __restrict__ stats,
+                                              const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
+                                              const int* __restrict__ dir, const float* __restrict__ gamma2,
+                                              const float* __restrict__ beta2) {
   pdl_sync();
   const int vecs = C >> 3;
   const int vx = threadIdx.x % vecs, vy = threadIdx.x / vecs, rows = blockDim.x / vecs;
   const int n = blockIdx.y;
   if (vy >= rows) return;
+  if constexpr (SEL) {
+    if (dir[n]) { gamma = gamma2; beta = beta2; }
+  }
   float sc[8], sh[8];
   int gprev = -1;
   float mean = 0.f, rstd = 0.f;
@@ -217,6 +223,22 @@ __global__ void gn_apply_kernel(const T* __restrict__ x, long long ximg, int ldx
     st16(yb + static_cast<long long>(p + 3 * rows) * ldy, xf(u3));
   }
   for (; p < p1; p += rows) st16(yb + static_cast<long long>(p) * ldy, xf(ld_nc16(xb + static_cast<long long>(p) * ldx)));
+}
+
+template <typename T>
+__global__ void gn_apply_kernel(const T* __restrict__ x, long long ximg, int ldx, T* __restrict__ y, long long yimg,
+                                int ldy, int C, int HW, int cg, int pix_per_cta, const float* __restrict__ stats,
+                                const float* __restrict__ gamma, const float* __restrict__ beta, int silu) {
+  gn_apply_body<T, false>(x, ximg, ldx, y, yimg, ldy, C, HW, cg, pix_per_cta, stats, gamma, beta, silu, nullptr, nullptr, nullptr);
+}
+
+// GroupNorm apply of a mixed-direction batch: image n takes (gamma2, beta2) where dir[n] != 0, else (gamma, beta)
+template <typename T>
+__global__ void gn_apply_sel_kernel(const T* __restrict__ x, long long ximg, int ldx, T* __restrict__ y, long long yimg,
+                                    int ldy, int C, int HW, int cg, int pix_per_cta, const float* __restrict__ stats,
+                                    const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
+                                    const int* __restrict__ dir, const float* __restrict__ gamma2, const float* __restrict__ beta2) {
+  gn_apply_body<T, true>(x, ximg, ldx, y, yimg, ldy, C, HW, cg, pix_per_cta, stats, gamma, beta, silu, dir, gamma2, beta2);
 }
 
 // =============================================================================================

@@ -591,9 +591,26 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
   I2IT_CHECK(finalized_, "i2it_finalize_weights must be called before a forward");
   std::string vp = "vae.";
   if (cfg.model_kind == I2IT_CYCLEGAN && direction == I2IT_B2A) vp = "vae_b2a.";
+  const bool mixed = direction == DIR_MIXED;
+  if (mixed) {
+    I2IT_CHECK(cfg.model_kind == I2IT_CYCLEGAN, "mixed-direction forward: a pix2pix handle has one VAE; directions are CycleGAN's");
+    const std::string why = mixed_size_rule(H, W);
+    I2IT_CHECK(why.empty(), "mixed-direction forward: " + why);
+  }
   std::unique_ptr<Plan> up(new Plan());
   Plan& P = *up;
   P.key = key;
+  // a mixed plan builds the VAE from the vae. weights paired with their vae_b2a. twins (prep / norm do the pairing while
+  // mixed_dir_ is set); its launches read the image's direction from P.dir, which every call rewrites before the first launch
+  struct MixedBuild {
+    const int*& slot;
+    ~MixedBuild() { slot = nullptr; }
+  } mixed_build{mixed_dir_};
+  if (mixed) {
+    P.dir = static_cast<int*>(P.pool.get_fresh(static_cast<size_t>(B) * sizeof(int)));
+    I2IT_CUDA(cudaMemset(P.dir, 0, static_cast<size_t>(B) * sizeof(int)));
+    mixed_dir_ = P.dir;
+  }
   P.pool.arena = &arena_;      // transient buffers alias those of the handle's other forward plans
   // a build that throws must not leave engine members pointing into the dying plan's pool (text_ holds a pool block):
   // declared after `up`, so it runs before the plan is destroyed

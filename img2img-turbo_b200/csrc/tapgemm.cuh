@@ -115,6 +115,18 @@ struct TapGemmParams {
   unsigned long long* trace;   // optional (I2IT_TRACE=1): 16 %clock64 stamps per CTA at the phase boundaries, else nullptr
 };
 
+// Operands of a selecting launch (tapgemm_sel_kernel), kept out of TapGemmParams so that no field of the plain kernels moves
+// (see layout_pad1).  Every 128-row tile belongs to one image; dir[image] picks that tile's weight set: 0 = the launch's own
+// maps and bias, 1 = the alternative maps (tmX for B, tmX2 for the second source's B; tmX for A when sel_a) and `bias`.
+struct TapGemmSel {
+  const int* dir;          // [images], 0 or 1, device memory (rewritten before each forward; the graph reads it)
+  const float* bias;       // the alternative column bias (row bias when sel_a), nullptr iff p.bias is
+  int dim;                 // the tile coordinate that holds the image: image = t[dim] / div  (dim 0, 2 or 3)
+  int div;                 // 1, or the m-tiles per image of a flattened-token launch
+  uint32_t magic;          // make_magic(., div)
+  int sel_a;               // 1: the weight is the row operand (V^T projection): the selection replaces A, not B
+};
+
 // ------------------------------------------------------------------------------------------
 // PTX wrappers
 // ------------------------------------------------------------------------------------------
@@ -440,6 +452,13 @@ __device__ __forceinline__ void stage_bias(const TapGemmParams& p, float* sb, in
   asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");   // the epilogue warps only
 }
 
+// stage_bias with the tile's bias chosen by the caller (tapgemm_sel_kernel: the bias of the tile's image's weight set)
+__device__ __forceinline__ void stage_bias_from(const TapGemmParams& p, const float* bias, float* sb, int n0, int warp) {
+  for (int cc = warp * 32 + (threadIdx.x & 31); cc < p.BN; cc += TG_EPI_WARPS * 32)
+    sb[cc] = (p.bias_mode == TG_BIAS_COL && n0 + cc < p.N) ? bias[n0 + cc] : 0.f;
+  asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
+}
+
 // TMA-store epilogue, straight from the wgmma fragments (every tma_out launch: no staging tile, so the operand ring stays with
 // the producer, which loads the next tile while this runs).  Rounds of 64 OUTPUT columns (128 accumulator columns for GEGLU)
 // go through swizzled 32 x 64 store boxes (see TG_OSTG_WARP).  The tile's 32-row quarter q = warp >> 1 comes from the two
@@ -613,9 +632,9 @@ __device__ __forceinline__ void epilogue_frag(const TapGemmParams& p, const CUte
 // Direct-store epilogue of one output tile for one thread (= one accumulator row, read from the fp32 staging tile at `arow`):
 // the launches whose output does not fit whole TMA-store rounds (fp32 logits, NCHW image, row-bias V^T, split-K partials,
 // channel counts that are not multiples of 64).  The row's warp pair takes the 32-column rounds in turn (grp = warp & 1).
-template <typename T>
+template <typename T, bool SEL = false>
 __device__ __forceinline__ void epilogue_direct(const TapGemmParams& p, const TileCoord& c, const RowCoord& rc, int warp,
-                                                uint32_t arow, const float* sb, bool stamp) {
+                                                uint32_t arow, const float* sb, bool stamp, const float* sel_bias = nullptr) {
   const int g1 = rc.g1, g2 = rc.g2, g3 = rc.g3, g4 = rc.g4;
   const bool row_ok = rc.ok;
   const long long rbase = rc.rbase;
@@ -630,7 +649,7 @@ __device__ __forceinline__ void epilogue_direct(const TapGemmParams& p, const Ti
     }
   };
   const long long obase = g1 * p.ostride[0] + g2 * p.ostride[1] + g3 * p.ostride[2] + g4 * p.ostride[3] + c.split * p.split_ostride;
-  const float rbias = (p.bias_mode == TG_BIAS_ROW && row_ok) ? p.bias[g1] : 0.0f;
+  const float rbias = (p.bias_mode == TG_BIAS_ROW && row_ok) ? (SEL ? sel_bias : p.bias)[g1] : 0.0f;
   // This thread's WHOLE residual slice (its row x the 32-column rounds r = grp, grp+2, ...; <= 256 B) is requested up front,
   // so the global loads are in flight together.
   const int nrounds = (p.BN + 31) >> 5;
@@ -673,6 +692,213 @@ __device__ __forceinline__ void epilogue_direct(const TapGemmParams& p, const Ti
   }
 }
 
+
+// the weight set of tile c of a selecting launch: 0 (the launch's own) or 1 (the alternative)
+__device__ __forceinline__ int sel_dir(const TapGemmSel& s, const TileCoord& c) {
+  const int v = s.dim == 0 ? c.t[0] : (s.dim == 2 ? c.t[2] : c.t[3]);
+  return s.dir[fast_div(v, s.div, s.magic)];
+}
+
+// tapgemm with a weight set chosen per tile by the tile's image (mixed-direction CycleGAN batches; see TapGemmSel).  It is
+// tapgemm_kernel's code with two changes, marked SEL: the map the producer loads each tile's weight stages from, and the
+// bias slice the epilogue stages for the tile.  The ring, the MMA chain, the accumulation order, the GroupNorm slots and
+// the stores are the same.  A copy rather than a shared body: tapgemm_kernel's code (and ptxas's register allocation of
+// it, see layout_pad1) stays exactly as it was.
+template <typename T, bool LEAN, int BN>
+__global__ void __launch_bounds__(TG_THREADS, 1)
+tapgemm_sel_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+                   const __grid_constant__ CUtensorMap tmO, const __grid_constant__ TapGemmParams p,
+                   const __grid_constant__ CUtensorMap tmXm, const __grid_constant__ CUtensorMap tmX2m,
+                   const __grid_constant__ TapGemmSel selm) {
+  constexpr bool SEL = true;
+  const CUtensorMap* const tmX = &tmXm;
+  const CUtensorMap* const tmX2 = &tmX2m;
+  const TapGemmSel* const sel = &selm;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  if (TG_ALIGN_PAD < 1024 && base - smem_u32(smem_raw) > static_cast<uint32_t>(TG_ALIGN_PAD)) {
+    if (threadIdx.x == 0 && p.err) { atomicExch(p.err, 90); __threadfence_system(); }
+    __trap();
+  }
+  const int NS = p.stages;
+  const uint32_t BST = static_cast<uint32_t>(p.b_stage);
+  const uint32_t sA = base;
+  const uint32_t sB = base + NS * TG_A_STAGE;
+  const uint32_t ostg = base + TG_STAGES * (TG_A_STAGE + TG_B_STAGE);   // epilogue store boxes (1024-byte aligned)
+  const uint32_t ostg2 = ostg - TG_OSTG_BYTES;                          // optional second set: the ring's last 32 KB (p.ostg2)
+  const uint32_t bars = ostg + TG_OSTG_BYTES;
+  auto full_bar = [&](int s) { return bars + 8u * s; };
+  auto empty_bar = [&](int s) { return bars + 8u * (TG_MAX_STAGES + s); };
+  const uint32_t epi_done = bars + 8u * (2 * TG_MAX_STAGES);
+  float* const s_bias = reinterpret_cast<float*>(smem_raw + (bars - smem_u32(smem_raw)) + TG_BAR_BYTES);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) tg_stamp(p, 0);
+  const int nsplit = p.ksplit > 1 ? p.ksplit : 1;
+  const int total_tiles = p.n_tiles * p.tdim[0] * p.tdim[1] * p.tdim[2] * p.tdim[3] * nsplit;
+  int steps = 0, sec_steps = 0;
+  for (int t = 0; t < p.num_taps; ++t) steps += p.tap_kc[t];
+  for (int t = p.nprim; t < p.num_taps; ++t) sec_steps += p.tap_kc[t];
+
+  if (warp == TG_EPI_WARPS && lane == 0) {
+    for (int s = 0; s < NS; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TG_EPI_WARPS); }
+    mbar_init(epi_done, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA2)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB2)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmO)) : "memory");
+    if constexpr (SEL) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmX)) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmX2)) : "memory");
+    }
+  }
+  __syncthreads();
+  pdl_sync();   // prologue (barriers, descriptor prefetch) overlaps the previous kernel's tail; no global access before here
+  if (threadIdx.x == 0) tg_stamp(p, 1);
+
+  // setmaxnreg inside each role's branch: issued by all warps before the role branches, both were ignored (C7507)
+  if (warp >= TG_EPI_WARPS) {
+    reg_dec<TG_REGS_PRODUCER>();
+    if (warp == TG_EPI_WARPS) {             // warps 9..11 only hand their registers to the consumers
+      // ================================ TMA producer (whole warp runs the loop, one elected lane issues) ==========
+      int stage = 0, phase = 0, iter = 0;
+      const uint32_t tx_bytes = TG_A_STAGE + static_cast<uint32_t>(p.BN) * (TG_BK * 2);
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
+        const TileCoord c = decode_tile(p, tile);
+        const int a1 = c.t[0] * p.a_mul[0], a2 = c.t[1] * p.a_mul[1], a3 = c.t[2] * p.a_mul[2],
+                  a4 = c.t[3] * p.a_mul[3];
+        const int b2 = c.t[1] * p.b_mul[0], b3 = c.t[2] * p.b_mul[1], b4 = c.t[3] * p.b_mul[2];
+        const int n0 = c.nt * p.BN;
+        // direct-store launches: the ring doubles as the previous tile's accumulator staging tile until its epilogue has read it
+        if (iter > 0 && !p.tma_out) mbar_wait(epi_done, (iter - 1) & 1, p.err, 2);
+        bool alt = false;
+        if constexpr (SEL) alt = sel_dir(*sel, c) != 0;
+        auto load_step = [&](int t, int kc) {
+          const CUtensorMap* ta = p.tap_src[t] ? &tmA2 : &tmA;
+          const CUtensorMap* tb = p.tap_src[t] ? &tmB2 : &tmB;
+          if constexpr (SEL) {
+            if (alt && sel->sel_a) ta = tmX;
+            else if (alt) tb = p.tap_src[t] ? tmX2 : tmX;
+          }
+          mbar_wait(empty_bar(stage), phase ^ 1, p.err, 1);
+          if (elect_one()) {
+            mbar_expect_tx(full_bar(stage), tx_bytes);
+            tma_load_5d(sA + stage * TG_A_STAGE, ta, full_bar(stage), kc * TG_BK + p.tap_a[t][0],
+                        a1 + p.tap_a[t][1], a2 + p.tap_a[t][2], a3 + p.tap_a[t][3], a4 + p.tap_a[t][4]);
+            tma_load_5d(sB + stage * BST, tb, full_bar(stage), kc * TG_BK + p.tap_b[t][0], n0,
+                        b2 + p.tap_b[t][1], b3 + p.tap_b[t][2], b4 + p.tap_b[t][3]);
+          }
+          __syncwarp();
+          if (++stage == NS) { stage = 0; phase ^= 1; }
+        };
+        const int kc0 = nsplit > 1 ? c.split * p.kc_per : 0, kc1 = nsplit > 1 ? min(p.kchunks, kc0 + p.kc_per) : p.kchunks;
+        for (int kc = kc0; kc < kc1; ++kc)
+          for (int t = 0; t < p.nprim; ++t) load_step(t, kc);
+        if (c.split == 0)
+          for (int t = p.nprim; t < p.num_taps; ++t)
+            for (int kc = 0; kc < p.tap_kc[t]; ++kc) load_step(t, kc);
+        if (tile == static_cast<int>(blockIdx.x) && lane == 0) tg_stamp(p, 2);   // first tile's loads all issued
+      }
+      if (lane == 0) tg_stamp(p, 3);
+    }
+  } else {
+    reg_inc<TG_REGS_CONSUMER>();
+    // ============================ consumers: wgmma mainloop + epilogue (warps 0..7) ============================
+    const int wg = warp >> 2;                    // warpgroup: tile rows [64 wg, 64 wg + 64) in the mainloop
+    const int row = 32 * (warp >> 1) + lane;     // epilogue: tile row described by this lane (quarter warp >> 1)
+    int rr = row;
+    const int j1 = rr % p.box[0]; rr /= p.box[0];
+    const int j2 = rr % p.box[1]; rr /= p.box[1];
+    const int j3 = rr % p.box[2];
+    const int j4 = rr / p.box[2];
+    constexpr int spitch = BN + 4;               // staging row pitch in floats
+    const uint32_t arow = base + static_cast<uint32_t>(row * spitch * 4);
+    // one k-step (one ring stage): four k16 MMAs of the tile's full width; the first of a tile overwrites the accumulators
+    auto mma_stage = [&](float (&accum)[BN / 2], int stage, auto first) {
+      wgmma_fence();
+      const uint32_t a0 = sA + stage * TG_A_STAGE + wg * (64 * 128), b0 = sB + stage * BST;
+#pragma unroll
+      for (int k = 0; k < TG_BK / 16; ++k) {
+        const uint64_t adesc = wgmma_desc_sw128(a0) + 2 * k, bdesc = wgmma_desc_sw128(b0) + 2 * k;
+        if (decltype(first)::value && k == 0) wgmma_ss<BN, false, T>(accum, adesc, bdesc);
+        else wgmma_ss<BN, true, T>(accum, adesc, bdesc);
+      }
+      wgmma_commit();
+    };
+    int stage = 0, phase = 0, iter = 0, rsel = 0;   // rsel: store-box rounds so far (epilogue_frag)
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
+      int tsteps = steps;
+      if (nsplit > 1) {                                                         // this tile's share of the K loop
+        const int split = tile / (total_tiles / nsplit);
+        const int kc0 = split * p.kc_per, kc1 = min(p.kchunks, kc0 + p.kc_per);
+        tsteps = (kc1 - kc0) * p.nprim + (split == 0 ? sec_steps : 0);
+      }
+      float accum[BN / 2];                         // live from the tile's first MMA to the staging store only
+      mbar_wait(full_bar(stage), phase, p.err, 3);
+      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 4);                         // first operands landed
+      mma_stage(accum, stage, std::true_type());
+      int prev = stage;
+      if (++stage == NS) { stage = 0; phase ^= 1; }
+      for (int s = 1; s < tsteps; ++s) {
+        mbar_wait(full_bar(stage), phase, p.err, 3);
+        mma_stage(accum, stage, std::false_type());
+        wgmma_wait<1>();                                   // the previous step's MMAs have read their stage
+        if (lane == 0) mbar_arrive(empty_bar(prev));
+        prev = stage;
+        if (++stage == NS) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(empty_bar(prev));
+      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 5);                        // first tile's MMAs complete
+
+      const TileCoord c = decode_tile(p, tile);
+      const RowCoord rc = row_coord(p, c, j1, j2, j3, j4);
+      float* const sb = s_bias + (iter & 1) * 256;
+      // a launch with a single n-tile stages its one slice into both buffers during the first two tiles and then skips this and
+      // its barrier (110 tiles per CTA in the 512x512 convs)
+      const float* sel_bias = nullptr;
+      if constexpr (SEL) {
+        sel_bias = sel_dir(*sel, c) ? sel->bias : p.bias;
+        stage_bias_from(p, sel_bias, sb, c.nt * BN, warp);   // every tile: the slice changes with the tile's image
+      } else if (p.n_tiles > 1 || iter < 2) {
+        stage_bias(p, sb, c.nt * BN, warp);
+      }
+      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 7);
+      if (LEAN || p.tma_out) {
+        epilogue_frag<T, LEAN, BN>(p, &tmO, c, fast_div(tile, p.n_tiles, p.magic[0]), accum, warp, rc, sb, ostg, ostg2, rsel,
+                                   iter == 0 && threadIdx.x == 0);
+      } else if constexpr (!LEAN) {
+        // accumulators -> fp32 staging tile (the producer is parked on epi_done, so no load writes the ring meanwhile); the
+        // barrier first: the other warpgroup's last MMAs may still be reading the ring stages the staging tile overlays
+        asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
+        {
+          const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+          for (int g = 0; g < BN / 8; ++g) {
+            const uint32_t a = base + static_cast<uint32_t>((r0 * spitch + 8 * g + c0) * 4);
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(accum[4 * g]), "f"(accum[4 * g + 1]) : "memory");
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a + 8 * spitch * 4), "f"(accum[4 * g + 2]),
+                         "f"(accum[4 * g + 3]) : "memory");
+          }
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
+        epilogue_direct<T, SEL>(p, c, rc, warp, arow, sb, iter == 0 && threadIdx.x == 0, sel_bias);
+        // staging tile consumed: the ring goes back to the producer (generic reads ordered before the TMA's async writes)
+        fence_async_smem();
+        asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
+        if (threadIdx.x == 0) mbar_arrive(epi_done);
+      }
+      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 9);                        // first tile stored
+    }
+    if (p.tma_out && lane == 0) bulk_wait_all();      // the store boxes live in this CTA's shared memory
+    if (threadIdx.x == 0) tg_stamp(p, 10);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) tg_stamp(p, 11);
+}
 
 template <typename T, bool LEAN, int BN>
 __global__ void __launch_bounds__(TG_THREADS, 1)

@@ -55,6 +55,36 @@ class VAE_decode(nn.Module):
         raise RuntimeError("VAE_decode is fused into libi2it; call CycleGAN_Turbo.forward / forward_with_networks")
 
 
+def direction_codes(direction, batch):
+    """The engine's direction for a forward of `batch` images: "a2b" / "b2a" -> i2it.A2B / i2it.B2A (one direction, the
+    single-direction plans), or a list of `batch` of those strings -> a list of codes (a mixed-direction forward, one plan
+    for every mix).  Raises ValueError for anything else."""
+    codes = {"a2b": i2it.A2B, "b2a": i2it.B2A}
+    if isinstance(direction, str):
+        if direction not in codes:
+            raise ValueError(f"direction must be 'a2b' or 'b2a', got {direction!r}")
+        return codes[direction]
+    if not isinstance(direction, (list, tuple)):
+        raise ValueError(f"direction must be 'a2b', 'b2a' or a list of them, got {type(direction).__name__}")
+    if len(direction) != batch:
+        raise ValueError(f"{batch} images but {len(direction)} directions")
+    for i, d in enumerate(direction):
+        if not isinstance(d, str) or d not in codes:
+            raise ValueError(f"direction {d!r} of image {i} is neither 'a2b' nor 'b2a'")
+    return [codes[d] for d in direction]
+
+
+def check_caption(caption, batch):
+    """A caption is one string, or a list of `batch` strings (one per image, encoded in one text-tower call)."""
+    if isinstance(caption, str):
+        return caption
+    if not isinstance(caption, (list, tuple)) or not all(isinstance(c, str) for c in caption):
+        raise ValueError("caption must be a string or a list of strings")
+    if len(caption) != batch:
+        raise ValueError(f"{batch} images but {len(caption)} captions")
+    return list(caption)
+
+
 class CycleGAN_Turbo(TurboBase):
     MODEL_KIND = i2it.CYCLEGAN
 
@@ -134,7 +164,9 @@ class CycleGAN_Turbo(TurboBase):
         pass   # all three adapters stay active with weight 1 (reference :72,181)
 
     def _run(self, x, direction, text_emb, eps=None):
-        assert direction in ["a2b", "b2a"]
+        if isinstance(direction, str):
+            assert direction in ["a2b", "b2a"]
+        code = direction_codes(direction, x.shape[0])
         dt = self.compute_dtype
         in_dtype = x.dtype
         B, _, H, Wd = x.shape
@@ -146,14 +178,14 @@ class CycleGAN_Turbo(TurboBase):
         if text.shape[0] not in (1, B):
             raise ValueError("caption embedding batch must be 1 or match the image batch")
         eng = self._finalize(1.0, 1.0, 1.0, -1.0)
-        out = self._staged_forward(eng, xd, text, eps, direction=i2it.A2B if direction == "a2b" else i2it.B2A)
+        out = self._staged_forward(eng, xd, text, eps, direction=code)
         return out if in_dtype == dt else out.to(in_dtype)
 
     @staticmethod
     def forward_with_networks(x, direction, vae_enc, unet, vae_dec, sched, timesteps, text_emb, eps=None):
         """Reference :199-207.  `vae_enc` must be the VAE_encode of a CycleGAN_Turbo built by this module; the UNet,
-        scheduler and decoder that run are that model's (fused on device)."""
-        assert direction in ["a2b", "b2a"]
+        scheduler and decoder that run are that model's (fused on device).  direction may be a list of one direction per
+        image (see forward)."""
         owner = getattr(vae_enc, "owner", None)
         if owner is None:
             raise RuntimeError("forward_with_networks needs the VAE_encode handle of an i2it CycleGAN_Turbo")
@@ -164,6 +196,10 @@ class CycleGAN_Turbo(TurboBase):
         raise NotImplementedError("training is outside this build's scope (inference hot path only)")
 
     def forward(self, x_t, direction=None, caption=None, caption_emb=None, *, eps=None):
+        """direction: "a2b" / "b2a", or a list of one per image: a batch that mixes both directions runs as ONE forward
+        (i2it.Engine.forward_mixed), image i byte-equal to the single-direction forward of the batch in direction[i].  A
+        network size a mixed forward refuses raises ValueError (i2it.mixed_size_check).  caption: one string or a list of B
+        strings; caption_emb: batch 1 or B."""
         if direction is None:
             assert self.direction is not None
             direction = self.direction
@@ -173,7 +209,7 @@ class CycleGAN_Turbo(TurboBase):
         if caption_emb is not None:
             caption_enc = caption_emb
         else:
-            caption_enc = self._encode_text(caption)
+            caption_enc = self._encode_text(check_caption(caption, x_t.shape[0]))
         return self.forward_with_networks(x_t, direction, self.vae_enc, self.unet, self.vae_dec, self.sched, self.timesteps,
                                           caption_enc, eps)
 
@@ -209,21 +245,27 @@ class CycleGAN_Turbo(TurboBase):
         -> a list of uint8 CUDA tensors [H_i, W_i, 3].  Each image goes through build_transform(image_prep)
         (_host.image_prep_geometry: ValueError for the random crops) and comes back at its input size, all on device
         (i2it.Engine.forward_u8_ragged).  The preps must give every image the same network size; eps is [B,4,H/8,W/8] of it.
-        Output i equals forward_u8(images[i][None], eps=eps[i:i+1], resize=, crop=, out_size=(H_i, W_i)) byte for byte."""
+        Output i equals forward_u8(images[i][None], eps=eps[i:i+1], resize=, crop=, out_size=(H_i, W_i)) byte for byte.
+        direction may be a list of one direction per upload (i2it.Engine.forward_u8_ragged_mixed: one plan for every mix);
+        caption one string or a list of B strings."""
         if direction is None:
             assert self.direction is not None
             direction = self.direction
         if caption is None and caption_emb is None:
             assert self.caption is not None
             caption = self.caption
-        assert direction in ["a2b", "b2a"]
+        if isinstance(direction, str):
+            assert direction in ["a2b", "b2a"]
+        code = direction_codes(direction, len(images))
         dt = self.compute_dtype
+        caption = caption if caption_emb is not None else check_caption(caption, len(images))
         text = self._prep(caption_emb if caption_emb is not None else self._encode_text(caption), dt)
+        if text.shape[0] not in (1, len(images)):
+            raise ValueError("caption embedding batch must be 1 or match the image batch")
         xs = [x.to(device=_host.DEVICE, non_blocking=True).contiguous() for x in images]
         H, Wd, geoms = _host.ragged_geometries([tuple(x.shape[:2]) for x in xs], image_prep=image_prep)
         if eps is None:
             eps = torch.randn((len(xs), 4, H // 8, Wd // 8), device=_host.DEVICE, dtype=dt)
         eps = self._prep(eps, dt)
         eng = self._finalize(1.0, 1.0, 1.0, -1.0)
-        return self._staged_forward(eng, xs, text, eps, direction=i2it.A2B if direction == "a2b" else i2it.B2A,
-                                    u8_mode=i2it.IN_NORMALIZE, ragged=geoms)
+        return self._staged_forward(eng, xs, text, eps, direction=code, u8_mode=i2it.IN_NORMALIZE, ragged=geoms)

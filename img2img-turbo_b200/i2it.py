@@ -36,6 +36,7 @@ SYMBOLS = [
     "i2it_debug_tapgemm_override", "i2it_forward_variations", "i2it_forward_u8_variations",
     "i2it_forward_u8_ragged", "i2it_op_resize_u8_ragged", "i2it_debug_ragged_tables", "i2it_debug_graph_captures",
     "i2it_refold_weights", "i2it_debug_refold_info",
+    "i2it_forward_mixed", "i2it_forward_u8_ragged_mixed", "i2it_mixed_size_check", "i2it_op_conv2d_sel",
 ]
 TEXT_TOKEN_EMB = "text_encoder.text_model.embeddings.token_embedding.weight"
 TEXT_POS_EMB = "text_encoder.text_model.embeddings.position_embedding.weight"
@@ -215,6 +216,11 @@ def load_library(path: Optional[str] = None):
     lib.i2it_debug_graph_captures.argtypes = [vp, C.POINTER(ci)]
     lib.i2it_refold_weights.argtypes = [vp, cf, cf, cf, cf]
     lib.i2it_debug_refold_info.argtypes = [vp, C.c_char_p, C.c_size_t]
+    lib.i2it_forward_mixed.argtypes = [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, C.POINTER(ci), vp]
+    lib.i2it_forward_u8_ragged_mixed.argtypes = [vp, C.POINTER(vp), ci, C.POINTER(ResizeDesc), ci, vp, ci, vp, C.POINTER(vp), vp,
+                                                 ci, ci, ci, C.POINTER(ci), vp]
+    lib.i2it_mixed_size_check.argtypes = [ci, ci, C.c_char_p, C.c_size_t]
+    lib.i2it_op_conv2d_sel.argtypes = [vp, C.POINTER(ConvDesc), vp, vp, vp, C.POINTER(ci), vp]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name not in ("i2it_destroy", "i2it_last_error"):
@@ -240,6 +246,25 @@ def _check_u8_images(images, what):
 
 def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def mixed_size_check(H: int, W: int) -> str:
+    """Why a mixed-direction forward refuses the network size H x W, or "" when it accepts it (i2it_mixed_size_check: every
+    VAE tile must hold rows of one image).  Host only."""
+    buf = C.create_string_buffer(1024)
+    load_library().i2it_mixed_size_check(int(H), int(W), buf, 1024)
+    return buf.value.decode()
+
+
+def directions_array(directions, n: int):
+    """The C array of a mixed-direction call: n values, each A2B (0) or B2A (1).  Raises ValueError otherwise."""
+    dirs = list(directions)
+    if len(dirs) != n:
+        raise ValueError(f"{n} images but {len(dirs)} directions")
+    for i, d in enumerate(dirs):
+        if isinstance(d, bool) or not isinstance(d, int) or d not in (A2B, B2A):
+            raise ValueError(f"direction {d!r} of image {i} is neither A2B (0) nor B2A (1)")
+    return (C.c_int * n)(*dirs)
 
 
 class Engine:
@@ -477,6 +502,51 @@ class Engine:
                                                     W, direction, _stream()), "i2it_forward_u8_ragged")
         return list(outs)
 
+    def forward_mixed(self, x: torch.Tensor, text_emb: Optional[torch.Tensor], eps: torch.Tensor, directions,
+                      out: Optional[torch.Tensor] = None, out_latent: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """CycleGAN forward of a batch that mixes both directions (i2it_forward_mixed): image i through vae (directions[i] ==
+        A2B) or vae_b2a (B2A).  Output i equals image i of forward(..., direction=directions[i]) byte for byte; one plan and
+        one CUDA graph serve every mix.  A refused size raises ValueError with the engine's rule (mixed_size_check)."""
+        B, Cc, H, W = x.shape
+        assert Cc == 3, "image must be [B,3,H,W]"
+        dirs = directions_array(directions, B)
+        why = mixed_size_check(H, W)
+        if why:
+            raise ValueError("mixed-direction forward: " + why)
+        tb = self._check_operands(B, H, W, text_emb, eps, (x, out, out_latent))
+        if out is None:
+            out = torch.empty_like(x)
+        self._check(self.lib.i2it_forward_mixed(self._h, _ptr(x), _ptr(text_emb), tb, _ptr(eps), _ptr(out), _ptr(out_latent),
+                                                B, H, W, dirs, _stream()), "i2it_forward_mixed")
+        return out
+
+    def forward_u8_ragged_mixed(self, images: Sequence[torch.Tensor], in_mode: int, text_emb: Optional[torch.Tensor],
+                                eps: torch.Tensor, directions, *, geometries, max_side: Optional[int] = None,
+                                outs: Optional[Sequence[torch.Tensor]] = None, out_latent: Optional[torch.Tensor] = None):
+        """forward_u8_ragged with a direction per image (i2it_forward_u8_ragged_mixed): uploads of any size, both directions,
+        one plan.  Output i equals forward_u8(images[i][None], ..., direction=directions[i], **geometries[i]) byte for byte."""
+        n = len(images)
+        _check_u8_images(images, "forward_u8_ragged_mixed")
+        dirs = directions_array(directions, n)
+        H, W, descs = _ragged_descs(geometries, [tuple(x.shape[:2]) for x in images])
+        why = mixed_size_check(H, W)
+        if why:
+            raise ValueError("mixed-direction forward: " + why)
+        if eps.shape[0] != n:
+            raise ValueError(f"{n} images but eps has batch {eps.shape[0]}")
+        tb = self._check_operands(n, H, W, text_emb, eps, (out_latent,))
+        if max_side is None:
+            max_side = ragged_max_side([v for d in descs for v in (d.in_H, d.in_W, d.resize_H, d.resize_W, d.out_H, d.out_W)])
+        if outs is None:
+            outs = [torch.empty(d.out_H, d.out_W, 3, dtype=torch.uint8, device=images[0].device) for d in descs]
+        if len(outs) != n or any(tuple(o.shape) != (d.out_H, d.out_W, 3) or o.dtype != torch.uint8 or not o.is_cuda
+                                 or not o.is_contiguous() for o, d in zip(outs, descs)):
+            raise ValueError("outs must be n contiguous uint8 CUDA tensors [out_H_i, out_W_i, 3]")
+        self._check(self.lib.i2it_forward_u8_ragged_mixed(self._h, _ptrs(images), int(in_mode), descs, int(max_side),
+                                                          _ptr(text_emb), tb, _ptr(eps), _ptrs(outs), _ptr(out_latent), n, H, W,
+                                                          dirs, _stream()), "i2it_forward_u8_ragged_mixed")
+        return list(outs)
+
     def graph_captures(self) -> int:
         """CUDA graphs this engine has captured (a replayed forward captures none)."""
         n = C.c_int(0)
@@ -593,8 +663,16 @@ class Engine:
                                             int(out_fp32), _stream()), "i2it_op_conv2d")
         return out
 
+    def op_conv2d_sel(self, x_nhwc, w, bias, w_alt, bias_alt, directions, *, w2_alt=None, **kw):
+        """op_conv2d_ex with a second weight set chosen per image (i2it_op_conv2d_sel): image n uses (w_alt, bias_alt, w2_alt)
+        where directions[n] == 1.  w2_alt None shares w2.  Keywords as op_conv2d_ex."""
+        dirs = directions_array(directions, x_nhwc.shape[0])
+        keep = [w_alt.float().contiguous(), bias_alt.float().contiguous() if bias_alt is not None else None,
+                w2_alt.float().contiguous() if w2_alt is not None else None]
+        return self.op_conv2d_ex(x_nhwc, w, bias, _sel=(keep, dirs), **kw)
+
     def op_conv2d_ex(self, x_nhwc, w, bias=None, *, stride=1, asym_pad=False, residual=None, act=ACT_NONE, out=None,
-                     out_fp32=False, x2=None, w2=None, up2x=False, tokens=False, gn=None, gn_out=None):
+                     out_fp32=False, x2=None, w2=None, up2x=False, tokens=False, gn=None, gn_out=None, _sel=None):
         """Every conv variant of the engine (i2it_conv_desc).  NHWC views may be channel slices (pixel stride > C);
         `out` / `gn_out` are optional preallocated views.  gn = (gamma, beta, eps, silu) adds the GroupNorm that consumes the
         output.  Returns out, or (out, groupnorm output) when gn is given."""
@@ -623,7 +701,12 @@ class Engine:
             keep += [gamma.float().contiguous(), beta.float().contiguous()]
             d.gn_y, d.ldg, d.gn_silu, d.gn_eps = g.data_ptr(), g.stride(2), int(silu), float(eps)
             d.gn_gamma, d.gn_beta = _ptr(keep[3]), _ptr(keep[4])
-        self._check(self.lib.i2it_op_conv2d_ex(self._h, C.byref(d), _stream()), "i2it_op_conv2d_ex")
+        if _sel is not None:
+            (wa, ba, w2a), dirs = _sel
+            self._check(self.lib.i2it_op_conv2d_sel(self._h, C.byref(d), _ptr(wa), _ptr(ba), _ptr(w2a), dirs, _stream()),
+                        "i2it_op_conv2d_sel")
+        else:
+            self._check(self.lib.i2it_op_conv2d_ex(self._h, C.byref(d), _stream()), "i2it_op_conv2d_ex")
         return (out, g) if gn is not None else out
 
     def op_launches(self):

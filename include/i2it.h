@@ -238,6 +238,35 @@ int i2it_forward_u8_ragged(i2it_handle* h, const void* const* x_u8, int in_mode,
                            const void* text_emb, int text_batch, const void* eps, const void* noise_map, float r,
                            void* const* out_u8, void* out_latent, int n, int H, int W, int direction, void* stream);
 
+/* A CycleGAN batch that mixes both directions in one forward: image i goes through vae (directions[i] == I2IT_A2B) or
+ * vae_b2a (I2IT_B2A).  directions is a HOST array of batch values; every other operand is i2it_forward's (there is no
+ * noise_map: CycleGAN has none), with text_batch 1 or batch and text_emb NULL for the i2it_set_text cache.  The UNet, the
+ * DDPM step and the latent sampling are the same for both directions; every VAE launch that reads weights (the convs,
+ * quant_conv / post_quant_conv, the attention's projections and the GroupNorm applies) takes each 128-row tile's or each
+ * image's weights from its direction, in the same accumulation order, so output image i is byte-equal to image i of a
+ * single-direction i2it_forward in directions[i] (same x, eps, text).  One plan per (batch, H, W, text mode) serves every
+ * mix: the directions are copied to the plan ahead of the first launch, and its CUDA graph reads them there.  It has the
+ * launch count and tile geometry of the single-direction plan.
+ * Accepted sizes: those whose every VAE tile holds rows of one image (i2it_mixed_size_check), e.g. 256x256, 512x512,
+ * 512x768 and 1024x1024; 1280x720 is refused (its (H/8)(W/8) = 14400 latent pixels are not a multiple of 128).
+ * Rejected before any launch, and without building a plan: a pix2pix handle, a NULL directions array, a value other
+ * than 0 or 1, a refused size, and whatever i2it_forward rejects. */
+int i2it_forward_mixed(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps, void* out,
+                       void* out_latent, int batch, int H, int W, const int* directions, void* stream);
+
+/* i2it_forward_u8_ragged with a direction per image (host array of n values, as i2it_forward_mixed): uploads of any size
+ * and both directions through one plan.  Output i is byte-equal to the batch-1 i2it_forward_u8_resize of upload i in
+ * directions[i].  Rejected before any launch: what i2it_forward_u8_ragged and i2it_forward_mixed reject. */
+int i2it_forward_u8_ragged_mixed(i2it_handle* h, const void* const* x_u8, int in_mode, const i2it_resize_desc* g, int max_side,
+                                 const void* text_emb, int text_batch, const void* eps, void* const* out_u8, void* out_latent,
+                                 int n, int H, int W, const int* directions, void* stream);
+
+/* Whether a mixed-direction forward accepts the network size H x W: 0 if it does, 1 if not, with the reason (naming the
+ * rule) in msg (cap bytes, NUL-terminated; msg may be NULL).  The rule: (H/8)(W/8) is a multiple of 128 (the VAE
+ * attention's token launches), and on every VAE map level H/2^k x W/2^k the conv's 128-row tile box covers pixels of one
+ * image.  No GPU needed. */
+int i2it_mixed_size_check(int H, int W, char* msg, size_t cap);
+
 /* Number of kernel launches one forward of this shape issues (for bench accounting): the plan the last forward used if it
  * has this shape, else the plan with the text embedding passed inline. */
 int i2it_launch_count(i2it_handle* h, int batch, int H, int W, int direction, int* launches);
@@ -326,6 +355,12 @@ typedef struct i2it_conv_desc {
   void* gn_y; int ldg, gn_silu; float gn_eps; const float* gn_gamma; const float* gn_beta;
 } i2it_conv_desc;
 int i2it_op_conv2d_ex(i2it_handle* h, const i2it_conv_desc* d, void* stream);
+/* i2it_op_conv2d_ex with a second weight set chosen per image, as a mixed-direction plan's VAE convs run: image n uses
+ * (w_alt, bias_alt, w2_alt) where directions[n] == 1 (host array of d->N values, each 0 or 1) and d's weights where it is
+ * 0.  bias_alt is required iff d->bias is; w2_alt NULL shares d->w2.  A GroupNorm (d->gn_y) uses d's gamma / beta for
+ * every image.  Refused: a tile that would hold rows of two images (tokens: H*W not a multiple of 128). */
+int i2it_op_conv2d_sel(i2it_handle* h, const i2it_conv_desc* d, const float* w_alt, const float* bias_alt, const float* w2_alt,
+                       const int* directions, void* stream);
 /* Launch list of the last op call, as a JSON array [{"kind","shape"}...] (GEMM shape strings carry BN, tma/tma2, gn;
  * softmax launches carry their variant 32 / 128 / long). */
 int i2it_op_launches(i2it_handle* h, char* json, size_t cap);
