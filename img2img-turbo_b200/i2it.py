@@ -733,9 +733,15 @@ class Engine:
         return out
 
     def op_attention(self, q, k, vt, heads, causal=False):
+        """q [B, Nq, C], k [1|B, Nk, C], vt [1|B, C, ldv >= Nk].  Rows may be strided (q and k as column slices of one fused
+        projection), but the C ABI takes one leading dimension per operand: image b must start b * rows * ld elements in."""
         B, Nq, Cc = q.shape
         kvb, Nk, _ = k.shape
-        out = torch.empty_like(q)
+        for t, rows in ((q, Nq), (k, Nk), (vt, Cc)):
+            if t.stride(2) != 1 or (t.shape[0] > 1 and t.stride(0) != rows * t.stride(1)):
+                raise ValueError(f"op_attention: operand of shape {list(t.shape)} has strides {t.stride()}; images must be "
+                                 "[rows, ld] blocks with unit column stride")
+        out = torch.empty(B, Nq, Cc, device=q.device, dtype=q.dtype)
         self._check(self.lib.i2it_op_attention(self._h, _ptr(q), q.stride(1), _ptr(k), k.stride(1), _ptr(vt), vt.stride(1), B, Nq,
                                                Nk, heads, Cc // heads, kvb, int(causal), _ptr(out), Cc, _stream()),
                     "i2it_op_attention")

@@ -186,11 +186,11 @@ class Audit:
 
     def attention(self, name, q, k, v, heads, H, W, causal=False):
         """q [B, Nq, C], k / v [kvB, Nk, C] (the engine's own operands) -> stage [B, C, H, W]."""
-        o, pav, e_s = kref.attention64(q, k, v, heads, causal=causal)
+        o, pav, e_s, psub = kref.attention64(q, k, v, heads, causal=causal)
         B, C = q.shape[0], q.shape[2]
         sp = lambda t: t.reshape(B, H, W, C).permute(0, 3, 1, 2)
-        ref, pav, e_s = sp(o), sp(pav), sp(e_s)
-        self.emit("attention", name, ref, lambda got: kref.check_attention(name, got, ref, pav, e_s, k.shape[1], self.dt))
+        ref, pav, e_s, psub = sp(o), sp(pav), sp(e_s), sp(psub)
+        self.emit("attention", name, ref, lambda got: kref.check_attention(name, got, ref, pav, e_s, psub, k.shape[1], self.dt))
 
     # ------------------------------------------------------------------------------------------------ blocks
     def vae_resnet(self, p, x, skip=None, skip_key=None):

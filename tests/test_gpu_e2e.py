@@ -223,9 +223,8 @@ def test_runtime_switches_agree(monkeypatch):
     args = (x.to(dt).cuda(), text[:1].to(dt).cuda(), eps.to(dt).cuda())
 
     def run(**env):
-        for k in ("I2IT_NO_CATFUSE", "I2IT_NO_TMAOUT", "I2IT_NO_GNEPI", "I2IT_NO_SPLITK", "I2IT_FLASH_V1", "I2IT_NO_IDRES", "I2IT_IDRES",
-                  "I2IT_NO_LEAN", "I2IT_NO_OSTG2",
-                  "I2IT_NO_HALO", "I2IT_NO_PAIR"):
+        for k in ("I2IT_NO_CATFUSE", "I2IT_NO_TMAOUT", "I2IT_NO_GNEPI", "I2IT_NO_SPLITK", "I2IT_NO_IDRES", "I2IT_IDRES",
+                  "I2IT_NO_LEAN", "I2IT_NO_OSTG2", "I2IT_NO_FLASH"):
             monkeypatch.delenv(k, raising=False)
         for k, v in env.items():
             monkeypatch.setenv(k, v)
@@ -239,10 +238,11 @@ def test_runtime_switches_agree(monkeypatch):
     assert torch.equal(base, run(I2IT_NO_LEAN="1"))            # the compile-time-stripped epilogue computes the same bits
     assert torch.equal(base, run(I2IT_NO_OSTG2="1"))           # one or two store boxes: data movement only
     assert torch.equal(run(I2IT_NO_GNEPI="1"), run(I2IT_NO_GNEPI="1", I2IT_NO_TMAOUT="1"))
-    for env in ({"I2IT_NO_GNEPI": "1"}, {"I2IT_NO_SPLITK": "1"}, {"I2IT_IDRES": "1"}):
+    for env in ({"I2IT_NO_GNEPI": "1"}, {"I2IT_NO_SPLITK": "1"}, {"I2IT_IDRES": "1"}, {"I2IT_NO_FLASH": "1"}):
         y = run(**env)
         d = (y.float() - base.float()).abs()
         # different summation orders of the fp32 statistics / K ranges flip last bits of bf16 activations (1 ulp at 1.0 = 7.8e-3),
+        # and the unfused attention normalises P before rounding it where the flash kernel rounds exp(s - m) and divides last,
         # which the rest of the network carries to the output: the variants agree to about one output ulp on average
         assert torch.isfinite(y.float()).all() and d.mean().item() < 1.2e-2 and d.max().item() < 0.2, (env, d.mean().item(), d.max().item())
 

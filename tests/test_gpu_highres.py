@@ -70,14 +70,14 @@ def operands(B, Nq, Nk, kvb, dtype, qscale=1.0):
     return q, k, v, vt
 
 
-def check_rows(name, got, q, k, v, dtype, rows=None):
-    """float64 reference for all query rows, or only for `rows` (a list of (start, stop) ranges)."""
+def check_rows(name, got, q, k, v, dtype, rows=None, flash=True):
+    """float64 reference for all query rows, or only for `rows` (a list of (start, stop) ranges); flash: the fused kernel."""
     Nk = k.shape[1]
     parts = [(0, q.shape[1])] if rows is None else rows
     checks = []
     for a, b in parts:
-        ref, pav, e_s = kref.attention64(q[:, a:b], k, v, 1)
-        checks.append(kref.check_attention(f"{name} rows {a}:{b}", got[:, a:b], ref, pav, e_s, Nk, dtype))
+        ref, pav, e_s, psub = kref.attention64(q[:, a:b], k, v, 1, flash=flash)
+        checks.append(kref.check_attention(f"{name} rows {a}:{b}", got[:, a:b], ref, pav, e_s, psub, Nk, dtype))
     report(*checks)
 
 
@@ -132,13 +132,13 @@ def test_d512_path_boundary(dtype):
     got = E.op_attention(q, k, vt, 1)
     ops = launches(E, f"d512 k8192 {dtype}")
     assert "flash_attn512" not in kinds(ops) and [o["shape"] for o in ops if o["kind"] == "softmax"] == ["long"]
-    check_rows(f"d512 k8192 {dtype}", got, q, k, v, dtype)
+    check_rows(f"d512 k8192 {dtype}", got, q, k, v, dtype, flash=False)
     E = engine(dtype, no_flash=True)
     q, k, v, vt = operands(1, 300, 16384, 1, dtype)
     got = E.op_attention(q, k, vt, 1)
     ops = launches(E, f"d512 k16384 I2IT_NO_FLASH {dtype}")
     assert "flash_attn512" not in kinds(ops) and [o["shape"] for o in ops if o["kind"] == "softmax"] == ["long"]
-    check_rows(f"d512 k16384 I2IT_NO_FLASH {dtype}", got, q, k, v, dtype)
+    check_rows(f"d512 k16384 I2IT_NO_FLASH {dtype}", got, q, k, v, dtype, flash=False)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -328,8 +328,8 @@ def attn_case(E, dtype, B, Nq, Nk, heads, d, kvb, causal=False, name=""):
     vt[:, :, :Nk] = v.transpose(1, 2)
     got = E.op_attention(q, k, vt, heads, causal=causal)
     ops = launches(E, name)
-    ref, pav, e_s = kref.attention64(q, k, v, heads, causal=causal)
-    report(kref.check_attention(name, got, ref, pav, e_s, Nk, dtype))
+    ref, pav, e_s, psub = kref.attention64(q, k, v, heads, causal=causal, flash=d == 64)     # d = 64 runs flash_attn
+    report(kref.check_attention(name, got, ref, pav, e_s, psub, Nk, dtype))
     return q, k, vt, got, ops
 
 

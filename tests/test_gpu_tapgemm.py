@@ -174,10 +174,10 @@ def attn_sub(dtype, bn, Nq=200, heads=2, d=128):
     q, k, v = mk(1, Nq, C, dtype=dtype, seed=1), mk(1, Nk, C, dtype=dtype, seed=2), mk(1, Nk, C, dtype=dtype, seed=3)
     vt = torch.zeros(1, C, (Nk + 7) // 8 * 8, device="cuda", dtype=dtype)
     vt[:, :, :Nk] = v.transpose(1, 2)
-    ref, pav, e_s = kref.attention64(q, k, v, heads)
+    ref, pav, e_s, psub = kref.attention64(q, k, v, heads)
     name = f"attention logits Nq={Nq} Nk={Nk} d={d}"
     return Sub(name, lambda E: (E.op_attention(q, k, vt, heads), None),
-               lambda y, g: [kref.check_attention(name, y, ref, pav, e_s, Nk, dtype)],
+               lambda y, g: [kref.check_attention(name, y, ref, pav, e_s, psub, Nk, dtype)],
                main="tapgemm:attn_qk", ksteps=d // 64, tma=False)
 
 

@@ -98,8 +98,8 @@ def test_attention_rejects_a_causal_mask_one_key_off(dtype):
     g = _gen(6)
     B, N, heads, d = 1, 77, 2, 64
     q, k, v = (torch.randn(B, N, heads * d, generator=g).to(dtype) for _ in range(3))
-    ref, pav, e_s = kref.attention64(q, k, v, heads, causal=True)
-    ok = kref.check_attention("ok", kref.round16(ref, dtype), ref, pav, e_s, N, dtype)
+    ref, pav, e_s, psub = kref.attention64(q, k, v, heads, causal=True)
+    ok = kref.check_attention("ok", kref.round16(ref, dtype), ref, pav, e_s, psub, N, dtype)
     assert ok, str(ok)
     # the mask admits key i+1 for query i
     qf = q.double().view(B, N, heads, d).transpose(1, 2)
@@ -107,7 +107,7 @@ def test_attention_rejects_a_causal_mask_one_key_off(dtype):
     vf = v.double().view(B, N, heads, d).transpose(1, 2)
     s = (qf @ kf.transpose(-1, -2) / math.sqrt(d)).masked_fill(torch.ones(N, N, dtype=torch.bool).triu(2), float("-inf"))
     leak = (torch.softmax(s, -1) @ vf).transpose(1, 2).reshape(B, N, heads * d)
-    bad = kref.check_attention("leak", kref.round16(leak, dtype), ref, pav, e_s, N, dtype)
+    bad = kref.check_attention("leak", kref.round16(leak, dtype), ref, pav, e_s, psub, N, dtype)
     assert not bad and bad.n_bad > 0, str(bad)
 
 

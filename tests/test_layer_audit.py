@@ -109,7 +109,7 @@ def test_cross_attention_with_the_neighbouring_blocks_k(sd_det):
         q = a.src.stages[name + ".to_q"].double().permute(0, 2, 3, 1).reshape(B, H * W, C)
         k = a.src.stages[other].double().permute(0, 2, 3, 1).reshape(1, 77, C)
         vv = a.src.stages[name + ".to_v"].double()[:, :77, 0, :]
-        o, _, _ = kref.attention64(q, k, vv, 1)
+        o = kref.attention64(q, k, vv, 1)[0]
         return kref.round16(o.reshape(B, H, W, C).permute(0, 3, 1, 2), DT)
     assert _failed(_audit(_spec(sd_det), stage_hook=hook)) == [name]
 
