@@ -300,6 +300,8 @@ class Engine:
         rc = self.lib.i2it_create(C.byref(c), C.byref(self._h))
         if rc != 0:
             raise RuntimeError("i2it_create failed: " + self.lib.i2it_last_error(C.c_void_p(0)).decode())
+        # i2it_create reads I2IT_NO_FLASH: without it d = 64 attention runs flash_attn, and d = 512 flash_attn512 above 8192 keys
+        self.flash = os.environ.get("I2IT_NO_FLASH") is None
         if max_plans:
             self.set_max_plans(max_plans)
 

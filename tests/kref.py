@@ -24,7 +24,12 @@ sub = sum_{j in S} |V_j| + |S| |out|.  Where the row's weight sits on a key whos
 The attention bound's Nk * 2^-24 term (the fp32 P V chain's worst case) is 1.1 % of P @ |V| at 190512 keys, about the size of
 the output itself, so there the per-element bound alone would pass a dropped KV tile or an all-zero output.  Those checks
 also cap the mean-ulp statistic at 0.75: a correct 16-bit rounding lands near 0.25 and the flash kernel's fp32 chains over
-190512 keys measure 0.40 (bf16) to 0.49 (fp16) on an H100, while one dropped KV tile already gives several ulps on average.
+190512 keys measure 0.40 (bf16) to 0.49 (fp16) on an H100, while one dropped KV tile already gives several ulps on average;
+the d = 512 flash kernel measures the same (0.41 and 0.50 at 190512 keys).  The cap does not hold on the unfused path in
+fp16 past about 16384 keys, and is not applied there: its probabilities are relative to the row sum, p_j ~ 1 / Nk falls below
+fp16's smallest normal 2^-14, and each then carries an absolute rounding error up to 2^-25, several percent of itself.  The
+per-element bound covers that through eta * sub, but the mean error grows with Nk: 0.60 ulp at 32400 keys, 1.03 at 65536,
+2.88 at 190512 (H100, d = 512, I2IT_NO_FLASH).  The model runs that path only up to 8192 keys, where p_j stays normal.
 Everything here runs on CPU or GPU tensors alike.
 """
 import math

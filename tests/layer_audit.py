@@ -184,9 +184,18 @@ class Audit:
     def read_v(self, name, ntok):
         return self.S(name)[:, 0, :, :ntok].transpose(1, 2)            # NHWC [B, 1, C, ldv] -> V [B, ntok, C]
 
+    def flash_path(self, heads, d, Nk):
+        """Whether the source's engine ran this attention on a flash kernel, whose probabilities are relative to the row
+        maximum (tests/kref.py header): d = 64 unless the engine was created with I2IT_NO_FLASH, and the one-head d = 512
+        attention above 8192 keys.  A source that does not say (the emulated one) gets the unfused set, which contains it."""
+        if not getattr(self.src, "flash", False):
+            return False
+        return d == 64 or (d == 512 and heads == 1 and Nk > 8192)
+
     def attention(self, name, q, k, v, heads, H, W, causal=False):
         """q [B, Nq, C], k / v [kvB, Nk, C] (the engine's own operands) -> stage [B, C, H, W]."""
-        o, pav, e_s, psub = kref.attention64(q, k, v, heads, causal=causal)
+        flash = self.flash_path(heads, q.shape[2] // heads, k.shape[1])
+        o, pav, e_s, psub = kref.attention64(q, k, v, heads, causal=causal, flash=flash)
         B, C = q.shape[0], q.shape[2]
         sp = lambda t: t.reshape(B, H, W, C).permute(0, 3, 1, 2)
         ref, pav, e_s, psub = sp(o), sp(pav), sp(e_s), sp(psub)
@@ -685,6 +694,10 @@ class EngineSource:
         self.e, self.inputs = engine, inputs
         self._cache = {}
         self._dims = dict(engine.stage_names())
+
+    @property
+    def flash(self):
+        return self.e.flash
 
     def read_stage(self, name):
         if name not in self._cache:

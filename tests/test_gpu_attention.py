@@ -147,6 +147,9 @@ CASES = [
     (1, 1, 300, 14400, 5, "spiky", "slice"),
     (2, 2, 136, 14400, 10, "flat", "dense"),
     (1, 1, 9, 14400, 1, "uniform", "dense"),
+    (2, 2, 65, 65, 5, "sunken", "slice"),        # every real logit near -32: an unmasked tail would win every row
+    (1, 1, 129, 4097, 10, "sunken", "dense"),
+    (2, 1, 300, 14401, 5, "sunken", "slice"),
 ]
 IDS = [f"b{b}_kv{kv}_q{nq}_k{nk}_h{h}_{r}_{lay}" for b, kv, nq, nk, h, r, lay in CASES]
 

@@ -1,14 +1,12 @@
-"""-m gpu: images past 512^2.  The VAE mid-block attention (one head of 512) runs fused above 8192 keys, and the decoder's
-full-resolution tensors of a 12-megapixel image (256 x 4032 x 3024 = 3.1e9 elements) pass 2^31 elements.
+"""-m gpu: images past 512^2.  The decoder's full-resolution tensors of a 12-megapixel image (256 x 4032 x 3024 = 3.1e9
+elements) pass 2^31 elements.  The VAE mid-block attention (one head of 512, fused above 8192 keys) has its own file,
+tests/test_gpu_attention_d512.py.
 
-  attention   op_attention at d = 512 against the float64 softmax of tests/kref.py, with the same per-element bound as the
-              d = 64 flash kernel; the path taken is asserted from the launch list
   2^31        the decoder's largest convs and GroupNorm at 4032x3024x256, checked on row bands (first rows, the rows around
               the 2^31-element offset, last rows) against float64 references computed for those bands only
   end to end  1280x720 against the CPU fp32 oracle stage by stage; 4032x3024 through the public wrapper (finite, in range)
 """
 import math
-import os
 import sys
 
 import pytest
@@ -23,17 +21,9 @@ DTYPES = [pytest.param(bf, id="bf16"), pytest.param(hf, id="fp16")]
 H12, W12 = 3024, 4032            # a 12 MP phone photo (landscape 4032 x 3024)
 
 
-def engine(dtype, no_flash=False):
+def engine(dtype):
     import i2it
-    saved = os.environ.pop("I2IT_NO_FLASH", None)
-    try:
-        if no_flash:
-            os.environ["I2IT_NO_FLASH"] = "1"
-        return i2it.Engine(dtype, use_cuda_graph=False)
-    finally:
-        os.environ.pop("I2IT_NO_FLASH", None)
-        if saved is not None:
-            os.environ["I2IT_NO_FLASH"] = saved
+    return i2it.Engine(dtype, use_cuda_graph=False)
 
 
 def mk(*shape, dtype=torch.float32, scale=1.0, seed=0):
@@ -56,89 +46,6 @@ def report(*checks):
         print("   ", c)
     for c in checks:
         assert c, str(c)
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# attention, d = 512
-# ---------------------------------------------------------------------------------------------------------------------
-def operands(B, Nq, Nk, kvb, dtype, qscale=1.0):
-    q = mk(B, Nq, 512, dtype=dtype, scale=qscale, seed=1)
-    k = mk(kvb, Nk, 512, dtype=dtype, seed=2)
-    v = mk(kvb, Nk, 512, dtype=dtype, seed=3)
-    vt = torch.zeros(kvb, 512, (Nk + 7) // 8 * 8, device="cuda", dtype=dtype)
-    vt[:, :, :Nk] = v.transpose(1, 2)
-    return q, k, v, vt
-
-
-def check_rows(name, got, q, k, v, dtype, rows=None, flash=True):
-    """float64 reference for all query rows, or only for `rows` (a list of (start, stop) ranges); flash: the fused kernel."""
-    Nk = k.shape[1]
-    parts = [(0, q.shape[1])] if rows is None else rows
-    checks = []
-    for a, b in parts:
-        ref, pav, e_s, psub = kref.attention64(q[:, a:b], k, v, 1, flash=flash)
-        checks.append(kref.check_attention(f"{name} rows {a}:{b}", got[:, a:b], ref, pav, e_s, psub, Nk, dtype))
-    report(*checks)
-
-
-ATTN = [(1, 300, 8193, 1), (2, 300, 8193, 2), (1, 300, 14400, 1), (2, 129, 14400, 1), (2, 300, 16384, 2), (1, 300, 65536, 1)]
-
-
-@pytest.mark.parametrize("B,Nq,Nk,kvb", ATTN, ids=[f"b{b}_q{q}_k{k}_kv{v}" for b, q, k, v in ATTN])
-@pytest.mark.parametrize("dtype", DTYPES)
-def test_fused_attention_d512(dtype, B, Nq, Nk, kvb):
-    E = engine(dtype)
-    q, k, v, vt = operands(B, Nq, Nk, kvb, dtype)
-    got = E.op_attention(q, k, vt, 1)
-    name = f"d512 q{Nq} k{Nk} b{B} kvb{kvb} {dtype}"
-    ops = launches(E, name)
-    assert kinds(ops)[0] == "flash_attn512" and "softmax" not in kinds(ops)
-    check_rows(name, got, q, k, v, dtype)
-    if B > 1 and kvb == B:
-        one = E.op_attention(q[1:].contiguous(), k[1:].contiguous(), vt[1:].contiguous(), 1)
-        assert torch.equal(one, got[1:])
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
-def test_fused_attention_d512_peaked(dtype):
-    """Q scaled x4: logits of std ~4, so the running maximum moves and the rescale of O and l carries the result."""
-    E = engine(dtype)
-    q, k, v, vt = operands(1, 300, 14400, 1, dtype, qscale=4.0)
-    got = E.op_attention(q, k, vt, 1)
-    assert kinds(launches(E, f"d512 peaked {dtype}"))[0] == "flash_attn512"
-    check_rows(f"d512 peaked {dtype}", got, q, k, v, dtype)
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
-def test_fused_attention_d512_12mp(dtype):
-    """The decoder attention of a 4032x3024 image: Nq = Nk = 190512.  The float64 reference covers sampled query tiles."""
-    N = (H12 // 8) * (W12 // 8)
-    E = engine(dtype)
-    q, k, v, vt = operands(1, N, N, 1, dtype)
-    got = E.op_attention(q, k, vt, 1)
-    torch.cuda.synchronize()
-    assert kinds(launches(E, f"d512 12MP {dtype}"))[0] == "flash_attn512"
-    assert torch.isfinite(got.float()).all()
-    rows = [(0, 64), (64 * 997 + 13, 64 * 998 + 13), (N // 2, N // 2 + 64), (N - 64 * 40, N - 64 * 39), (N - 100, N)]
-    check_rows(f"d512 12MP {dtype}", got, q, k, v, dtype, rows)
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
-def test_d512_path_boundary(dtype):
-    """8192 keys stay on the unfused path (fp32 logits GEMM, `long` softmax, PV GEMM); I2IT_NO_FLASH turns the fused kernel
-    off above the threshold too, and the unfused result passes the same bound."""
-    E = engine(dtype)
-    q, k, v, vt = operands(1, 300, 8192, 1, dtype)
-    got = E.op_attention(q, k, vt, 1)
-    ops = launches(E, f"d512 k8192 {dtype}")
-    assert "flash_attn512" not in kinds(ops) and [o["shape"] for o in ops if o["kind"] == "softmax"] == ["long"]
-    check_rows(f"d512 k8192 {dtype}", got, q, k, v, dtype, flash=False)
-    E = engine(dtype, no_flash=True)
-    q, k, v, vt = operands(1, 300, 16384, 1, dtype)
-    got = E.op_attention(q, k, vt, 1)
-    ops = launches(E, f"d512 k16384 I2IT_NO_FLASH {dtype}")
-    assert "flash_attn512" not in kinds(ops) and [o["shape"] for o in ops if o["kind"] == "softmax"] == ["long"]
-    check_rows(f"d512 k16384 I2IT_NO_FLASH {dtype}", got, q, k, v, dtype, flash=False)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -358,18 +358,6 @@ def test_flash_attention(dtype, B, Nq, Nk, heads, kvb):
         assert torch.equal(one, got[1:])
 
 
-UNFUSED = [(1024, "32"), (1025, "128"), (4096, "128"), (4097, "long"), (7350, "long")]
-
-
-@pytest.mark.parametrize("Nk,variant", UNFUSED, ids=[f"k{n}" for n, _ in UNFUSED])
-@pytest.mark.parametrize("dtype", DTYPES)
-def test_unfused_attention_d512(dtype, Nk, variant):
-    """VAE mid-block attention (one head of 512): fp32 logits GEMM, softmax variant by row length, PV GEMM."""
-    E = engine(dtype)
-    _, _, _, _, ops = attn_case(E, dtype, 1, 300, Nk, 1, 512, 1, name=f"d512 k{Nk} {dtype}")
-    assert [o["shape"] for o in ops if o["kind"] == "softmax"] == [variant]
-
-
 @pytest.mark.parametrize("ntok", [77, 4096])
 @pytest.mark.parametrize("dtype", DTYPES)
 def test_vt_projection(dtype, ntok):

@@ -169,3 +169,18 @@ def test_nonzero_cin_pad_column(sd_det):
     a = _audit(_spec(sd_det), weight_hook=hook)
     assert _failed(a) == [key]
     assert "padding" in [c for _, n, c in a.failures()][0].extra
+
+
+def test_attention_bound_follows_the_engines_path():
+    """The subnormal set of the attention bound (kref.py header) is the flash one where the engine ran a flash kernel:
+    every d = 64 layer unless the engine was created with I2IT_NO_FLASH, the one-head d = 512 layer above 8192 keys."""
+    class Src:
+        def __init__(self, flash):
+            self.flash, self.inputs = flash, dict(x=torch.zeros(1, 3, S, S))
+
+    import weights as W
+    on, off = LA.Audit(Src(True), LA.Spec({}, W.TINY), DT), LA.Audit(Src(False), LA.Spec({}, W.TINY), DT)
+    assert on.flash_path(5, 64, 4096) and on.flash_path(1, 64, 1)
+    assert not on.flash_path(1, 512, 8192) and on.flash_path(1, 512, 8193)
+    assert not any(off.flash_path(h, d, n) for h, d, n in ((5, 64, 4096), (1, 512, 8193)))
+    assert not LA.Audit(LA.EmulatedSource(Src(True).inputs), LA.Spec({}, W.TINY), DT).flash_path(5, 64, 4096)
