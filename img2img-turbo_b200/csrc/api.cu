@@ -134,15 +134,11 @@ int i2it_debug_poison_workspace(i2it_handle* h, int value) {
   API_END
 }
 
-int i2it_forward(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps,
-                 const void* noise_map, float r, void* out, void* out_latent, int batch, int H, int W, int direction,
-                 void* stream) {
+int i2it_forward(i2it_handle* h, const i2it_forward_desc* d, void* stream) {
   API_BEGIN(h)
-  IO io;
-  std::memset(&io, 0, sizeof io);
-  io.x = x; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r; io.out = out; io.out_latent = out_latent;
+  I2IT_CHECK(d != nullptr, "i2it_forward: null request");
   E.check_device_error();
-  E.forward(io, batch, H, W, direction, text_batch, static_cast<cudaStream_t>(stream));
+  E.forward(*d, static_cast<cudaStream_t>(stream));
   API_END
 }
 
@@ -157,105 +153,6 @@ int i2it_encode_text(i2it_handle* h, const int32_t* tokens, int batch, void* out
   API_BEGIN(h)
   E.check_device_error();
   E.encode_text(reinterpret_cast<const int*>(tokens), batch, out, static_cast<cudaStream_t>(stream));
-  API_END
-}
-
-int i2it_forward_u8(i2it_handle* h, const void* x_u8_hwc, int in_mode, const void* text_emb, int text_batch, const void* eps,
-                    const void* noise_map, float r, void* out_u8_hwc, void* out_latent, int batch, int H, int W, int direction,
-                    void* stream) {
-  API_BEGIN(h)
-  I2IT_CHECK(in_mode >= 0 && in_mode <= 2, "i2it_forward_u8: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
-  I2IT_CHECK(x_u8_hwc && out_u8_hwc, "i2it_forward_u8: null image pointer");
-  IO io;
-  std::memset(&io, 0, sizeof io);
-  io.x_u8 = x_u8_hwc; io.in_mode = in_mode; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r;
-  io.out_u8 = out_u8_hwc; io.out_latent = out_latent;
-  E.check_device_error();
-  E.forward(io, batch, H, W, direction, text_batch, static_cast<cudaStream_t>(stream));
-  API_END
-}
-
-int i2it_forward_u8_resize(i2it_handle* h, const void* x_u8_hwc, int in_mode, const i2it_resize_desc* g, const void* text_emb,
-                           int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc, void* out_latent,
-                           int batch, int H, int W, int direction, void* stream) {
-  API_BEGIN(h)
-  I2IT_CHECK(in_mode >= 0 && in_mode <= 2, "i2it_forward_u8_resize: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
-  I2IT_CHECK(x_u8_hwc && out_u8_hwc && g, "i2it_forward_u8_resize: null image pointer or geometry");
-  IO io;
-  std::memset(&io, 0, sizeof io);
-  io.x_u8 = x_u8_hwc; io.in_mode = in_mode; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r;
-  io.out_u8 = out_u8_hwc; io.out_latent = out_latent;
-  E.check_device_error();
-  E.forward(io, batch, H, W, direction, text_batch, static_cast<cudaStream_t>(stream), g);
-  API_END
-}
-
-int i2it_forward_variations(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps,
-                            const void* noise_map, float r, void* out, void* out_latent, int n, int H, int W, int direction,
-                            void* stream) {
-  API_BEGIN(h)
-  I2IT_CHECK(n >= 1, "i2it_forward_variations: n must be >= 1");
-  IO io;
-  std::memset(&io, 0, sizeof io);
-  io.x = x; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r; io.out = out; io.out_latent = out_latent;
-  E.check_device_error();
-  E.forward(io, n, H, W, direction, text_batch, static_cast<cudaStream_t>(stream), nullptr, /*shared_input=*/true);
-  API_END
-}
-
-int i2it_forward_u8_variations(i2it_handle* h, const void* x_u8_hwc, int in_mode, const i2it_resize_desc* g, const void* text_emb,
-                               int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc,
-                               void* out_latent, int n, int H, int W, int direction, void* stream) {
-  API_BEGIN(h)
-  I2IT_CHECK(n >= 1, "i2it_forward_u8_variations: n must be >= 1");
-  I2IT_CHECK(in_mode >= 0 && in_mode <= 2, "i2it_forward_u8_variations: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
-  I2IT_CHECK(x_u8_hwc && out_u8_hwc, "i2it_forward_u8_variations: null image pointer");
-  IO io;
-  std::memset(&io, 0, sizeof io);
-  io.x_u8 = x_u8_hwc; io.in_mode = in_mode; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r;
-  io.out_u8 = out_u8_hwc; io.out_latent = out_latent;
-  E.check_device_error();
-  E.forward(io, n, H, W, direction, text_batch, static_cast<cudaStream_t>(stream), g, /*shared_input=*/true);
-  API_END
-}
-
-int i2it_forward_u8_ragged(i2it_handle* h, const void* const* x_u8, int in_mode, const i2it_resize_desc* g, int max_side,
-                           const void* text_emb, int text_batch, const void* eps, const void* noise_map, float r,
-                           void* const* out_u8, void* out_latent, int n, int H, int W, int direction, void* stream) {
-  API_BEGIN(h)
-  I2IT_CHECK(n >= 1, "i2it_forward_u8_ragged: n must be >= 1");
-  I2IT_CHECK(in_mode >= 0 && in_mode <= 2, "i2it_forward_u8_ragged: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
-  IO io;
-  std::memset(&io, 0, sizeof io);
-  io.in_mode = in_mode; io.text = text_emb; io.eps = eps; io.noise = noise_map; io.r = r; io.out_latent = out_latent;
-  E.check_device_error();
-  E.forward_ragged(io, x_u8, out_u8, g, max_side, n, H, W, direction, text_batch, static_cast<cudaStream_t>(stream));
-  API_END
-}
-
-int i2it_forward_mixed(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps, void* out,
-                       void* out_latent, int batch, int H, int W, const int* directions, void* stream) {
-  API_BEGIN(h)
-  IO io;
-  std::memset(&io, 0, sizeof io);
-  io.x = x; io.text = text_emb; io.eps = eps; io.out = out; io.out_latent = out_latent;
-  E.check_device_error();
-  E.forward_mixed(io, directions, batch, H, W, text_batch, static_cast<cudaStream_t>(stream));
-  API_END
-}
-
-int i2it_forward_u8_ragged_mixed(i2it_handle* h, const void* const* x_u8, int in_mode, const i2it_resize_desc* g, int max_side,
-                                 const void* text_emb, int text_batch, const void* eps, void* const* out_u8, void* out_latent,
-                                 int n, int H, int W, const int* directions, void* stream) {
-  API_BEGIN(h)
-  I2IT_CHECK(n >= 1, "i2it_forward_u8_ragged_mixed: n must be >= 1");
-  I2IT_CHECK(in_mode >= 0 && in_mode <= 2, "i2it_forward_u8_ragged_mixed: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
-  E.check_mixed(directions, n, H, W);
-  IO io;
-  std::memset(&io, 0, sizeof io);
-  io.in_mode = in_mode; io.text = text_emb; io.eps = eps; io.out_latent = out_latent;
-  E.check_device_error();
-  E.forward_ragged(io, x_u8, out_u8, g, max_side, n, H, W, I2IT_A2B, text_batch, static_cast<cudaStream_t>(stream), directions);
   API_END
 }
 

@@ -1985,33 +1985,52 @@ bool Engine::check_forward(int B, int H, int W, int text_batch, const void* text
   return true;
 }
 
-void Engine::forward(const IO& io_in, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
-                     const i2it_resize_desc* g, bool shared_input) {
-  const bool text_cached = check_forward(B, H, W, text_batch, io_in.text);
-  IO io = io_in;
-  // one variation of one image is the plain batch-1 forward: same plan, same output
-  const int io_mode = (io.x_u8 ? IO_U8_IN : 0) | (io.out_u8 ? IO_U8_OUT : 0) | (shared_input && B > 1 ? IO_SHARED_IN : 0);
-  I2IT_CHECK((io.x || io.x_u8) && io.eps && (io.out || io.out_u8), "null input/output pointer");
-  if (g) {
-    I2IT_CHECK(io.x_u8 && io.out_u8, "a resize geometry needs the uint8 boundary");
-    rs_check_geometry(*g, H, W);
-    // nothing to resize or crop: the plan (and its key) of the plain uint8 forward
-    if (g->in_H == H && g->in_W == W && g->resize_H == H && g->resize_W == W && g->out_H == H && g->out_W == W) g = nullptr;
+void Engine::forward(const i2it_forward_desc& d, cudaStream_t st) {
+  const int B = d.batch, H = d.H, W = d.W;
+  const i2it_resize_desc* g = d.geometry;
+  const bool u8 = d.x_u8 || d.out_u8, ragged = d.x_u8_list || d.out_u8_list, mixed = d.directions != nullptr;
+  // the requests include/i2it.h lists; every other combination is refused before its operands are looked at
+  I2IT_CHECK((d.x || d.out) + u8 + ragged <= 1,
+             "i2it_forward: one image boundary per request: x / out, x_u8 / out_u8 or x_u8_list / out_u8_list");
+  I2IT_CHECK(!g || u8 || ragged, "i2it_forward: a resize geometry needs a uint8 input (x_u8 or x_u8_list), not the NCHW x");
+  I2IT_CHECK(!(d.shared_input && ragged), "i2it_forward: shared_input (variations of one image) with a ragged x_u8_list");
+  I2IT_CHECK(!(mixed && d.shared_input), "mixed-direction forward: directions with shared_input (variations of one image)");
+  I2IT_CHECK(!(mixed && u8), "mixed-direction forward: directions with the uint8 x_u8 (a mixed uint8 batch is a ragged x_u8_list)");
+  I2IT_CHECK(!(mixed && d.noise_map), "mixed-direction forward: directions with a noise_map (CycleGAN has none)");
+  I2IT_CHECK(mixed || d.direction == I2IT_A2B || d.direction == I2IT_B2A,
+             "i2it_forward: direction " + std::to_string(d.direction) + " is neither I2IT_A2B (0) nor I2IT_B2A (1)");
+  I2IT_CHECK(B >= 1, "i2it_forward: batch size n must be >= 1");
+  if (u8 || ragged)
+    I2IT_CHECK(d.in_mode >= 0 && d.in_mode <= 2, "i2it_forward: in_mode must be I2IT_IN_UNIT, I2IT_IN_NORMALIZE or I2IT_IN_SKETCH");
+  int direction = d.direction;
+  if (mixed) { check_mixed(d.directions, B, H, W); direction = DIR_MIXED; }
+  const bool text_cached = check_forward(B, H, W, d.text_batch, d.text_emb);
+  IO io;
+  std::memset(&io, 0, sizeof io);
+  io.text = d.text_emb; io.eps = d.eps; io.noise = d.noise_map; io.r = d.r; io.out_latent = d.out_latent;
+  if (u8 || ragged) io.in_mode = d.in_mode;
+  if (!ragged) {
+    io.x = d.x; io.x_u8 = d.x_u8; io.out = d.out; io.out_u8 = d.out_u8;
+    I2IT_CHECK((io.x || io.x_u8) && io.eps && (io.out || io.out_u8), "null input/output pointer");
+    if (g) {
+      rs_check_geometry(*g, H, W);
+      // nothing to resize or crop: the plan (and its key) of the plain uint8 forward
+      if (g->in_H == H && g->in_W == W && g->resize_H == H && g->resize_W == W && g->out_H == H && g->out_W == W) g = nullptr;
+    }
+    // one variation of one image is the plain batch-1 forward: same plan, same output
+    const int io_mode = (u8 ? IO_U8_IN | IO_U8_OUT : 0) | (d.shared_input && B > 1 ? IO_SHARED_IN : 0);
+    Plan* P = plan_for(B, H, W, direction, d.text_batch, text_cached, io_mode, g, /*evict=*/false);
+    if (u8) io.out = P->u8_out_tmp;
+    run(P, io, st, mixed ? stage_dirs(P, d.directions, B) : nullptr);
+    return;
   }
-  Plan* P = plan_for(B, H, W, direction, text_batch, text_cached, io_mode, g, /*evict=*/false);
-  if (io_mode & IO_U8_OUT) io.out = P->u8_out_tmp;
-  run(P, io, st);
-}
-
-void Engine::forward_ragged(const IO& io_in, const void* const* x, void* const* out, const i2it_resize_desc* g, int max_side,
-                            int B, int H, int W, int direction, int text_batch, cudaStream_t st, const int* dirs) {
-  if (dirs) { check_mixed(dirs, B, H, W); direction = DIR_MIXED; }
-  const bool text_cached = check_forward(B, H, W, text_batch, io_in.text);
+  const void* const* x = d.x_u8_list;
+  void* const* out = d.out_u8_list;
   I2IT_CHECK(x && out && g, "ragged forward: null image or geometry array");
-  rs_check_ragged(g, B, H, W, max_side);      // before the pointers: an empty output (a zero size) has a null one
+  rs_check_ragged(g, B, H, W, d.max_side);    // before the pointers: an empty output (a zero size) has a null one
   for (int i = 0; i < B; ++i)
     I2IT_CHECK(x[i] && out[i], "ragged forward: null image pointer (image " + std::to_string(i) + ")");
-  I2IT_CHECK(io_in.eps, "null input/output pointer");
+  I2IT_CHECK(io.eps, "null input/output pointer");
   // the tables first: a size pair the table builder refuses fails here, before a plan is built or anything is enqueued
   for (int i = 0; i < B; ++i) {
     const int pairs[4][2] = {{g[i].in_H, g[i].resize_H}, {g[i].in_W, g[i].resize_W}, {H, g[i].out_H}, {W, g[i].out_W}};
@@ -2019,17 +2038,15 @@ void Engine::forward_ragged(const IO& io_in, const void* const* x, void* const* 
       if (pr[0] != pr[1]) rs_tables_.get(pr[0], pr[1]);
   }
   // the images live in the descriptors, not in the launches: the graph cache key holds no image pointer
-  IO io = io_in;
-  io.x_u8 = nullptr; io.out_u8 = nullptr;
-  Plan* P = plan_for(B, H, W, direction, text_batch, text_cached, IO_U8_IN | IO_U8_OUT | IO_RAGGED, nullptr, /*evict=*/false,
-                     max_side);
+  Plan* P = plan_for(B, H, W, direction, d.text_batch, text_cached, IO_U8_IN | IO_U8_OUT | IO_RAGGED, nullptr, /*evict=*/false,
+                     d.max_side);
   io.out = P->u8_out_tmp;
-  const RsCall c = rs_forward_call(g, B, H, W, max_side, rs_tables_, x, out, &P->rg);
+  const RsCall c = rs_forward_call(g, B, H, W, d.max_side, rs_tables_, x, out, &P->rg);
   for (int k = 0; k < 4; ++k) P->meta[P->rg.ops[k]].bytes = c.bytes[k];   // i2it_profile: this call's geometries
   const size_t bytes = stage_ragged(c, P->rg.dev_bytes);
   char* dev = P->rg.dev;
   const char* blob = rs_blob_;
-  const std::function<void(cudaStream_t)> dir_copy = dirs ? stage_dirs(P, dirs, B) : nullptr;
+  const std::function<void(cudaStream_t)> dir_copy = mixed ? stage_dirs(P, d.directions, B) : nullptr;
   run(P, io, st, [=](cudaStream_t s) {
     I2IT_CUDA(cudaMemcpyAsync(dev, blob, bytes, cudaMemcpyHostToDevice, s));
     I2IT_CUDA(cudaEventRecord(rs_ev_, s));
@@ -2064,8 +2081,6 @@ std::string mixed_size_rule(int H, int W) {
 
 void Engine::check_mixed(const int* dirs, int B, int H, int W) const {
   I2IT_CHECK(cfg.model_kind == I2IT_CYCLEGAN, "mixed-direction forward: a pix2pix handle has one VAE; directions are CycleGAN's");
-  I2IT_CHECK(dirs != nullptr, "mixed-direction forward: null direction array");
-  I2IT_CHECK(B >= 1, "mixed-direction forward: batch must be >= 1");
   for (int i = 0; i < B; ++i)
     I2IT_CHECK(dirs[i] == I2IT_A2B || dirs[i] == I2IT_B2A, "mixed-direction forward: direction " + std::to_string(dirs[i]) +
                                                                 " of image " + std::to_string(i) + " is neither I2IT_A2B (0) nor I2IT_B2A (1)");
@@ -2091,14 +2106,6 @@ std::function<void(cudaStream_t)> Engine::stage_dirs(Plan* P, const int* dirs, i
     I2IT_CUDA(cudaMemcpyAsync(dev, blob, static_cast<size_t>(B) * sizeof(int), cudaMemcpyHostToDevice, s));
     I2IT_CUDA(cudaEventRecord(ev, s));
   };
-}
-
-void Engine::forward_mixed(const IO& io, const int* dirs, int B, int H, int W, int text_batch, cudaStream_t st) {
-  check_mixed(dirs, B, H, W);
-  const bool text_cached = check_forward(B, H, W, text_batch, io.text);
-  I2IT_CHECK(io.x && io.eps && io.out, "null input/output pointer");
-  Plan* P = plan_for(B, H, W, DIR_MIXED, text_batch, text_cached, 0, nullptr, /*evict=*/false);
-  run(P, io, st, stage_dirs(P, dirs, B));
 }
 
 size_t Engine::stage_ragged(const RsCall& c, size_t cap) {

@@ -134,13 +134,13 @@ struct NormW {
 struct IO {
   const void* x = nullptr; const void* text = nullptr; const void* eps = nullptr; const void* noise = nullptr;
   float r = 1.f; void* out = nullptr; void* out_latent = nullptr;
-  const void* x_u8 = nullptr; void* out_u8 = nullptr;   // uint8 HWC boundary (i2it_forward_u8): x / out then point at internal buffers
+  const void* x_u8 = nullptr; void* out_u8 = nullptr;   // uint8 HWC boundary (x_u8 / out_u8 requests): out then points at an internal buffer
   int in_mode = 0;                                      // u8 input transform (see pack_input_im2col_u8_kernel)
   int pad_ = 0;
   bool operator==(const IO& o) const { return std::memcmp(this, &o, sizeof(IO)) == 0; }
 };
 // IO_SHARED_IN: a variations forward, one input image for the whole batch (its encoder runs at batch 1)
-// IO_RAGGED: uint8 images of their own sizes, each resized to and from the one network size (i2it_forward_u8_ragged)
+// IO_RAGGED: uint8 images of their own sizes, each resized to and from the one network size (x_u8_list requests)
 enum IoMode : int { IO_U8_IN = 1, IO_U8_OUT = 2, IO_SHARED_IN = 4, IO_RAGGED = 8 };
 // the plan-key direction of a mixed-direction CycleGAN plan (I2IT_A2B = 0 and I2IT_B2A = 1 are the single-direction ones)
 constexpr int DIR_MIXED = 2;
@@ -285,21 +285,16 @@ class Engine {
   // i2it_refold_weights: rewrite, in place, the prepared weights whose fold inputs changed since the last fold
   void refold(float lw_unet, float lw_vae, float skip_gamma, float twin_r);
   std::string refold_info_json() const;                               // i2it_debug_refold_info
-  // g: LANCZOS resize geometry of a uint8 forward (i2it_forward_u8_resize); part of the plan key
+  // g: LANCZOS resize geometry of a uint8 forward; part of the plan key
   // evict: enforce the plan limit once the plan is in (forward() does it itself after the plan becomes the last-run one)
   // max_side: the capacity of an IO_RAGGED plan (part of its key)
   Plan* plan_for(int B, int H, int W, int direction, int text_batch, bool text_cached = false, int io_mode = 0,
                  const i2it_resize_desc* g = nullptr, bool evict = true, int max_side = 0);
-  // shared_input: x / x_u8 hold ONE image that all B outputs start from (i2it_forward_variations); B == 1 is the plain forward
-  void forward(const IO& io, int B, int H, int W, int direction, int text_batch, cudaStream_t st,
-               const i2it_resize_desc* g = nullptr, bool shared_input = false);
-  // B images of their own sizes (x[i], out[i], g[i]) through one IO_RAGGED plan of capacity max_side on an H x W network
-  void forward_ragged(const IO& io, const void* const* x, void* const* out, const i2it_resize_desc* g, int max_side, int B,
-                      int H, int W, int direction, int text_batch, cudaStream_t st, const int* dirs = nullptr);
-  // mixed-direction CycleGAN forward: image i through vae (dirs[i] == I2IT_A2B) or vae_b2a (I2IT_B2A), one plan for every mix
-  void forward_mixed(const IO& io, const int* dirs, int B, int H, int W, int text_batch, cudaStream_t st);
-  // rejects, with a message, what a mixed forward refuses before building anything: a pix2pix handle, a direction array
-  // that is null or holds a value other than 0 / 1, and a size whose VAE tiles would hold rows of two images
+  // one image forward (i2it_forward): refuses every request include/i2it.h does not list, then runs check_mixed (a mixed
+  // request), check_forward and the operand checks, all before a plan is built
+  void forward(const i2it_forward_desc& d, cudaStream_t st);
+  // rejects, with a message, what a mixed forward refuses before building anything: a pix2pix handle, a direction other
+  // than 0 / 1, and a size whose VAE tiles would hold rows of two images
   void check_mixed(const int* dirs, int B, int H, int W) const;
   // the checks every image forward starts with (network size, text batch, a cached text when text is null); returns
   // whether the text is the cached one

@@ -591,12 +591,7 @@ Plan* Engine::plan_for(int B, int H, int W, int direction, int text_batch, bool 
   I2IT_CHECK(finalized_, "i2it_finalize_weights must be called before a forward");
   std::string vp = "vae.";
   if (cfg.model_kind == I2IT_CYCLEGAN && direction == I2IT_B2A) vp = "vae_b2a.";
-  const bool mixed = direction == DIR_MIXED;
-  if (mixed) {
-    I2IT_CHECK(cfg.model_kind == I2IT_CYCLEGAN, "mixed-direction forward: a pix2pix handle has one VAE; directions are CycleGAN's");
-    const std::string why = mixed_size_rule(H, W);
-    I2IT_CHECK(why.empty(), "mixed-direction forward: " + why);
-  }
+  const bool mixed = direction == DIR_MIXED;     // Engine::forward has run check_mixed
   std::unique_ptr<Plan> up(new Plan());
   Plan& P = *up;
   P.key = key;

@@ -19,7 +19,7 @@ F16, BF16, F32 = 0, 1, 2
 PIX2PIX, CYCLEGAN = 0, 1
 A2B, B2A = 0, 1
 ACT_NONE, ACT_CLAMP1, ACT_GEGLU, ACT_GELU, ACT_QUICKGELU = 0, 1, 2, 3, 4   # epilogue activations (tapgemm TgAct)
-IN_UNIT, IN_NORMALIZE, IN_SKETCH = 0, 1, 2      # uint8 input transforms of i2it_forward_u8
+IN_UNIT, IN_NORMALIZE, IN_SKETCH = 0, 1, 2      # uint8 input transforms (ForwardDesc.in_mode)
 
 _TORCH2DT = {torch.float16: F16, torch.bfloat16: BF16, torch.float32: F32}
 _DT2TORCH = {F16: torch.float16, BF16: torch.bfloat16}
@@ -28,15 +28,14 @@ _DT2TORCH = {F16: torch.float16, BF16: torch.bfloat16}
 SYMBOLS = [
     "i2it_default_config", "i2it_create", "i2it_destroy", "i2it_last_error", "i2it_set_weight",
     "i2it_set_adapter_scale", "i2it_finalize_weights", "i2it_workspace_bytes", "i2it_forward",
-    "i2it_set_text", "i2it_encode_text", "i2it_forward_u8", "i2it_prep_launch_count", "i2it_debug_fast_div", "i2it_launch_count", "i2it_profile", "i2it_read_stage", "i2it_op_conv2d", "i2it_op_group_norm", "i2it_op_layer_norm",
+    "i2it_set_text", "i2it_encode_text", "i2it_prep_launch_count", "i2it_debug_fast_div", "i2it_launch_count", "i2it_profile", "i2it_read_stage", "i2it_op_conv2d", "i2it_op_group_norm", "i2it_op_layer_norm",
     "i2it_op_attention", "i2it_op_upsample2x", "i2it_op_conv2d_ex", "i2it_op_launches", "i2it_op_vt_proj",
     "i2it_op_upsample_to", "i2it_stage_names", "i2it_prepared_keys", "i2it_read_prepared", "i2it_text_stage_names",
-    "i2it_forward_u8_resize", "i2it_op_resize_u8", "i2it_debug_resample_coeffs",
+    "i2it_op_resize_u8", "i2it_debug_resample_coeffs",
     "i2it_set_max_plans", "i2it_release_plans", "i2it_memory_stats_get", "i2it_debug_poison_workspace",
-    "i2it_debug_tapgemm_override", "i2it_forward_variations", "i2it_forward_u8_variations",
-    "i2it_forward_u8_ragged", "i2it_op_resize_u8_ragged", "i2it_debug_ragged_tables", "i2it_debug_graph_captures",
+    "i2it_debug_tapgemm_override", "i2it_op_resize_u8_ragged", "i2it_debug_ragged_tables", "i2it_debug_graph_captures",
     "i2it_refold_weights", "i2it_debug_refold_info",
-    "i2it_forward_mixed", "i2it_forward_u8_ragged_mixed", "i2it_mixed_size_check", "i2it_op_conv2d_sel",
+    "i2it_mixed_size_check", "i2it_op_conv2d_sel",
 ]
 TEXT_TOKEN_EMB = "text_encoder.text_model.embeddings.token_embedding.weight"
 TEXT_POS_EMB = "text_encoder.text_model.embeddings.position_embedding.weight"
@@ -71,6 +70,17 @@ class ConvDesc(C.Structure):
 class ResizeDesc(C.Structure):
     """i2it_resize_desc (include/i2it.h); sizes are rows x columns."""
     _fields_ = [(n, C.c_int) for n in ("in_H", "in_W", "resize_H", "resize_W", "crop_y", "crop_x", "out_H", "out_W")]
+
+
+class ForwardDesc(C.Structure):
+    """i2it_forward_desc (include/i2it.h): one image forward; unset fields are zero (unused)."""
+    _fields_ = [
+        ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int), ("direction", C.c_int), ("directions", C.POINTER(C.c_int)),
+        ("shared_input", C.c_int), ("x", C.c_void_p), ("x_u8", C.c_void_p), ("x_u8_list", C.POINTER(C.c_void_p)),
+        ("in_mode", C.c_int), ("geometry", C.POINTER(ResizeDesc)), ("max_side", C.c_int),
+        ("text_emb", C.c_void_p), ("text_batch", C.c_int), ("eps", C.c_void_p), ("noise_map", C.c_void_p), ("r", C.c_float),
+        ("out", C.c_void_p), ("out_u8", C.c_void_p), ("out_u8_list", C.POINTER(C.c_void_p)), ("out_latent", C.c_void_p),
+    ]
 
 
 def resize_geometry(in_hw, resize=None, crop=None, out_size=None):
@@ -174,10 +184,9 @@ def load_library(path: Optional[str] = None):
     lib.i2it_set_adapter_scale.argtypes = [vp, C.c_char_p, cf]
     lib.i2it_finalize_weights.argtypes = [vp, cf, cf, cf, cf]
     lib.i2it_workspace_bytes.argtypes = [vp, ci, ci, ci, C.POINTER(C.c_size_t)]
-    lib.i2it_forward.argtypes = [vp, vp, vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci, vp]
+    lib.i2it_forward.argtypes = [vp, C.POINTER(ForwardDesc), vp]
     lib.i2it_set_text.argtypes = [vp, vp, ci, vp]
     lib.i2it_encode_text.argtypes = [vp, vp, ci, vp, vp]
-    lib.i2it_forward_u8.argtypes = [vp, vp, ci, vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci, vp]
     lib.i2it_prep_launch_count.argtypes = [vp, C.POINTER(ci)]
     lib.i2it_debug_fast_div.argtypes = [C.c_longlong, ci, ci]
     lib.i2it_debug_fast_div.restype = C.c_longlong
@@ -197,7 +206,6 @@ def load_library(path: Optional[str] = None):
     lib.i2it_text_stage_names.argtypes = [vp, C.c_char_p, C.c_size_t]
     lib.i2it_prepared_keys.argtypes = [vp, C.c_char_p, C.c_size_t]
     lib.i2it_read_prepared.argtypes = [vp, C.c_char_p, vp, C.c_size_t, vp, C.c_size_t, C.POINTER(ci)]
-    lib.i2it_forward_u8_resize.argtypes = [vp, vp, ci, C.POINTER(ResizeDesc), vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci, vp]
     lib.i2it_op_resize_u8.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci, vp]
     lib.i2it_debug_resample_coeffs.argtypes = [ci, ci, C.POINTER(ci), C.POINTER(ci), ci]
     lib.i2it_set_max_plans.argtypes = [vp, ci]
@@ -205,20 +213,12 @@ def load_library(path: Optional[str] = None):
     lib.i2it_memory_stats_get.argtypes = [vp, C.POINTER(MemoryStats)]
     lib.i2it_debug_poison_workspace.argtypes = [vp, ci]
     lib.i2it_debug_tapgemm_override.argtypes = [vp, ci, ci, ci]
-    lib.i2it_forward_variations.argtypes = [vp, vp, vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci, vp]
-    lib.i2it_forward_u8_variations.argtypes = [vp, vp, ci, C.POINTER(ResizeDesc), vp, ci, vp, vp, cf, vp, vp, ci, ci, ci, ci,
-                                               vp]
-    lib.i2it_forward_u8_ragged.argtypes = [vp, C.POINTER(vp), ci, C.POINTER(ResizeDesc), ci, vp, ci, vp, vp, cf, C.POINTER(vp),
-                                           vp, ci, ci, ci, ci, vp]
     lib.i2it_op_resize_u8_ragged.argtypes = [vp, C.POINTER(vp), C.POINTER(ci), C.POINTER(vp), C.POINTER(ci), ci, ci, vp]
     lib.i2it_debug_ragged_tables.argtypes = [C.POINTER(ResizeDesc), ci, ci, ci, ci, C.POINTER(C.c_longlong),
                                              C.POINTER(C.c_longlong)]
     lib.i2it_debug_graph_captures.argtypes = [vp, C.POINTER(ci)]
     lib.i2it_refold_weights.argtypes = [vp, cf, cf, cf, cf]
     lib.i2it_debug_refold_info.argtypes = [vp, C.c_char_p, C.c_size_t]
-    lib.i2it_forward_mixed.argtypes = [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, C.POINTER(ci), vp]
-    lib.i2it_forward_u8_ragged_mixed.argtypes = [vp, C.POINTER(vp), ci, C.POINTER(ResizeDesc), ci, vp, ci, vp, C.POINTER(vp), vp,
-                                                 ci, ci, ci, C.POINTER(ci), vp]
     lib.i2it_mixed_size_check.argtypes = [ci, ci, C.c_char_p, C.c_size_t]
     lib.i2it_op_conv2d_sel.argtypes = [vp, C.POINTER(ConvDesc), vp, vp, vp, C.POINTER(ci), vp]
     for name in SYMBOLS:
@@ -394,6 +394,12 @@ class Engine:
             raise ValueError("eps must be [B,4,H/8,W/8]")
         return tb
 
+    def _forward(self, n, H, W, text_emb, tb, eps, out_latent, **fields):
+        """One i2it_forward call on n images (or variations) of an H x W network; `fields` fill the rest of its ForwardDesc."""
+        d = ForwardDesc(batch=n, H=H, W=W, text_emb=_ptr(text_emb), text_batch=tb, eps=_ptr(eps), out_latent=_ptr(out_latent),
+                        **fields)
+        self._check(self.lib.i2it_forward(self._h, C.byref(d), _stream()), "i2it_forward")
+
     def forward(self, x: torch.Tensor, text_emb: Optional[torch.Tensor], eps: torch.Tensor,
                 noise_map: Optional[torch.Tensor] = None, r: float = 1.0, direction: int = A2B,
                 out: Optional[torch.Tensor] = None, out_latent: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -402,9 +408,8 @@ class Engine:
         tb = self._check_operands(B, H, W, text_emb, eps, (x, noise_map, out, out_latent))
         if out is None:
             out = torch.empty_like(x)
-        self._check(self.lib.i2it_forward(self._h, _ptr(x), _ptr(text_emb), tb, _ptr(eps), _ptr(noise_map),
-                                          float(r), _ptr(out), _ptr(out_latent), B, H, W, direction, _stream()),
-                    "i2it_forward")
+        self._forward(B, H, W, text_emb, tb, eps, out_latent, direction=direction, x=_ptr(x), noise_map=_ptr(noise_map),
+                      r=float(r), out=_ptr(out))
         return out
 
     def forward_u8(self, x_u8: torch.Tensor, in_mode: int, text_emb: Optional[torch.Tensor], eps: torch.Tensor,
@@ -418,21 +423,15 @@ class Engine:
         `out_size` (H, W).  eps / noise_map / out_latent then have the crop's size."""
         B, Hi, Wi, Cc = x_u8.shape
         assert Cc == 3 and x_u8.dtype == torch.uint8 and x_u8.is_cuda and x_u8.is_contiguous(), "image must be uint8 CUDA [B,H,W,3]"
-        geom = resize is not None or crop is not None or out_size is not None
         rs, (cy, cx, H, W), osz = resize_geometry((Hi, Wi), resize, crop, out_size)
         tb = self._check_operands(B, H, W, text_emb, eps, (noise_map, out_latent))
         if out is None:
             out = torch.empty(B, osz[0], osz[1], 3, dtype=torch.uint8, device=x_u8.device)
         assert out.dtype == torch.uint8 and out.is_cuda and out.is_contiguous() and out.shape == (B, osz[0], osz[1], 3)
-        if not geom:
-            self._check(self.lib.i2it_forward_u8(self._h, _ptr(x_u8), int(in_mode), _ptr(text_emb), tb, _ptr(eps), _ptr(noise_map),
-                                                 float(r), _ptr(out), _ptr(out_latent), B, H, W, direction, _stream()),
-                        "i2it_forward_u8")
-            return out
-        d = ResizeDesc(Hi, Wi, rs[0], rs[1], cy, cx, osz[0], osz[1])
-        self._check(self.lib.i2it_forward_u8_resize(self._h, _ptr(x_u8), int(in_mode), C.byref(d), _ptr(text_emb), tb, _ptr(eps),
-                                                    _ptr(noise_map), float(r), _ptr(out), _ptr(out_latent), B, H, W, direction,
-                                                    _stream()), "i2it_forward_u8_resize")
+        # without resize / crop / out_size this is the identity geometry, which runs the plan of the plain uint8 forward
+        g = ResizeDesc(Hi, Wi, rs[0], rs[1], cy, cx, osz[0], osz[1])
+        self._forward(B, H, W, text_emb, tb, eps, out_latent, direction=direction, x_u8=_ptr(x_u8), in_mode=int(in_mode),
+                      geometry=C.pointer(g), noise_map=_ptr(noise_map), r=float(r), out_u8=_ptr(out))
         return out
 
     def forward_variations(self, x1: torch.Tensor, text_emb: Optional[torch.Tensor], eps: torch.Tensor,
@@ -447,9 +446,8 @@ class Engine:
         tb = self._check_operands(n, H, W, text_emb, eps, (x1, noise_map, out, out_latent))
         if out is None:
             out = torch.empty(n, 3, H, W, device=x1.device, dtype=x1.dtype)
-        self._check(self.lib.i2it_forward_variations(self._h, _ptr(x1), _ptr(text_emb), tb, _ptr(eps), _ptr(noise_map),
-                                                     float(r), _ptr(out), _ptr(out_latent), n, H, W, direction, _stream()),
-                    "i2it_forward_variations")
+        self._forward(n, H, W, text_emb, tb, eps, out_latent, direction=direction, shared_input=1, x=_ptr(x1),
+                      noise_map=_ptr(noise_map), r=float(r), out=_ptr(out))
         return out
 
     def forward_u8_variations(self, x_u8_1: torch.Tensor, in_mode: int, text_emb: Optional[torch.Tensor], eps: torch.Tensor,
@@ -469,10 +467,9 @@ class Engine:
         if out is None:
             out = torch.empty(n, osz[0], osz[1], 3, dtype=torch.uint8, device=x_u8_1.device)
         assert out.dtype == torch.uint8 and out.is_cuda and out.is_contiguous() and out.shape == (n, osz[0], osz[1], 3)
-        d = ResizeDesc(Hi, Wi, rs[0], rs[1], cy, cx, osz[0], osz[1])
-        self._check(self.lib.i2it_forward_u8_variations(self._h, _ptr(x_u8_1), int(in_mode), C.byref(d), _ptr(text_emb), tb,
-                                                        _ptr(eps), _ptr(noise_map), float(r), _ptr(out), _ptr(out_latent), n,
-                                                        H, W, direction, _stream()), "i2it_forward_u8_variations")
+        g = ResizeDesc(Hi, Wi, rs[0], rs[1], cy, cx, osz[0], osz[1])
+        self._forward(n, H, W, text_emb, tb, eps, out_latent, direction=direction, shared_input=1, x_u8=_ptr(x_u8_1),
+                      in_mode=int(in_mode), geometry=C.pointer(g), noise_map=_ptr(noise_map), r=float(r), out_u8=_ptr(out))
         return out
 
     def forward_u8_ragged(self, images: Sequence[torch.Tensor], in_mode: int, text_emb: Optional[torch.Tensor],
@@ -486,28 +483,13 @@ class Engine:
 
         max_side: the plan's capacity, at least every in / resize / out dimension; None takes ragged_max_side of the call's
         dimensions, so a stream of calls with the same n reuses one plan and one graph."""
-        n = len(images)
-        _check_u8_images(images, "forward_u8_ragged")
-        H, W, descs = _ragged_descs(geometries, [tuple(x.shape[:2]) for x in images])
-        if eps.shape[0] != n:
-            raise ValueError(f"{n} images but eps has batch {eps.shape[0]}")
-        tb = self._check_operands(n, H, W, text_emb, eps, (noise_map, out_latent))
-        if max_side is None:
-            max_side = ragged_max_side([v for d in descs for v in (d.in_H, d.in_W, d.resize_H, d.resize_W, d.out_H, d.out_W)])
-        if outs is None:
-            outs = [torch.empty(d.out_H, d.out_W, 3, dtype=torch.uint8, device=images[0].device) for d in descs]
-        if len(outs) != n or any(tuple(o.shape) != (d.out_H, d.out_W, 3) or o.dtype != torch.uint8 or not o.is_cuda
-                                 or not o.is_contiguous() for o, d in zip(outs, descs)):
-            raise ValueError("outs must be n contiguous uint8 CUDA tensors [out_H_i, out_W_i, 3]")
-        self._check(self.lib.i2it_forward_u8_ragged(self._h, _ptrs(images), int(in_mode), descs, int(max_side), _ptr(text_emb), tb,
-                                                    _ptr(eps), _ptr(noise_map), float(r), _ptrs(outs), _ptr(out_latent), n, H,
-                                                    W, direction, _stream()), "i2it_forward_u8_ragged")
-        return list(outs)
+        return self._forward_u8_ragged("forward_u8_ragged", images, in_mode, text_emb, eps, geometries, max_side, outs,
+                                       out_latent, noise_map=noise_map, r=r, direction=direction)
 
     def forward_mixed(self, x: torch.Tensor, text_emb: Optional[torch.Tensor], eps: torch.Tensor, directions,
                       out: Optional[torch.Tensor] = None, out_latent: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """CycleGAN forward of a batch that mixes both directions (i2it_forward_mixed): image i through vae (directions[i] ==
-        A2B) or vae_b2a (B2A).  Output i equals image i of forward(..., direction=directions[i]) byte for byte; one plan and
+        """CycleGAN forward of a batch that mixes both directions (ForwardDesc.directions): image i through vae (directions[i]
+        == A2B) or vae_b2a (B2A).  Output i equals image i of forward(..., direction=directions[i]) byte for byte; one plan and
         one CUDA graph serve every mix.  A refused size raises ValueError with the engine's rule (mixed_size_check)."""
         B, Cc, H, W = x.shape
         assert Cc == 3, "image must be [B,3,H,W]"
@@ -518,25 +500,31 @@ class Engine:
         tb = self._check_operands(B, H, W, text_emb, eps, (x, out, out_latent))
         if out is None:
             out = torch.empty_like(x)
-        self._check(self.lib.i2it_forward_mixed(self._h, _ptr(x), _ptr(text_emb), tb, _ptr(eps), _ptr(out), _ptr(out_latent),
-                                                B, H, W, dirs, _stream()), "i2it_forward_mixed")
+        self._forward(B, H, W, text_emb, tb, eps, out_latent, directions=dirs, x=_ptr(x), out=_ptr(out))
         return out
 
     def forward_u8_ragged_mixed(self, images: Sequence[torch.Tensor], in_mode: int, text_emb: Optional[torch.Tensor],
                                 eps: torch.Tensor, directions, *, geometries, max_side: Optional[int] = None,
                                 outs: Optional[Sequence[torch.Tensor]] = None, out_latent: Optional[torch.Tensor] = None):
-        """forward_u8_ragged with a direction per image (i2it_forward_u8_ragged_mixed): uploads of any size, both directions,
+        """forward_u8_ragged with a direction per image (ForwardDesc.directions): uploads of any size, both directions,
         one plan.  Output i equals forward_u8(images[i][None], ..., direction=directions[i], **geometries[i]) byte for byte."""
+        return self._forward_u8_ragged("forward_u8_ragged_mixed", images, in_mode, text_emb, eps, geometries, max_side, outs,
+                                       out_latent, directions=directions)
+
+    def _forward_u8_ragged(self, what, images, in_mode, text_emb, eps, geometries, max_side, outs, out_latent, *,
+                           noise_map=None, r=0.0, direction=A2B, directions=None):
+        """The body of forward_u8_ragged and forward_u8_ragged_mixed (directions given: a mixed batch, which has no noise_map)."""
         n = len(images)
-        _check_u8_images(images, "forward_u8_ragged_mixed")
-        dirs = directions_array(directions, n)
+        _check_u8_images(images, what)
+        dirs = directions_array(directions, n) if directions is not None else None
         H, W, descs = _ragged_descs(geometries, [tuple(x.shape[:2]) for x in images])
-        why = mixed_size_check(H, W)
-        if why:
-            raise ValueError("mixed-direction forward: " + why)
+        if dirs is not None:
+            why = mixed_size_check(H, W)
+            if why:
+                raise ValueError("mixed-direction forward: " + why)
         if eps.shape[0] != n:
             raise ValueError(f"{n} images but eps has batch {eps.shape[0]}")
-        tb = self._check_operands(n, H, W, text_emb, eps, (out_latent,))
+        tb = self._check_operands(n, H, W, text_emb, eps, (noise_map, out_latent))
         if max_side is None:
             max_side = ragged_max_side([v for d in descs for v in (d.in_H, d.in_W, d.resize_H, d.resize_W, d.out_H, d.out_W)])
         if outs is None:
@@ -544,9 +532,9 @@ class Engine:
         if len(outs) != n or any(tuple(o.shape) != (d.out_H, d.out_W, 3) or o.dtype != torch.uint8 or not o.is_cuda
                                  or not o.is_contiguous() for o, d in zip(outs, descs)):
             raise ValueError("outs must be n contiguous uint8 CUDA tensors [out_H_i, out_W_i, 3]")
-        self._check(self.lib.i2it_forward_u8_ragged_mixed(self._h, _ptrs(images), int(in_mode), descs, int(max_side),
-                                                          _ptr(text_emb), tb, _ptr(eps), _ptrs(outs), _ptr(out_latent), n, H, W,
-                                                          dirs, _stream()), "i2it_forward_u8_ragged_mixed")
+        self._forward(n, H, W, text_emb, tb, eps, out_latent, direction=direction, directions=dirs, x_u8_list=_ptrs(images),
+                      in_mode=int(in_mode), geometry=descs, max_side=int(max_side), noise_map=_ptr(noise_map), r=float(r),
+                      out_u8_list=_ptrs(outs))
         return list(outs)
 
     def graph_captures(self) -> int:

@@ -34,7 +34,7 @@ typedef struct i2it_handle i2it_handle;
 enum { I2IT_F16 = 0, I2IT_BF16 = 1, I2IT_F32 = 2 };
 enum { I2IT_PIX2PIX = 0, I2IT_CYCLEGAN = 1 };
 enum { I2IT_A2B = 0, I2IT_B2A = 1 };
-/* uint8 input transforms of i2it_forward_u8 (what the reference CLIs do on the host before the forward) */
+/* uint8 input transforms of a uint8 forward (what the reference CLIs do on the host before the forward) */
 enum { I2IT_IN_UNIT = 0,        /* F.to_tensor(img): u8/255                       src/inference_paired.py:50      */
        I2IT_IN_NORMALIZE = 1,   /* ToTensor + Normalize([0.5],[0.5])              src/inference_unpaired.py:45-47 */
        I2IT_IN_SKETCH = 2 };    /* (F.to_tensor(img) < 0.5).float()               src/inference_paired.py:56-57   */
@@ -131,7 +131,36 @@ int i2it_memory_stats_get(i2it_handle* h, i2it_memory_stats* s);
  * write itself, so poisoning between forwards must leave every output unchanged. */
 int i2it_debug_poison_workspace(i2it_handle* h, int value);
 
-/* The fused hot path.  All pointers are DEVICE pointers in the handle dtype, NCHW contiguous:
+/* LANCZOS resize geometry of a uint8 forward (i2it_forward_desc.geometry): what the reference CLIs do with PIL on the host
+ * around the forward (src/inference_unpaired.py:40-45,53; src/inference_paired.py:38-41), bit-exact with
+ * Image.resize(size, Image.LANCZOS).  The caller's image [batch, in_H, in_W, 3] is resized to resize_H x resize_W; the network
+ * runs on the H x W window at (crop_y, crop_x) of it (transforms.CenterCrop); its output image is resized to out_H x out_W.
+ * All sizes are rows x columns. */
+typedef struct i2it_resize_desc {
+  int in_H, in_W;
+  int resize_H, resize_W;
+  int crop_y, crop_x;
+  int out_H, out_W;
+} i2it_resize_desc;
+
+/* One image forward (i2it_forward).  Plain fields; zero (or NULL) means unused.  The accepted requests, by which input,
+ * geometry, shared_input and directions they set (the output pointer matches the input: out, out_u8 or out_u8_list):
+ *
+ *   request              input              geometry                 shared_input   directions
+ *   plain                x                  NULL                     0              NULL
+ *   uint8                x_u8               NULL                     0              NULL
+ *   uint8 resize         x_u8               one                      0              NULL
+ *   variations           x [1]              NULL                     1              NULL
+ *   uint8 variations     x_u8 [1]           one or NULL              1              NULL
+ *   ragged               x_u8_list          batch, with max_side     0              NULL
+ *   mixed                x                  NULL                     0              host array, no noise_map
+ *   ragged mixed         x_u8_list          batch, with max_side     0              host array, no noise_map
+ *
+ * Every other combination is rejected before any launch and without building a plan: two inputs or outputs of different
+ * kinds, a geometry on the NCHW x, shared_input with x_u8_list or with directions, directions with x_u8, and a noise_map
+ * with directions.
+ *
+ * Plain.  All pointers are DEVICE pointers in the handle dtype, NCHW contiguous:
  *   x        [batch, 3, H, W]          control image / input image (fed to the VAE as is)
  *   text_emb [text_batch, 77, cross]   CLIP hidden states (text_batch is 1 or batch)
  *   eps      [batch, 4, H/8, W/8]      the posterior noise of latent_dist.sample()
@@ -149,10 +178,88 @@ int i2it_debug_poison_workspace(i2it_handle* h, int value);
  * The transient workspace of all of a handle's forward plans is one shared arena, sized by the largest resident plan;
  * each plan also holds a few small persistent buffers of its own.  Plans stay until i2it_finalize_weights,
  * i2it_release_plans or an eviction under i2it_set_max_plans; an evicted plan is rebuilt, bit-identically, when its key
- * returns.  `stream` is a cudaStream_t. */
-int i2it_forward(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps,
-                 const void* noise_map, float r, void* out, void* out_latent, int batch, int H, int W,
-                 int direction, void* stream);
+ * returns.
+ *
+ * uint8.  The plain forward with a uint8 HWC boundary: x_u8 [batch, H, W, 3] and out_u8 [batch, H, W, 3] are device
+ * pointers.  Input transform `in_mode` (I2IT_IN_*) and the output `ToPILImage()(out*0.5+0.5)` (src/inference_paired.py:72,
+ * src/inference_unpaired.py:53; three activation-dtype roundings then truncation to uint8) are fused into the first /
+ * a trailing kernel, so a caller moves 3 bytes per pixel each way instead of 2 x 3 x sizeof(half).
+ *
+ * uint8 resize.  The uint8 forward with a resize geometry: x_u8 [batch, in_H, in_W, 3] -> out_u8 [batch, out_H, out_W, 3]
+ * (device pointers); eps / noise_map / out_latent have the network size H x W (multiples of 8).  Each resize is one or two
+ * launches (horizontal pass if the width changes, then vertical if the height changes; none for an unchanged size), captured
+ * in the same CUDA graph; the coefficient tables are computed on the host once per plan.  The geometry is part of the plan
+ * key.  Rejected before any launch: non-positive sizes, or a crop window outside the resized image.
+ *
+ * Variations.  n = batch variations of ONE image in one forward: the plain forward with x [1, 3, H, W] and every other
+ * operand at batch n (eps [n, 4, H/8, W/8], noise_map [n, 4, H/8, W/8] or NULL, out [n, 3, H, W], out_latent [n, 4, H/8, W/8]
+ * or NULL, text_emb [text_batch, 77, cross] with text_batch 1 or n, or NULL for the i2it_set_text cache).  The VAE encoder
+ * runs once, at batch 1: its moments feed every image's posterior sample (each with its own eps and noise_map rows), and
+ * each of its four skips is replicated to batch n right before the decoder conv that reads it.  Output image i is
+ * bit-identical to image i of the plain forward on the image repeated n times (and to a batch-1 forward of it with eps[i],
+ * noise_map[i]): the encoder of a batch computes each image alone.  A variations key is its own plan (n = 1 is the plain
+ * batch-1 plan).  Rejected before any launch: n < 1, text_batch not 1 or n, and whatever the plain forward rejects.
+ * Replaces the one-forward-per-seed loop of gradio_sketch2image.py.
+ *
+ * uint8 variations.  Variations with the uint8 HWC boundary of the uint8 / uint8 resize forwards: x_u8 [1, in_H, in_W, 3]
+ * -> out_u8 [n, out_H, out_W, 3].  geometry is one resize geometry or NULL (then in_H = out_H = H, in_W = out_W = W); the
+ * input resize passes and packing run at batch 1, the output conversion and resize at batch n.  Rejected before any launch:
+ * what the variations and uint8 resize forwards reject.
+ *
+ * Ragged.  n = batch uint8 images of their own sizes through one forward at batch n on an H x W network:
+ *   x_u8_list[i]   [geometry[i].in_H, geometry[i].in_W, 3]    device pointers, one per image
+ *   out_u8_list[i] [geometry[i].out_H, geometry[i].out_W, 3]  device pointers, one per image
+ *   geometry[i]    image i's resize geometry (its crop window is H x W)
+ *   eps / noise_map / out_latent [n, 4, H/8, W/8], text_emb [text_batch, 77, cross] or NULL, as in the uint8 forward.
+ * Each image goes through exactly the passes of the uint8 resize forward, so output i is byte-equal to a batch-1
+ * uint8 resize forward of image i with eps[i] and noise_map[i].  A dimension that does not change is an identity pass,
+ * so every call makes two resize launches per side.
+ * The plan is keyed by (n, H, W, direction, text mode, max_side) and by no image size: max_side is a capacity that
+ * every in_*, resize_* and out_* size of the call must not exceed, and its buffers are sized by it.  Each call
+ * builds its descriptors and coefficient tables on the host (tables cached per size pair) and copies them to the plan with
+ * one asynchronous copy ahead of the first launch.  The image pointers live in those descriptors, not in the captured
+ * graph, so any mix of sizes and pointers replays one graph.
+ * Rejected before any launch: n < 1, a NULL array or image pointer, non-positive sizes, a crop window outside its resized
+ * image, a dimension above max_side (or max_side <= 0), and whatever the uint8 forward rejects.
+ *
+ * Mixed.  A CycleGAN batch that mixes both directions in one forward: image i goes through vae (directions[i] == I2IT_A2B)
+ * or vae_b2a (I2IT_B2A).  directions is a HOST array of batch values; every other operand is the plain forward's (there is
+ * no noise_map: CycleGAN has none), with text_batch 1 or batch and text_emb NULL for the i2it_set_text cache.  The UNet, the
+ * DDPM step and the latent sampling are the same for both directions; every VAE launch that reads weights (the convs,
+ * quant_conv / post_quant_conv, the attention's projections and the GroupNorm applies) takes each 128-row tile's or each
+ * image's weights from its direction, in the same accumulation order, so output image i is byte-equal to image i of a
+ * single-direction forward in directions[i] (same x, eps, text).  One plan per (batch, H, W, text mode) serves every
+ * mix: the directions are copied to the plan ahead of the first launch, and its CUDA graph reads them there.  It has the
+ * launch count and tile geometry of the single-direction plan.
+ * Accepted sizes: those whose every VAE tile holds rows of one image (i2it_mixed_size_check), e.g. 256x256, 512x512,
+ * 512x768 and 1024x1024; 1280x720 is refused (its (H/8)(W/8) = 14400 latent pixels are not a multiple of 128).
+ * Rejected before any launch, and without building a plan: a pix2pix handle, a NULL directions array, a value other
+ * than 0 or 1, a refused size, and whatever the plain forward rejects.
+ *
+ * Ragged mixed.  The ragged forward with a direction per image (host array of n values, as the mixed forward): uploads of
+ * any size and both directions through one plan.  Output i is byte-equal to the batch-1 uint8 resize forward of upload i in
+ * directions[i].  Rejected before any launch: what the ragged and mixed forwards reject. */
+typedef struct i2it_forward_desc {
+  int batch, H, W;
+  int direction;                       /* I2IT_A2B | I2IT_B2A (other values are refused); unused with directions */
+  const int* directions;               /* host array of batch directions (mixed requests), or NULL */
+  int shared_input;                    /* 1: variations of one input image */
+  const void* x;                       /* NCHW input in the handle dtype */
+  const void* x_u8;                    /* uint8 HWC input */
+  const void* const* x_u8_list;        /* batch uint8 HWC inputs (ragged requests) */
+  int in_mode;                         /* I2IT_IN_* of a uint8 input */
+  const i2it_resize_desc* geometry;    /* NULL, one geometry, or batch geometries (ragged requests) */
+  int max_side;                        /* capacity of a ragged plan */
+  const void* text_emb; int text_batch;
+  const void* eps; const void* noise_map; float r;
+  void* out;                           /* NCHW output in the handle dtype */
+  void* out_u8;                        /* uint8 HWC output */
+  void* const* out_u8_list;            /* batch uint8 HWC outputs (ragged requests) */
+  void* out_latent;
+} i2it_forward_desc;
+
+/* The fused hot path: run the forward `d` describes on `stream` (a cudaStream_t). */
+int i2it_forward(i2it_handle* h, const i2it_forward_desc* d, void* stream);
 
 /* Project and cache the cross-attention operands of a prompt: K = to_k(text_emb), V^T = to_v(text_emb)^T for every
  * transformer block (32 small launches, enqueued on `stream`).  text_emb [text_batch, 77, cross] device pointer in the
@@ -169,97 +276,6 @@ int i2it_set_text(i2it_handle* h, const void* text_emb, int text_batch, void* st
  * The kernels read batch * 77 ids and write batch * 77 rows: the caller owns both sizes, and every id must lie in
  * [0, vocab) (the Python binding checks both before the launch). */
 int i2it_encode_text(i2it_handle* h, const int32_t* tokens, int batch, void* out, void* stream);
-
-/* i2it_forward with a uint8 HWC boundary: x_u8_hwc [batch, H, W, 3] and out_u8_hwc [batch, H, W, 3] are device pointers.
- * Input transform `in_mode` (I2IT_IN_*) and the output `ToPILImage()(out*0.5+0.5)` (src/inference_paired.py:72,
- * src/inference_unpaired.py:53; three activation-dtype roundings then truncation to uint8) are fused into the first /
- * a trailing kernel, so a caller moves 3 bytes per pixel each way instead of 2 x 3 x sizeof(half). */
-int i2it_forward_u8(i2it_handle* h, const void* x_u8_hwc, int in_mode, const void* text_emb, int text_batch,
-                    const void* eps, const void* noise_map, float r, void* out_u8_hwc, void* out_latent, int batch,
-                    int H, int W, int direction, void* stream);
-
-/* LANCZOS resize geometry of i2it_forward_u8_resize: what the reference CLIs do with PIL on the host around the forward
- * (src/inference_unpaired.py:40-45,53; src/inference_paired.py:38-41), bit-exact with Image.resize(size, Image.LANCZOS).
- * The caller's image [batch, in_H, in_W, 3] is resized to resize_H x resize_W; the network runs on the H x W window at
- * (crop_y, crop_x) of it (transforms.CenterCrop); its output image is resized to out_H x out_W.  All sizes are rows x columns. */
-typedef struct i2it_resize_desc {
-  int in_H, in_W;
-  int resize_H, resize_W;
-  int crop_y, crop_x;
-  int out_H, out_W;
-} i2it_resize_desc;
-
-/* i2it_forward_u8 with a resize geometry: x_u8_hwc [batch, in_H, in_W, 3] -> out_u8_hwc [batch, out_H, out_W, 3] (device
- * pointers); eps / noise_map / out_latent have the network size H x W (multiples of 8).  Each resize is one or two launches
- * (horizontal pass if the width changes, then vertical if the height changes; none for an unchanged size), captured in the
- * same CUDA graph; the coefficient tables are computed on the host once per plan.  The geometry is part of the plan key.
- * Rejected before any launch: non-positive sizes, or a crop window outside the resized image. */
-int i2it_forward_u8_resize(i2it_handle* h, const void* x_u8_hwc, int in_mode, const i2it_resize_desc* g, const void* text_emb,
-                           int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc, void* out_latent,
-                           int batch, int H, int W, int direction, void* stream);
-
-/* n variations of ONE image in one forward: i2it_forward with x [1, 3, H, W] and every other operand at batch n
- * (eps [n, 4, H/8, W/8], noise_map [n, 4, H/8, W/8] or NULL, out [n, 3, H, W], out_latent [n, 4, H/8, W/8] or NULL,
- * text_emb [text_batch, 77, cross] with text_batch 1 or n, or NULL for the i2it_set_text cache).  The VAE encoder runs once, at
- * batch 1: its moments feed every image's posterior sample (each with its own eps and noise_map rows), and each of its four
- * skips is replicated to batch n right before the decoder conv that reads it.  Output image i is bit-identical to image i of
- * i2it_forward on the image repeated n times (and to a batch-1 forward of it with eps[i], noise_map[i]): the encoder of a
- * batch computes each image alone.  A variations key is its own plan (n = 1 is the plain batch-1 plan).  Rejected before any
- * launch: n < 1, text_batch not 1 or n, and whatever i2it_forward rejects.  Replaces the one-forward-per-seed loop of
- * gradio_sketch2image.py. */
-int i2it_forward_variations(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps,
-                            const void* noise_map, float r, void* out, void* out_latent, int n, int H, int W, int direction,
-                            void* stream);
-
-/* i2it_forward_variations with the uint8 HWC boundary of i2it_forward_u8 / i2it_forward_u8_resize: x_u8_hwc [1, in_H, in_W, 3]
- * -> out_u8_hwc [n, out_H, out_W, 3].  g is a resize geometry or NULL (then in_H = out_H = H, in_W = out_W = W); the input
- * resize passes and packing run at batch 1, the output conversion and resize at batch n.  Rejected before any launch: what
- * i2it_forward_variations and i2it_forward_u8_resize reject. */
-int i2it_forward_u8_variations(i2it_handle* h, const void* x_u8_hwc, int in_mode, const i2it_resize_desc* g, const void* text_emb,
-                               int text_batch, const void* eps, const void* noise_map, float r, void* out_u8_hwc,
-                               void* out_latent, int n, int H, int W, int direction, void* stream);
-
-/* n uint8 images of their own sizes through one forward at batch n on an H x W network:
- *   x_u8[i]   [g[i].in_H, g[i].in_W, 3]    device pointers, one per image
- *   out_u8[i] [g[i].out_H, g[i].out_W, 3]  device pointers, one per image
- *   g[i]      image i's resize geometry (i2it_resize_desc; its crop window is H x W)
- *   eps / noise_map / out_latent [n, 4, H/8, W/8], text_emb [text_batch, 77, cross] or NULL, as in i2it_forward_u8.
- * Each image goes through exactly the passes of i2it_forward_u8_resize, so output i is byte-equal to a batch-1
- * i2it_forward_u8_resize of image i with eps[i] and noise_map[i].  A dimension that does not change is an identity pass,
- * so every call makes two resize launches per side.
- * The plan is keyed by (n, H, W, direction, text mode, max_side) and by no image size: max_side is a capacity that
- * every in_*, resize_* and out_* size of the call must not exceed, and its buffers are sized by it.  Each call
- * builds its descriptors and coefficient tables on the host (tables cached per size pair) and copies them to the plan with
- * one asynchronous copy ahead of the first launch.  The image pointers live in those descriptors, not in the captured
- * graph, so any mix of sizes and pointers replays one graph.
- * Rejected before any launch: n < 1, a NULL array or image pointer, non-positive sizes, a crop window outside its resized
- * image, a dimension above max_side (or max_side <= 0), and whatever i2it_forward_u8 rejects. */
-int i2it_forward_u8_ragged(i2it_handle* h, const void* const* x_u8, int in_mode, const i2it_resize_desc* g, int max_side,
-                           const void* text_emb, int text_batch, const void* eps, const void* noise_map, float r,
-                           void* const* out_u8, void* out_latent, int n, int H, int W, int direction, void* stream);
-
-/* A CycleGAN batch that mixes both directions in one forward: image i goes through vae (directions[i] == I2IT_A2B) or
- * vae_b2a (I2IT_B2A).  directions is a HOST array of batch values; every other operand is i2it_forward's (there is no
- * noise_map: CycleGAN has none), with text_batch 1 or batch and text_emb NULL for the i2it_set_text cache.  The UNet, the
- * DDPM step and the latent sampling are the same for both directions; every VAE launch that reads weights (the convs,
- * quant_conv / post_quant_conv, the attention's projections and the GroupNorm applies) takes each 128-row tile's or each
- * image's weights from its direction, in the same accumulation order, so output image i is byte-equal to image i of a
- * single-direction i2it_forward in directions[i] (same x, eps, text).  One plan per (batch, H, W, text mode) serves every
- * mix: the directions are copied to the plan ahead of the first launch, and its CUDA graph reads them there.  It has the
- * launch count and tile geometry of the single-direction plan.
- * Accepted sizes: those whose every VAE tile holds rows of one image (i2it_mixed_size_check), e.g. 256x256, 512x512,
- * 512x768 and 1024x1024; 1280x720 is refused (its (H/8)(W/8) = 14400 latent pixels are not a multiple of 128).
- * Rejected before any launch, and without building a plan: a pix2pix handle, a NULL directions array, a value other
- * than 0 or 1, a refused size, and whatever i2it_forward rejects. */
-int i2it_forward_mixed(i2it_handle* h, const void* x, const void* text_emb, int text_batch, const void* eps, void* out,
-                       void* out_latent, int batch, int H, int W, const int* directions, void* stream);
-
-/* i2it_forward_u8_ragged with a direction per image (host array of n values, as i2it_forward_mixed): uploads of any size
- * and both directions through one plan.  Output i is byte-equal to the batch-1 i2it_forward_u8_resize of upload i in
- * directions[i].  Rejected before any launch: what i2it_forward_u8_ragged and i2it_forward_mixed reject. */
-int i2it_forward_u8_ragged_mixed(i2it_handle* h, const void* const* x_u8, int in_mode, const i2it_resize_desc* g, int max_side,
-                                 const void* text_emb, int text_batch, const void* eps, void* const* out_u8, void* out_latent,
-                                 int n, int H, int W, const int* directions, void* stream);
 
 /* Whether a mixed-direction forward accepts the network size H x W: 0 if it does, 1 if not, with the reason (naming the
  * rule) in msg (cap bytes, NUL-terminated; msg may be NULL).  The rule: (H/8)(W/8) is a multiple of 128 (the VAE
@@ -286,7 +302,7 @@ long long i2it_debug_fast_div(long long max_dividend, int d, int x);
  * No GPU needed. */
 int i2it_debug_resample_coeffs(int in_size, int out_size, int* bounds, int* coeffs, int cap);
 
-/* Host-side sizing of a ragged forward (i2it_forward_u8_ragged) on n geometries: *used = coefficient-table ints the call
+/* Host-side sizing of a ragged forward (i2it_forward_desc) on n geometries: *used = coefficient-table ints the call
  * uploads, *bound = the ints its plan reserves for any call with this n, H, W and max_side.  Returns -1 for a geometry the
  * forward would reject.  No GPU needed. */
 int i2it_debug_ragged_tables(const i2it_resize_desc* g, int n, int H, int W, int max_side, long long* used, long long* bound);
@@ -381,10 +397,10 @@ int i2it_op_upsample2x(i2it_handle* h, const void* x, int N, int H, int W, int C
 int i2it_op_upsample_to(i2it_handle* h, const void* x, int N, int H, int W, int C, int Ho, int Wo, void* out,
                         void* stream);
 /* LANCZOS resize of uint8 HWC images, bit-exact with PIL: x [B, H, W, 3] -> out [B, H2, W2, 3] (device pointers).
- * The same passes as i2it_forward_u8_resize; an unchanged size is a device copy (no launch). */
+ * The same passes as a uint8 resize forward; an unchanged size is a device copy (no launch). */
 int i2it_op_resize_u8(i2it_handle* h, const void* x, int B, int H, int W, void* out, int H2, int W2, void* stream);
 /* Ragged LANCZOS resize, bit-exact with PIL per image: x[i] [hw_in[2i], hw_in[2i+1], 3] -> out[i] [hw_out[2i],
- * hw_out[2i+1], 3] (device pointers).  Two launches, the passes of i2it_forward_u8_ragged; every dimension must be <= max_side.
+ * hw_out[2i+1], 3] (device pointers).  Two launches, the passes of a ragged forward; every dimension must be <= max_side.
  * Rejected before any launch: n < 1, NULL pointers, non-positive sizes, a dimension above max_side. */
 int i2it_op_resize_u8_ragged(i2it_handle* h, const void* const* x, const int* hw_in, void* const* out, const int* hw_out,
                              int n, int max_side, void* stream);

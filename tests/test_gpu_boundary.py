@@ -121,7 +121,7 @@ def test_weight_prep_is_a_handful_of_launches():
 
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
 def test_uint8_boundary_matches_host_pre_and_post_processing(dt):
-    """i2it_forward_u8 == torchvision-style host pre-processing -> i2it_forward -> ToPILImage()(out*0.5+0.5), bit for bit, for the
+    """The uint8 forward == torchvision-style host pre-processing -> i2it_forward -> ToPILImage()(out*0.5+0.5), bit for bit, for the
     three input transforms of the reference CLIs (src/inference_paired.py:50,56-57,72; src/inference_unpaired.py:45-47,53)."""
     import i2it
     import weights as W

@@ -1,6 +1,6 @@
-"""-m gpu: CycleGAN batches that mix both directions in one forward (i2it_forward_mixed / i2it_forward_u8_ragged_mixed /
-i2it_op_conv2d_sel).  Each image takes its own direction's prepared VAE weights in the same accumulation order, so every
-comparison with a single-direction forward is BYTE FOR BYTE; the selecting op is also checked against float64."""
+"""-m gpu: CycleGAN batches that mix both directions in one forward (i2it_forward with directions / i2it_op_conv2d_sel).
+Each image takes its own direction's prepared VAE weights in the same accumulation order, so every comparison with a
+single-direction forward is BYTE FOR BYTE; the selecting op is also checked against float64."""
 import ctypes as C
 
 import pytest
@@ -149,27 +149,63 @@ def _refused(e, fn, msg):
     assert e.memory_stats()["plan_builds"] == s0 and e.graph_captures() == g0
 
 
-def test_refusals(tiny, tiny_sd):
+def test_mixed_refusals(tiny, tiny_sd):
     import i2it
     import weights as W
     e, cfg = tiny
-    null = C.c_void_p(0)
     st = i2it._stream()
 
     def call(eng, H, W_, dirs):
-        return lambda: eng.lib.i2it_forward_mixed(eng._h, null, null, 1, null, null, null, len(dirs), H, W_,
-                                                  (C.c_int * len(dirs))(*dirs), st)
+        d = i2it.ForwardDesc(batch=len(dirs), H=H, W=W_, text_batch=1, directions=(C.c_int * len(dirs))(*dirs))
+        return lambda: eng.lib.i2it_forward(eng._h, C.byref(d), st)
     _refused(e, call(e, 720, 1280, [0, 1]), "multiple of 128")
     _refused(e, call(e, 32, 256, [0, 1]), "tile box")
     _refused(e, call(e, 128, 128, [0, 2]), "direction 2 of image 1")
-    _refused(e, lambda: e.lib.i2it_forward_mixed(e._h, null, null, 1, null, null, null, 2, 128, 128, None, st),
-             "null direction array")
+    # without a direction array the request has one direction, A2B or B2A
+    one = i2it.ForwardDesc(batch=2, H=128, W=128, direction=2, text_batch=1)
+    _refused(e, lambda: e.lib.i2it_forward(e._h, C.byref(one), st), "direction 2 is neither I2IT_A2B (0) nor I2IT_B2A (1)")
     with pytest.raises(ValueError, match="multiple of 128"):
         x, eps, text = _inputs(2, 720, 1280, cfg["cross_dim"], torch.float16)
         e.forward_mixed(x, text, eps, [0, 1])
     p = _engine("pix2pix", torch.bfloat16, tiny_sd, W.TINY)
     _refused(p, call(p, 128, 128, [0, 1]), "pix2pix handle")
     p.close()
+
+
+REFUSED_REQUESTS = {   # combination -> what the refusal says
+    "directions with x_u8": "directions with the uint8 x_u8",
+    "directions with shared_input": "directions with shared_input",
+    "x_u8_list with shared_input": "shared_input (variations of one image) with a ragged x_u8_list",
+    "geometry with x": "a resize geometry needs a uint8 input",
+    "directions with noise_map": "directions with a noise_map",
+}
+
+
+@pytest.mark.parametrize("case", list(REFUSED_REQUESTS))
+def test_refused_request_shapes(tiny, case):
+    """A combination of i2it_forward_desc fields outside the accepted requests is refused before any launch, without a plan
+    or a graph, although every operand it points at is valid."""
+    import i2it
+    e, cfg = tiny
+    B, H, W = 2, 128, 128
+    x, eps, text = _inputs(B, H, W, cfg["cross_dim"], torch.float16)
+    out, noise = torch.empty_like(x), torch.randn_like(eps)
+    imgs = torch.randint(0, 256, (B, H, W, 3), dtype=torch.uint8).cuda()
+    outs_u8 = torch.empty_like(imgs)
+    geom = (i2it.ResizeDesc * B)(*[i2it.ResizeDesc(H, W, H, W, 0, 0, H, W)] * B)
+    dirs = (C.c_int * B)(0, 1)
+    nchw = dict(x=x.data_ptr(), out=out.data_ptr())
+    fields = {
+        "directions with x_u8": dict(directions=dirs, x_u8=imgs.data_ptr(), in_mode=i2it.IN_NORMALIZE,
+                                     out_u8=outs_u8.data_ptr()),
+        "directions with shared_input": dict(nchw, directions=dirs, shared_input=1),
+        "x_u8_list with shared_input": dict(x_u8_list=i2it._ptrs(list(imgs)), in_mode=i2it.IN_NORMALIZE, geometry=geom,
+                                            max_side=4096, out_u8_list=i2it._ptrs(list(outs_u8)), shared_input=1),
+        "geometry with x": dict(nchw, geometry=geom),
+        "directions with noise_map": dict(nchw, directions=dirs, noise_map=noise.data_ptr(), r=0.5),
+    }[case]
+    d = i2it.ForwardDesc(batch=B, H=H, W=W, text_emb=text.data_ptr(), text_batch=1, eps=eps.data_ptr(), **fields)
+    _refused(e, lambda: e.lib.i2it_forward(e._h, C.byref(d), i2it._stream()), REFUSED_REQUESTS[case])
 
 
 # ------------------------------------------------------------------------------------------ the selecting op

@@ -1,4 +1,4 @@
-"""-m gpu: ragged uint8 batches (i2it_forward_u8_ragged / i2it_op_resize_u8_ragged).  Images of their own sizes share one
+"""-m gpu: ragged uint8 batches (i2it_forward with x_u8_list / i2it_op_resize_u8_ragged).  Images of their own sizes share one
 forward plan and one graph; each goes through the same LANCZOS passes as a batch-1 resize forward, so every case here compares
 BYTE FOR BYTE: the op with PIL, the forward with per-image forward_u8 calls (image i of a batch is computed alone)."""
 import ctypes as C
@@ -193,7 +193,7 @@ def test_profile_and_launch_count(tiny_sd_cyc):
     assert byts[1] > 10 * byts[0]                     # the algorithmic bytes follow the last call's geometries
 
 
-def test_rejections(tiny_sd_cyc):
+def test_ragged_rejections(tiny_sd_cyc):
     """Every rejection comes before any launch, with a message, and leaves the next valid call's output unchanged."""
     import i2it
     import weights as W
@@ -226,9 +226,10 @@ def test_rejections(tiny_sd_cyc):
     # a null image pointer, past the binding
     descs = i2it._ragged_descs(geoms, [(90, 160), (150, 97)])[2]
     outs = [torch.empty_like(y) for y in good]
-    rc = e.lib.i2it_forward_u8_ragged(e._h, (C.c_void_p * 2)(imgs[0].data_ptr(), 0), i2it.IN_NORMALIZE, descs, 4096,
-                                      i2it._ptr(text), 1, i2it._ptr(eps), None, 1.0, i2it._ptrs(outs), None, 2, 64, 64, i2it.A2B,
-                                      i2it._stream())
+    d = i2it.ForwardDesc(batch=2, H=64, W=64, direction=i2it.A2B, x_u8_list=(C.c_void_p * 2)(imgs[0].data_ptr(), 0),
+                         in_mode=i2it.IN_NORMALIZE, geometry=descs, max_side=4096, text_emb=i2it._ptr(text), text_batch=1,
+                         eps=i2it._ptr(eps), r=1.0, out_u8_list=i2it._ptrs(outs))
+    rc = e.lib.i2it_forward(e._h, C.byref(d), i2it._stream())
     assert rc != 0 and "null image pointer" in e.lib.i2it_last_error(e._h).decode()
     again = e.forward_u8_ragged(imgs, i2it.IN_NORMALIZE, text, eps, geometries=geoms)
     for a, b in zip(good, again):

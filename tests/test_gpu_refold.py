@@ -239,8 +239,10 @@ def test_checkpoint_in_place(dt, tiny_sd):
         never.refold(1.0, 1.0, 1.0, -1.0)
 
 
-def test_text_cache_dropped(tiny_sd):
+def test_text_cache_dropped_after_refold(tiny_sd):
     """After a refold text_emb=None raises set_text's error; after set_text the output equals the inline prompt's."""
+    import ctypes as C
+    import i2it
     dt = torch.bfloat16
     op = _ops(dt)
     e = _engine(dt, tiny_sd)
@@ -256,8 +258,9 @@ def test_text_cache_dropped(tiny_sd):
         _fwd(e, op, 1.0, text=None)
     out = torch.empty_like(op["x"])
     ptr = lambda t: t.data_ptr()
-    rc = e.lib.i2it_forward(e._h, ptr(op["x"]), None, 1, ptr(op["eps"]), ptr(op["noise"]), 1.0, ptr(out), None, 1, 64, 64,
-                            0, None)
+    d = i2it.ForwardDesc(batch=1, H=64, W=64, x=ptr(op["x"]), text_batch=1, eps=ptr(op["eps"]), noise_map=ptr(op["noise"]),
+                         r=1.0, out=ptr(out))
+    rc = e.lib.i2it_forward(e._h, C.byref(d), None)
     assert rc != 0 and "call i2it_set_text first" in e.lib.i2it_last_error(e._h).decode()
     e.set_text(op["text"])
     cached, _ = _fwd(e, op, 1.0, text=None)

@@ -1,5 +1,5 @@
 """-m gpu: the LANCZOS resize passes (csrc/resample.cuh) equal PIL's Image.resize(..., Image.LANCZOS) byte for byte, alone
-(i2it_op_resize_u8) and inside the uint8 forward (i2it_forward_u8_resize), where they replace the CLIs' host resizes
+(i2it_op_resize_u8) and inside the uint8 forward (a geometry of i2it_forward), where they replace the CLIs' host resizes
 (src/inference_unpaired.py:40-45,53; src/inference_paired.py:38-41)."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""-m gpu: variations of one image (i2it_forward_variations / i2it_forward_u8_variations).  The VAE encoder runs once at
+"""-m gpu: variations of one image (i2it_forward with shared_input).  The VAE encoder runs once at
 batch 1 and its moments and skips feed n outputs; image i of a batch is bit-identical to its batch-1 forward, so every case
 here compares BIT FOR BIT with the plain forward on the image repeated n times (which the layer audits pin to float64)."""
 import pytest
@@ -195,7 +195,7 @@ def test_arena_sharing_and_eviction(tiny_sd):
     assert (s["plans"], s["plan_builds"], s["plan_evictions"]) == (1, 7, 6), s
 
 
-def test_rejections_keep_the_handle_usable(tiny_sd):
+def test_variations_rejections_keep_the_handle_usable(tiny_sd):
     """n = 0, a text batch that is neither 1 nor n, a batch-2 image and a crop outside the resized image are refused before
     any launch (no plan is built); the handle then runs a variations forward that equals a fresh handle's."""
     import ctypes as C
@@ -211,8 +211,9 @@ def test_rejections_keep_the_handle_usable(tiny_sd):
         e.forward_variations(op["x"], text2, op["eps"])
     out = torch.empty(n, 3, 64, 64, device="cuda", dtype=dt)
     ptr = lambda t: C.c_void_p(t.data_ptr())
-    rc = e.lib.i2it_forward_variations(e._h, ptr(op["x"]), ptr(text2), 2, ptr(op["eps"]), None, 1.0,
-                                       ptr(out), None, n, 64, 64, i2it.A2B, None)
+    d = i2it.ForwardDesc(batch=n, H=64, W=64, direction=i2it.A2B, shared_input=1, x=ptr(op["x"]), text_emb=ptr(text2),
+                         text_batch=2, eps=ptr(op["eps"]), r=1.0, out=ptr(out))
+    rc = e.lib.i2it_forward(e._h, C.byref(d), None)
     assert rc != 0 and b"text_batch" in e.lib.i2it_last_error(e._h)
     with pytest.raises(ValueError, match="one image"):
         e.forward_variations(_rep(op["x"], 2), op["text"], op["eps"])

@@ -1,23 +1,46 @@
-"""CPU: the host side of the mixed-direction CycleGAN forward (i2it_forward_mixed).  The new symbols are exported, the wrappers
-validate direction and caption lists before anything reaches the engine, and the size rule holds at its boundaries."""
+"""CPU: the host side of the mixed-direction CycleGAN forward (i2it_forward with directions).  The new symbols are exported,
+the request descriptors have the C layout, the wrappers validate direction and caption lists before anything reaches the
+engine, and the size rule holds at its boundaries."""
 import ctypes as C
+import os
+import subprocess
 
 import pytest
 
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+NEW_SYMBOLS = ["i2it_mixed_size_check", "i2it_op_conv2d_sel"]
 
-NEW_SYMBOLS = ["i2it_forward_mixed", "i2it_forward_u8_ragged_mixed", "i2it_mixed_size_check", "i2it_op_conv2d_sel"]
 
-
-def test_new_symbols_are_exported_and_typed():
+def test_mixed_symbols_are_exported_and_typed():
     import i2it
     lib = i2it.load_library()
     for s in NEW_SYMBOLS:
         assert s in i2it.SYMBOLS
         fn = getattr(lib, s)
         assert fn.argtypes is not None and fn.restype is C.c_int, s
-    assert len(lib.i2it_forward_mixed.argtypes) == 12
-    assert len(lib.i2it_forward_u8_ragged_mixed.argtypes) == 15
     assert len(lib.i2it_op_conv2d_sel.argtypes) == 7
+
+
+def test_struct_layouts_match_ctypes(tmp_path):
+    """sizeof, and every field's offsetof and size, of the structs include/i2it.h declares, as the host C compiler lays them
+    out, equal the ctypes mirrors'.  A mismatch would hand the library shifted fields without any error."""
+    import i2it
+    structs = {"i2it_forward_desc": i2it.ForwardDesc, "i2it_resize_desc": i2it.ResizeDesc, "i2it_conv_desc": i2it.ConvDesc,
+               "i2it_config": i2it.Config, "i2it_memory_stats": i2it.MemoryStats}
+    lines, want = [], []
+    for name, cls in structs.items():
+        lines.append(f'printf("{name} %zu\\n", sizeof({name}));')
+        want.append(f"{name} {C.sizeof(cls)}")
+        for f, _ in cls._fields_:
+            lines.append(f'printf("{name}.{f} %zu %zu\\n", offsetof({name}, {f}), sizeof((({name}*)0)->{f}));')
+            want.append(f"{name}.{f} {getattr(cls, f).offset} {getattr(cls, f).size}")
+    src = tmp_path / "layout.c"
+    src.write_text("#include <stddef.h>\n#include <stdio.h>\n#include \"i2it.h\"\nint main(void) {\n" + "\n".join(lines) +
+                   "\nreturn 0;\n}\n")
+    exe = tmp_path / "layout"
+    subprocess.run(["cc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
+    got = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split("\n")[:-1]
+    assert got == want
 
 
 @pytest.mark.parametrize("H,W", [(512, 512), (256, 256), (512, 768), (768, 512), (1024, 1024), (128, 128), (64, 128)])

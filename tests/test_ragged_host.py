@@ -1,4 +1,4 @@
-"""CPU: the host side of the ragged uint8 forward (i2it_forward_u8_ragged).  A dimension that does not change is an identity
+"""CPU: the host side of the ragged uint8 forward (i2it_forward with x_u8_list).  A dimension that does not change is an identity
 pass whose bytes equal PIL skipping it; the descriptor tables a call uploads fit the area its plan reserves; the wrappers'
 geometry lists and the default capacity."""
 import numpy as np
