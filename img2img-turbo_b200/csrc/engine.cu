@@ -229,26 +229,20 @@ thread_local PdlState g_pdl;
 // 192, 224 and >= 256 (the model's are 64 and 512); 176, 208 and 240 are refused at plan time.
 #define TG_BN_LEAN(X) X(64) X(128) X(192) X(256)
 #define TG_BN_FULL(X) X(16) X(32) X(48) X(64) X(80) X(96) X(112) X(128) X(160) X(192) X(224) X(256)
-template <typename T> using TgKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TapGemmParams);
-template <typename T> static TgKernel<T> tapgemm_for(bool lean, int bn) {   // nullptr: no such instantiation
-#define TG_CASE_LEAN(n) if (lean && bn == n) return tapgemm_kernel<T, true, n>;
-#define TG_CASE_FULL(n) if (!lean && bn == n) return tapgemm_kernel<T, false, n>;
+// the plain and the selecting kernel of one instantiation (both nullptr: no such instantiation)
+template <typename T> struct TgKernels {
+  void (*plain)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TapGemmParams) = nullptr;
+  void (*sel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TapGemmParams, CUtensorMap, CUtensorMap,
+              TapGemmSel) = nullptr;
+};
+template <typename T> static TgKernels<T> tapgemm_for(bool lean, int bn) {
+#define TG_CASE_LEAN(n) if (lean && bn == n) return {tapgemm_kernel<T, true, n>, tapgemm_sel_kernel<T, true, n>};
+#define TG_CASE_FULL(n) if (!lean && bn == n) return {tapgemm_kernel<T, false, n>, tapgemm_sel_kernel<T, false, n>};
   TG_BN_LEAN(TG_CASE_LEAN)
   TG_BN_FULL(TG_CASE_FULL)
 #undef TG_CASE_LEAN
 #undef TG_CASE_FULL
-  return nullptr;
-}
-template <typename T> using TgSelKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TapGemmParams,
-                                                   CUtensorMap, CUtensorMap, TapGemmSel);
-template <typename T> static TgSelKernel<T> tapgemm_sel_for(bool lean, int bn) {   // the same widths as tapgemm_for
-#define TG_CASE_LEAN(n) if (lean && bn == n) return tapgemm_sel_kernel<T, true, n>;
-#define TG_CASE_FULL(n) if (!lean && bn == n) return tapgemm_sel_kernel<T, false, n>;
-  TG_BN_LEAN(TG_CASE_LEAN)
-  TG_BN_FULL(TG_CASE_FULL)
-#undef TG_CASE_LEAN
-#undef TG_CASE_FULL
-  return nullptr;
+  return {};
 }
 
 Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
@@ -259,14 +253,12 @@ Engine::Engine(const i2it_config& c) : cfg(c), dtype(c.dtype) {
   I2IT_CHECK(prop.major == 9 && prop.minor == 0, "libi2it is built for sm_90a (H100) only; found compute capability " +
                                                   std::to_string(prop.major) + "." + std::to_string(prop.minor));
   num_sms = prop.multiProcessorCount;
+  auto tg_smem = [](auto k) { if (k) I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM)); };
   for (int lean = 0; lean < 2; ++lean)
     for (int bn = 16; bn <= 256; bn += 16) {
-      if (auto k = tapgemm_for<__half>(lean, bn)) I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
-      if (auto k = tapgemm_for<__nv_bfloat16>(lean, bn))
-        I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
-      if (auto k = tapgemm_sel_for<__half>(lean, bn)) I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
-      if (auto k = tapgemm_sel_for<__nv_bfloat16>(lean, bn))
-        I2IT_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM));
+      const auto h = tapgemm_for<__half>(lean, bn);
+      const auto b = tapgemm_for<__nv_bfloat16>(lean, bn);
+      tg_smem(h.plain); tg_smem(h.sel); tg_smem(b.plain); tg_smem(b.sel);
     }
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
   I2IT_CUDA(cudaFuncSetAttribute(flash_attn_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
@@ -1034,7 +1026,7 @@ int Engine::pick_bn(long long m_tiles, int N, int step) const {
 int Engine::plan_bn(const Plan& P, long long m_tiles, int N, int step) const {
   if (!P.debug_tapgemm || dbg_bn == 0) return pick_bn(m_tiles, N, step);
   const int hi = round_up(N, 16);
-  if (tapgemm_for<__half>(false, dbg_bn) == nullptr || dbg_bn > hi) {
+  if (tapgemm_for<__half>(false, dbg_bn).plain == nullptr || dbg_bn > hi) {
     std::string legal;
 #define TG_LIST(n) if (n <= hi) legal += (legal.empty() ? "" : ", ") + std::to_string(n);
     TG_BN_FULL(TG_LIST)
@@ -1153,28 +1145,30 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
     p.gn_shift = 0;
     while ((1 << p.gn_shift) < p.gn_red) ++p.gn_shift;
   }
-  I2IT_CHECK(tapgemm_for<__half>(lean, p.BN) != nullptr, "tapgemm: no kernel instantiated for BN=" + std::to_string(p.BN));
+  I2IT_CHECK(tapgemm_for<__half>(lean, p.BN).plain != nullptr, "tapgemm: no kernel instantiated for BN=" + std::to_string(p.BN));
+  // a selecting launch (tapgemm_sel_kernel) also takes the alternative maps and TapGemmSel
+  CUtensorMap tx = tb, tx2 = tb2;
+  TapGemmSel s{};
   if (sel) {
     // the alternative maps have the geometry (and boxes) of the ones they replace; only the base differs
     I2IT_CHECK(p.ksplit <= 1, "tapgemm: a selecting launch cannot split K");
     I2IT_CHECK(sel->s.dir && (sel->s.dim == 0 || sel->s.dim == 2 || sel->s.dim == 3) && sel->s.div >= 1 &&
                (!sel->s.bias == !p.bias), "tapgemm: bad selecting launch");
-    const CUtensorMap tx = encode_tmap(sel->x, dtype), tx2 = sb2p ? encode_tmap(sel->x2, dtype) : tx;
-    TapGemmSel s = sel->s;
+    tx = encode_tmap(sel->x, dtype);
+    tx2 = sb2p ? encode_tmap(sel->x2, dtype) : tx;
+    s = sel->s;
     s.magic = make_magic(static_cast<long long>(p.tdim[s.dim]) + 1, s.div);
     I2IT_CHECK(s.magic != 0, "tapgemm: tile space too large for the division-free image decode");
-    add_op(P, [ta, tb, ta2, tb2, to, p, grid, dt, out_from_io, plan, lean, tx, tx2, s](cudaStream_t st) {
-      TapGemmParams q = p;
-      if (out_from_io) q.out = plan->io.out;
-      DISPATCH_T(dt, (launch_k(tapgemm_sel_for<T>(lean, q.BN), dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q,
-                               tx, tx2, s)));
-    }, kind, 2.0 * m_valid * p.N * k_valid, bytes, shp);
-    return;
   }
-  add_op(P, [ta, tb, ta2, tb2, to, p, grid, dt, out_from_io, plan, lean](cudaStream_t st) {
+  const bool selecting = sel != nullptr;
+  add_op(P, [ta, tb, ta2, tb2, to, p, grid, dt, out_from_io, plan, lean, selecting, tx, tx2, s](cudaStream_t st) {
     TapGemmParams q = p;
     if (out_from_io) q.out = plan->io.out;
-    DISPATCH_T(dt, (launch_k(tapgemm_for<T>(lean, q.BN), dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q)));
+    DISPATCH_T(dt, {
+      const auto k = tapgemm_for<T>(lean, q.BN);
+      if (selecting) launch_k(k.sel, dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q, tx, tx2, s);
+      else launch_k(k.plain, dim3(grid), dim3(TG_THREADS), TG_SMEM, st, 0, ta, tb, ta2, tb2, to, q);
+    });
   }, kind, 2.0 * m_valid * p.N * k_valid, bytes, shp);
 }
 

@@ -403,8 +403,9 @@ class Engine {
     P.meta.push_back(m);
   }
   // encodes the tensor maps and appends the launch
-  // sel: a selecting launch (tapgemm_sel_kernel); x / x2 are the alternative maps of B and the second source's B (of A when
-  // sel->sel_a), and sel's dir / bias / dim / div are set by the caller
+  // sel: a selecting launch (tapgemm_sel_kernel: tapgemm_kernel's body with each tile's weight set chosen by its image); x / x2
+  // are the alternative maps of B and the second source's B (of A when sel->sel_a), and sel's dir / bias / dim / div are set
+  // by the caller
   struct SelSpec { TmapSpec x, x2; TapGemmSel s; };
   void launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemmParams& p, bool out_from_io, const char* kind,
                    double k_valid, double bytes, const TmapSpec* sa2 = nullptr, const TmapSpec* sb2 = nullptr,

@@ -51,7 +51,7 @@ constexpr int TG_ALIGN_PAD = 512;
 constexpr int TG_SMEM = TG_STAGES * (TG_A_STAGE + TG_B_STAGE) + TG_BAR_BYTES + TG_BIAS_BYTES + TG_OSTG_BYTES + TG_ALIGN_PAD;
 // + one producer warpgroup (warp 8 issues the TMA loads, warps 9..11 idle).  Registers are allocated per warpgroup, so the
 // producer warpgroup gives its registers to the consumers (setmaxnreg): 128 x 40 + 256 x 232 <= 64 K.  ptxas honours the
-// two setmaxnreg with each inside its own role's branch (see the role split in tapgemm_kernel).  The kernel is still register-
+// two setmaxnreg with each inside its own role's branch (see the role split in tapgemm_body).  The kernel is still register-
 // allocated within the launch's 168 per thread: ptxas needs the launch bound to honour setmaxnreg (without it: C7508).
 constexpr int TG_THREADS = (TG_EPI_WARPS + 4) * 32;
 constexpr int TG_REGS_PRODUCER = 40, TG_REGS_CONSUMER = 232;
@@ -445,18 +445,13 @@ __device__ __forceinline__ RowCoord row_coord(const TapGemmParams& p, const Tile
 }
 
 // Stage this tile's column-bias slice in smem (zeros where there is none, so the epilogue adds unconditionally); all 256
-// epilogue threads take part.  The slice is double-buffered across tiles (acc = iter & 1).
-__device__ __forceinline__ void stage_bias(const TapGemmParams& p, float* sb, int n0, int warp) {
+// epilogue threads take part.  The slice is double-buffered across tiles (acc = iter & 1).  The bias is p.bias, or with SEL
+// `sel_bias`, the bias of the tile's image's weight set (tapgemm_sel_kernel).
+template <bool SEL>
+__device__ __forceinline__ void stage_bias(const TapGemmParams& p, const float* sel_bias, float* sb, int n0, int warp) {
   for (int cc = warp * 32 + (threadIdx.x & 31); cc < p.BN; cc += TG_EPI_WARPS * 32)
-    sb[cc] = (p.bias_mode == TG_BIAS_COL && n0 + cc < p.N) ? p.bias[n0 + cc] : 0.f;
+    sb[cc] = (p.bias_mode == TG_BIAS_COL && n0 + cc < p.N) ? (SEL ? sel_bias : p.bias)[n0 + cc] : 0.f;
   asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");   // the epilogue warps only
-}
-
-// stage_bias with the tile's bias chosen by the caller (tapgemm_sel_kernel: the bias of the tile's image's weight set)
-__device__ __forceinline__ void stage_bias_from(const TapGemmParams& p, const float* bias, float* sb, int n0, int warp) {
-  for (int cc = warp * 32 + (threadIdx.x & 31); cc < p.BN; cc += TG_EPI_WARPS * 32)
-    sb[cc] = (p.bias_mode == TG_BIAS_COL && n0 + cc < p.N) ? bias[n0 + cc] : 0.f;
-  asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
 }
 
 // TMA-store epilogue, straight from the wgmma fragments (every tma_out launch: no staging tile, so the operand ring stays with
@@ -699,22 +694,20 @@ __device__ __forceinline__ int sel_dir(const TapGemmSel& s, const TileCoord& c) 
   return s.dir[fast_div(v, s.div, s.magic)];
 }
 
-// tapgemm with a weight set chosen per tile by the tile's image (mixed-direction CycleGAN batches; see TapGemmSel).  It is
-// tapgemm_kernel's code with two changes, marked SEL: the map the producer loads each tile's weight stages from, and the
-// bias slice the epilogue stages for the tile.  The ring, the MMA chain, the accumulation order, the GroupNorm slots and
-// the stores are the same.  A copy rather than a shared body: tapgemm_kernel's code (and ptxas's register allocation of
-// it, see layout_pad1) stays exactly as it was.
-template <typename T, bool LEAN, int BN>
-__global__ void __launch_bounds__(TG_THREADS, 1)
-tapgemm_sel_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
-                   const __grid_constant__ CUtensorMap tmO, const __grid_constant__ TapGemmParams p,
-                   const __grid_constant__ CUtensorMap tmXm, const __grid_constant__ CUtensorMap tmX2m,
-                   const __grid_constant__ TapGemmSel selm) {
-  constexpr bool SEL = true;
-  const CUtensorMap* const tmX = &tmXm;
-  const CUtensorMap* const tmX2 = &tmX2m;
-  const TapGemmSel* const sel = &selm;
+// The body of tapgemm_kernel and tapgemm_sel_kernel.  SEL (a weight set chosen per tile by the tile's image: mixed-direction
+// CycleGAN batches, see TapGemmSel) changes three things, each under `if constexpr (SEL)`: the prefetch of the two
+// alternative maps, the map the producer loads each tile's weight stages from, and the bias slice the epilogue stages for the
+// tile.  The ring, the MMA chain, the accumulation order, the GroupNorm slots and the stores are the same.  One body, so an
+// edit to the mainloop, the producer or the epilogue reaches both kernels.  ptxas's allocation of tapgemm_kernel is fragile
+// (see layout_pad1), so the body was checked against the two separate kernels it replaced: `cuobjdump -sass` of every
+// tapgemm_sel_kernel instantiation is identical, and every tapgemm_kernel instantiation differs only in the order of two
+// `UMOV URx, URZ` of the prologue, with the same registers, stack and spills under -Xptxas -v.  Even small changes move
+// that code: a bias pointer argument for the plain path in stage_bias rewrote the LEAN kernels, hence its SEL form.
+// tmX / tmX2 / sel: the selecting launch's operands, nullptr when !SEL.
+template <typename T, bool LEAN, int BN, bool SEL>
+__device__ __forceinline__ void tapgemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmA2,
+                                             const CUtensorMap& tmB2, const CUtensorMap& tmO, const TapGemmParams& p,
+                                             const CUtensorMap* tmX, const CUtensorMap* tmX2, const TapGemmSel* sel) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   if (TG_ALIGN_PAD < 1024 && base - smem_u32(smem_raw) > static_cast<uint32_t>(TG_ALIGN_PAD)) {
@@ -862,9 +855,9 @@ tapgemm_sel_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       const float* sel_bias = nullptr;
       if constexpr (SEL) {
         sel_bias = sel_dir(*sel, c) ? sel->bias : p.bias;
-        stage_bias_from(p, sel_bias, sb, c.nt * BN, warp);   // every tile: the slice changes with the tile's image
+        stage_bias<SEL>(p, sel_bias, sb, c.nt * BN, warp);   // every tile: the slice changes with the tile's image
       } else if (p.n_tiles > 1 || iter < 2) {
-        stage_bias(p, sb, c.nt * BN, warp);
+        stage_bias<SEL>(p, nullptr, sb, c.nt * BN, warp);
       }
       if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 7);
       if (LEAN || p.tma_out) {
@@ -905,173 +898,19 @@ __global__ void __launch_bounds__(TG_THREADS, 1)
 tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
                const __grid_constant__ CUtensorMap tmO, const __grid_constant__ TapGemmParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  if (TG_ALIGN_PAD < 1024 && base - smem_u32(smem_raw) > static_cast<uint32_t>(TG_ALIGN_PAD)) {
-    if (threadIdx.x == 0 && p.err) { atomicExch(p.err, 90); __threadfence_system(); }
-    __trap();
-  }
-  const int NS = p.stages;
-  const uint32_t BST = static_cast<uint32_t>(p.b_stage);
-  const uint32_t sA = base;
-  const uint32_t sB = base + NS * TG_A_STAGE;
-  const uint32_t ostg = base + TG_STAGES * (TG_A_STAGE + TG_B_STAGE);   // epilogue store boxes (1024-byte aligned)
-  const uint32_t ostg2 = ostg - TG_OSTG_BYTES;                          // optional second set: the ring's last 32 KB (p.ostg2)
-  const uint32_t bars = ostg + TG_OSTG_BYTES;
-  auto full_bar = [&](int s) { return bars + 8u * s; };
-  auto empty_bar = [&](int s) { return bars + 8u * (TG_MAX_STAGES + s); };
-  const uint32_t epi_done = bars + 8u * (2 * TG_MAX_STAGES);
-  float* const s_bias = reinterpret_cast<float*>(smem_raw + (bars - smem_u32(smem_raw)) + TG_BAR_BYTES);
+  tapgemm_body<T, LEAN, BN, false>(tmA, tmB, tmA2, tmB2, tmO, p, nullptr, nullptr, nullptr);
+}
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) tg_stamp(p, 0);
-  const int nsplit = p.ksplit > 1 ? p.ksplit : 1;
-  const int total_tiles = p.n_tiles * p.tdim[0] * p.tdim[1] * p.tdim[2] * p.tdim[3] * nsplit;
-  int steps = 0, sec_steps = 0;
-  for (int t = 0; t < p.num_taps; ++t) steps += p.tap_kc[t];
-  for (int t = p.nprim; t < p.num_taps; ++t) sec_steps += p.tap_kc[t];
-
-  if (warp == TG_EPI_WARPS && lane == 0) {
-    for (int s = 0; s < NS; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TG_EPI_WARPS); }
-    mbar_init(epi_done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA2)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB2)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmO)) : "memory");
-  }
-  __syncthreads();
-  pdl_sync();   // prologue (barriers, descriptor prefetch) overlaps the previous kernel's tail; no global access before here
-  if (threadIdx.x == 0) tg_stamp(p, 1);
-
-  // setmaxnreg inside each role's branch: issued by all warps before the role branches, both were ignored (C7507)
-  if (warp >= TG_EPI_WARPS) {
-    reg_dec<TG_REGS_PRODUCER>();
-    if (warp == TG_EPI_WARPS) {             // warps 9..11 only hand their registers to the consumers
-      // ================================ TMA producer (whole warp runs the loop, one elected lane issues) ==========
-      int stage = 0, phase = 0, iter = 0;
-      const uint32_t tx_bytes = TG_A_STAGE + static_cast<uint32_t>(p.BN) * (TG_BK * 2);
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-        const TileCoord c = decode_tile(p, tile);
-        const int a1 = c.t[0] * p.a_mul[0], a2 = c.t[1] * p.a_mul[1], a3 = c.t[2] * p.a_mul[2],
-                  a4 = c.t[3] * p.a_mul[3];
-        const int b2 = c.t[1] * p.b_mul[0], b3 = c.t[2] * p.b_mul[1], b4 = c.t[3] * p.b_mul[2];
-        const int n0 = c.nt * p.BN;
-        // direct-store launches: the ring doubles as the previous tile's accumulator staging tile until its epilogue has read it
-        if (iter > 0 && !p.tma_out) mbar_wait(epi_done, (iter - 1) & 1, p.err, 2);
-        auto load_step = [&](int t, int kc) {
-          const CUtensorMap* ta = p.tap_src[t] ? &tmA2 : &tmA;
-          const CUtensorMap* tb = p.tap_src[t] ? &tmB2 : &tmB;
-          mbar_wait(empty_bar(stage), phase ^ 1, p.err, 1);
-          if (elect_one()) {
-            mbar_expect_tx(full_bar(stage), tx_bytes);
-            tma_load_5d(sA + stage * TG_A_STAGE, ta, full_bar(stage), kc * TG_BK + p.tap_a[t][0],
-                        a1 + p.tap_a[t][1], a2 + p.tap_a[t][2], a3 + p.tap_a[t][3], a4 + p.tap_a[t][4]);
-            tma_load_5d(sB + stage * BST, tb, full_bar(stage), kc * TG_BK + p.tap_b[t][0], n0,
-                        b2 + p.tap_b[t][1], b3 + p.tap_b[t][2], b4 + p.tap_b[t][3]);
-          }
-          __syncwarp();
-          if (++stage == NS) { stage = 0; phase ^= 1; }
-        };
-        const int kc0 = nsplit > 1 ? c.split * p.kc_per : 0, kc1 = nsplit > 1 ? min(p.kchunks, kc0 + p.kc_per) : p.kchunks;
-        for (int kc = kc0; kc < kc1; ++kc)
-          for (int t = 0; t < p.nprim; ++t) load_step(t, kc);
-        if (c.split == 0)
-          for (int t = p.nprim; t < p.num_taps; ++t)
-            for (int kc = 0; kc < p.tap_kc[t]; ++kc) load_step(t, kc);
-        if (tile == static_cast<int>(blockIdx.x) && lane == 0) tg_stamp(p, 2);   // first tile's loads all issued
-      }
-      if (lane == 0) tg_stamp(p, 3);
-    }
-  } else {
-    reg_inc<TG_REGS_CONSUMER>();
-    // ============================ consumers: wgmma mainloop + epilogue (warps 0..7) ============================
-    const int wg = warp >> 2;                    // warpgroup: tile rows [64 wg, 64 wg + 64) in the mainloop
-    const int row = 32 * (warp >> 1) + lane;     // epilogue: tile row described by this lane (quarter warp >> 1)
-    int rr = row;
-    const int j1 = rr % p.box[0]; rr /= p.box[0];
-    const int j2 = rr % p.box[1]; rr /= p.box[1];
-    const int j3 = rr % p.box[2];
-    const int j4 = rr / p.box[2];
-    constexpr int spitch = BN + 4;               // staging row pitch in floats
-    const uint32_t arow = base + static_cast<uint32_t>(row * spitch * 4);
-    // one k-step (one ring stage): four k16 MMAs of the tile's full width; the first of a tile overwrites the accumulators
-    auto mma_stage = [&](float (&accum)[BN / 2], int stage, auto first) {
-      wgmma_fence();
-      const uint32_t a0 = sA + stage * TG_A_STAGE + wg * (64 * 128), b0 = sB + stage * BST;
-#pragma unroll
-      for (int k = 0; k < TG_BK / 16; ++k) {
-        const uint64_t adesc = wgmma_desc_sw128(a0) + 2 * k, bdesc = wgmma_desc_sw128(b0) + 2 * k;
-        if (decltype(first)::value && k == 0) wgmma_ss<BN, false, T>(accum, adesc, bdesc);
-        else wgmma_ss<BN, true, T>(accum, adesc, bdesc);
-      }
-      wgmma_commit();
-    };
-    int stage = 0, phase = 0, iter = 0, rsel = 0;   // rsel: store-box rounds so far (epilogue_frag)
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-      int tsteps = steps;
-      if (nsplit > 1) {                                                         // this tile's share of the K loop
-        const int split = tile / (total_tiles / nsplit);
-        const int kc0 = split * p.kc_per, kc1 = min(p.kchunks, kc0 + p.kc_per);
-        tsteps = (kc1 - kc0) * p.nprim + (split == 0 ? sec_steps : 0);
-      }
-      float accum[BN / 2];                         // live from the tile's first MMA to the staging store only
-      mbar_wait(full_bar(stage), phase, p.err, 3);
-      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 4);                         // first operands landed
-      mma_stage(accum, stage, std::true_type());
-      int prev = stage;
-      if (++stage == NS) { stage = 0; phase ^= 1; }
-      for (int s = 1; s < tsteps; ++s) {
-        mbar_wait(full_bar(stage), phase, p.err, 3);
-        mma_stage(accum, stage, std::false_type());
-        wgmma_wait<1>();                                   // the previous step's MMAs have read their stage
-        if (lane == 0) mbar_arrive(empty_bar(prev));
-        prev = stage;
-        if (++stage == NS) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      if (lane == 0) mbar_arrive(empty_bar(prev));
-      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 5);                        // first tile's MMAs complete
-
-      const TileCoord c = decode_tile(p, tile);
-      const RowCoord rc = row_coord(p, c, j1, j2, j3, j4);
-      float* const sb = s_bias + (iter & 1) * 256;
-      // a launch with a single n-tile stages its one slice into both buffers during the first two tiles and then skips this and
-      // its barrier (110 tiles per CTA in the 512x512 convs)
-      if (p.n_tiles > 1 || iter < 2) stage_bias(p, sb, c.nt * BN, warp);
-      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 7);
-      if (LEAN || p.tma_out) {
-        epilogue_frag<T, LEAN, BN>(p, &tmO, c, fast_div(tile, p.n_tiles, p.magic[0]), accum, warp, rc, sb, ostg, ostg2, rsel,
-                                   iter == 0 && threadIdx.x == 0);
-      } else if constexpr (!LEAN) {
-        // accumulators -> fp32 staging tile (the producer is parked on epi_done, so no load writes the ring meanwhile); the
-        // barrier first: the other warpgroup's last MMAs may still be reading the ring stages the staging tile overlays
-        asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
-        {
-          const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
-#pragma unroll
-          for (int g = 0; g < BN / 8; ++g) {
-            const uint32_t a = base + static_cast<uint32_t>((r0 * spitch + 8 * g + c0) * 4);
-            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(accum[4 * g]), "f"(accum[4 * g + 1]) : "memory");
-            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a + 8 * spitch * 4), "f"(accum[4 * g + 2]),
-                         "f"(accum[4 * g + 3]) : "memory");
-          }
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
-        epilogue_direct<T>(p, c, rc, warp, arow, sb, iter == 0 && threadIdx.x == 0);
-        // staging tile consumed: the ring goes back to the producer (generic reads ordered before the TMA's async writes)
-        fence_async_smem();
-        asm volatile("bar.sync 1, %0;" ::"n"(TG_EPI_WARPS * 32) : "memory");
-        if (threadIdx.x == 0) mbar_arrive(epi_done);
-      }
-      if (iter == 0 && threadIdx.x == 0) tg_stamp(p, 9);                        // first tile stored
-    }
-    if (p.tma_out && lane == 0) bulk_wait_all();      // the store boxes live in this CTA's shared memory
-    if (threadIdx.x == 0) tg_stamp(p, 10);
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) tg_stamp(p, 11);
+// tapgemm with the weight set of each tile chosen by the tile's image (see TapGemmSel): the extra maps and TapGemmSel follow
+// the plain kernel's parameters, so none of those moves
+template <typename T, bool LEAN, int BN>
+__global__ void __launch_bounds__(TG_THREADS, 1)
+tapgemm_sel_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+                   const __grid_constant__ CUtensorMap tmO, const __grid_constant__ TapGemmParams p,
+                   const __grid_constant__ CUtensorMap tmXm, const __grid_constant__ CUtensorMap tmX2m,
+                   const __grid_constant__ TapGemmSel selm) {
+  tapgemm_body<T, LEAN, BN, true>(tmA, tmB, tmA2, tmB2, tmO, p, &tmXm, &tmX2m, &selm);
 }
 
 }  // namespace i2it
