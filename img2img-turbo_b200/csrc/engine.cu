@@ -25,6 +25,21 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+TmapSpec::TmapSpec(const char* what, const void* b, std::initializer_list<long long> dims,
+                   std::initializer_list<long long> strides, std::initializer_list<int> boxes) : base(b) {
+  std::copy(dims.begin(), dims.end(), dim);
+  std::copy(boxes.begin(), boxes.end(), box);
+  int i = 0;
+  for (const long long s : strides) {
+    const uint64_t bytes = 2ull * s;
+    if (dim[i + 1] > 1 && bytes % 16 != 0)
+      throw Error(std::string(what) + ": pitch " + std::to_string(s) + " elements (dimension " + std::to_string(i + 1) +
+                  ") is not a multiple of 8");
+    if (bytes != 0 && bytes % 16 == 0) stride[i] = bytes;
+    ++i;
+  }
+}
+
 static EncodeTiledFn encode_fn() {
   static EncodeTiledFn fn = nullptr;
   if (!fn) {
@@ -1053,8 +1068,6 @@ bool Engine::tma_eligible(const TapGemmParams& p, bool out_from_io) const {
   return true;
 }
 
-static void fill_strides(TmapSpec& s);
-
 void conv_box(bool stride1, int Ho, int Wo, bool nchw, int& tw, int& th, int& tn) {
   if (stride1) tw = (Ho == 1) ? std::min(128, pow2ceil(Wo)) : std::min(nchw ? 32 : 16, pow2ceil(Wo));
   else tw = std::min(16, pow2ceil(Wo));
@@ -1115,21 +1128,16 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
   if (!p.tma_out) p.gn_part = nullptr;
   CUtensorMap to = ta;
   if (p.tma_out) {
-    TmapSpec so;
-    so.base = p.out;
-    so.dim[0] = (p.act == TG_ACT_GEGLU) ? p.N / 2 : p.N;
-    int left = 32;
+    int left = 32, bx[4], ex[4];
     for (int d = 0; d < 4; ++d) {
-      so.dim[d + 1] = static_cast<uint64_t>(std::max(1, p.ext[d]));
-      so.stride[d] = static_cast<uint64_t>(p.ostride[d]) * 2ull;
-      const int sb = std::min(p.box[d], left);
-      so.box[d + 1] = static_cast<uint32_t>(sb);
-      left /= sb;
+      ex[d] = std::max(1, p.ext[d]);
+      bx[d] = std::min(p.box[d], left);
+      left /= bx[d];
     }
     I2IT_CHECK(left == 1, "TMA-store box: the tile's row box does not factor into 32-row warp boxes");
-    so.box[0] = 64;
-    fill_strides(so);
-    to = encode_tmap(so, dtype);
+    to = encode_tmap(TmapSpec("TMA-store output", p.out, {(p.act == TG_ACT_GEGLU) ? p.N / 2 : p.N, ex[0], ex[1], ex[2], ex[3]},
+                              {p.ostride[0], p.ostride[1], p.ostride[2], p.ostride[3]}, {64, bx[0], bx[1], bx[2], bx[3]}),
+                     dtype);
   }
   p.trace = nullptr;
   if (trace_on) {   // diagnostic timeline (I2IT_TRACE=1): 16 clock64 stamps per CTA, dumped to stderr after each forward
@@ -1172,10 +1180,50 @@ void Engine::launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemm
   }, kind, 2.0 * m_valid * p.N * k_valid, bytes, shp);
 }
 
-static void fill_strides(TmapSpec& s) {
-  // size-1 dims still need a legal (16-byte multiple) stride
-  for (int i = 0; i < 4; ++i)
-    if (s.stride[i] == 0 || (s.stride[i] % 16) != 0) s.stride[i] = 16;
+void Engine::launch_rows(Plan& P, const TmapSpec& sa, TmapSpec sb, TapGemmParams p, int M, int heads, int batch, int a_step,
+                         int b_head, int b_img, int N, int K, int bn, const char* kind, double k_valid, double bytes,
+                         const SelSpec* sel) {
+  p.tdim[0] = ceil_div(M, 128); p.tdim[1] = heads; p.tdim[2] = batch; p.tdim[3] = 1;
+  p.box[0] = 128; p.box[1] = 1; p.box[2] = 1; p.box[3] = 1;
+  p.ext[0] = M; p.ext[1] = heads; p.ext[2] = batch; p.ext[3] = 1;
+  p.a_mul[0] = 128; p.a_mul[1] = a_step; p.a_mul[2] = a_step;
+  p.b_mul[0] = b_head; p.b_mul[1] = b_img; p.b_mul[2] = 0;
+  p.N = N;
+  p.BN = bn ? bn : plan_bn(P, 1ll * p.tdim[0] * heads * batch, N, 0);
+  p.n_tiles = ceil_div(N, p.BN);
+  sb.box[0] = 64; sb.box[1] = p.BN;
+  p.num_taps = 1;
+  p.kchunks = ceil_div(K, 64);
+  p.ocol = 1;
+  p.err = d_err;
+  launch_gemm(P, sa, sb, p, false, kind, k_valid, bytes, nullptr, nullptr, sel);
+}
+
+// ---- TMA views of the GEMM operands that more than one launch describes ----
+// NHWC activation as (channel, x, y, image); phase >= 0: every other pixel and row, from parity (phase >> 1, phase & 1)
+static TmapSpec act_view(const char* what, const Act& x, int phase, std::initializer_list<int> box) {
+  const int s = phase >= 0 ? 2 : 1;
+  const long long ld = x.ld, img = x.img();
+  const uint16_t* base = phase >= 0 ? x.p + (static_cast<long long>(phase >> 1) * x.W + (phase & 1)) * ld : x.p;
+  return TmapSpec(what, base, {x.C, x.W / s, x.H / s, x.N}, {s * ld, s * x.W * ld, img, img}, box);
+}
+
+// prepared weight [taps][rows][cin_pad] as (k, row, tap), boxes of 64 x box_rows
+static TmapSpec pw_view(const char* what, const PW& w, int box_rows) {
+  const long long tap = 1ll * w.rows * w.cin_pad, all = tap * w.taps;
+  return TmapSpec(what, w.w, {w.cin_pad, w.rows, w.taps}, {w.cin_pad, tap, all, all}, {64, box_rows});
+}
+
+// head-split Q or K: rows [batch][n][heads * d] with pitch t.ld as (channel, token, head, image)
+static TmapSpec heads_view(const char* what, const Act& t, int d, int n, int heads, int batch, std::initializer_list<int> box) {
+  const long long img = 1ll * n * t.ld;
+  return TmapSpec(what, t.p, {d, n, heads, batch}, {t.ld, d, img, img}, box);
+}
+
+// V^T [kv_batch][heads * d][vt.ld] as (key, channel, head, image)
+static TmapSpec vt_view(const Act& vt, int nk, int d, int heads, int kv_batch, std::initializer_list<int> box) {
+  const long long ld = vt.ld, img = 1ll * heads * d * ld;
+  return TmapSpec("attention V^T", vt.p, {nk, d, heads, kv_batch}, {ld, d * ld, img, img}, box);
 }
 
 Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
@@ -1216,18 +1264,14 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
     out = alloc_act(P, x.N, Ho, Wo, small ? ld : outc, ld, small);
   }
 
-  TmapSpec sa, sb;
+  TmapSpec sa;
   TapGemmParams p;
   std::memset(&p, 0, sizeof p);
   int tw, th, tn;
   const long long ldo = o.to_io_out_nchw ? 0 : out.ld;
   if (o.stride == 1) {
     conv_box(true, x.H, x.W, o.to_io_out_nchw, tw, th, tn);
-    sa.base = x.p;
-    sa.dim[0] = x.C; sa.dim[1] = x.W; sa.dim[2] = x.H; sa.dim[3] = x.N; sa.dim[4] = 1;
-    sa.stride[0] = x.ld * 2ull; sa.stride[1] = 2ull * x.W * x.ld; sa.stride[2] = 2ull * x.H * x.W * x.ld;
-    sa.stride[3] = sa.stride[2];
-    sa.box[0] = 64; sa.box[1] = tw; sa.box[2] = th; sa.box[3] = tn; sa.box[4] = 1;
+    sa = act_view("conv x", x, -1, {64, tw, th, tn});
     p.tdim[0] = ceil_div(x.W, tw); p.tdim[1] = ceil_div(x.H, th); p.tdim[2] = ceil_div(x.N, tn); p.tdim[3] = 1;
     p.box[0] = tw; p.box[1] = th; p.box[2] = tn; p.box[3] = 1;
     p.ext[0] = Wo; p.ext[1] = Ho; p.ext[2] = x.N; p.ext[3] = 1;
@@ -1259,14 +1303,12 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
     I2IT_CHECK(o.stride == 2 && k == 3, "conv: only 3x3 stride-2 is on the path");
     I2IT_CHECK(x.ld % 8 == 0 && x.C % 64 == 0 && x.H % 2 == 0 && x.W % 2 == 0, "conv s2: needs NHWC with ld%8==0, C%64==0, even H/W");
     conv_box(false, Ho, Wo, false, tw, th, tn);
-    const unsigned long long C = x.C, LD = x.ld;
+    const long long LD = x.ld;
     // 5-D view (px*ld + c, xo, py, yo, n) of the NHWC input (pixel pitch ld >= C: the input may be a channel slice of a concat
     // buffer): a stride-2 tap is a plain box in this view.  dim 0 spans the C channels of the even pixel, the gap, and the C
     // channels of the odd pixel; boxes only ever start at c or ld + c with c + 64 <= C.
-    sa.base = x.p;
-    sa.dim[0] = LD + C; sa.dim[1] = Wo; sa.dim[2] = 2; sa.dim[3] = Ho; sa.dim[4] = x.N;
-    sa.stride[0] = 2 * LD * 2; sa.stride[1] = x.W * LD * 2; sa.stride[2] = 2ull * x.W * LD * 2; sa.stride[3] = 1ull * x.H * x.W * LD * 2;
-    sa.box[0] = 64; sa.box[1] = tw; sa.box[2] = 1; sa.box[3] = th; sa.box[4] = tn;
+    sa = TmapSpec("conv x", x.p, {LD + x.C, Wo, 2, Ho, x.N}, {2 * LD, x.W * LD, 2 * x.W * LD, 1ll * x.H * x.W * LD},
+                  {64, tw, 1, th, tn});
     p.tdim[0] = ceil_div(Wo, tw); p.tdim[1] = 1; p.tdim[2] = ceil_div(Ho, th); p.tdim[3] = ceil_div(x.N, tn);
     p.box[0] = tw; p.box[1] = 1; p.box[2] = th; p.box[3] = tn;
     p.ext[0] = Wo; p.ext[1] = 1; p.ext[2] = Ho; p.ext[3] = x.N;
@@ -1285,13 +1327,6 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
     p.ostride[3] = static_cast<long long>(Ho) * Wo * ldo;
     p.kchunks = x.C / 64;
   }
-  fill_strides(sa);
-
-  sb.base = w.w;
-  sb.dim[0] = w.cin_pad; sb.dim[1] = w.rows; sb.dim[2] = w.taps; sb.dim[3] = 1; sb.dim[4] = 1;
-  sb.stride[0] = w.cin_pad * 2ull; sb.stride[1] = 2ull * w.rows * w.cin_pad; sb.stride[2] = 2ull * w.taps * w.rows * w.cin_pad;
-  sb.stride[3] = sb.stride[2];
-  fill_strides(sb);
 
   const long long m_tiles = 1ll * p.tdim[0] * p.tdim[1] * p.tdim[2] * p.tdim[3];
   p.N = gemm_n;
@@ -1302,7 +1337,7 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
     p.BN = plan_bn(P, m_tiles, gemm_n, rounds ? acols : 0);
   }
   p.n_tiles = ceil_div(gemm_n, p.BN);
-  sb.box[0] = 64; sb.box[1] = p.BN; sb.box[2] = 1; sb.box[3] = 1; sb.box[4] = 1;
+  TmapSpec sb = pw_view("conv weight", w, p.BN);
   p.num_taps = taps;
   p.nprim = taps;
   p.ocol = 1;
@@ -1400,23 +1435,8 @@ Act Engine::conv(Plan& P, const Act& x, const PW& w, const ConvOpts& o_in) {
     I2IT_CHECK(o.x2->N == x.N && o.x2->H == sm * Ho && o.x2->W == sm * Wo && (o.x2->C == o.w2->cin || o.x2->C == o.w2->cin_pad),
                "conv: second source shape mismatch");
     I2IT_CHECK(taps + 1 <= TG_MAX_TAPS, "conv: too many taps");
-    sa2 = sa;
-    sa2.base = o.x2->p;
-    sa2.dim[0] = o.x2->C;
-    sa2.stride[0] = o.x2->ld * 2ull; sa2.stride[1] = 2ull * o.x2->W * o.x2->ld; sa2.stride[2] = 2ull * o.x2->H * o.x2->W * o.x2->ld;
-    sa2.stride[3] = sa2.stride[2];
-    if (sub) {
-      const int py = o.subpixel_phase >> 1, px = o.subpixel_phase & 1;
-      sa2.base = o.x2->p + (static_cast<long long>(py) * o.x2->W + px) * o.x2->ld;
-      sa2.stride[0] = 2ull * o.x2->ld * 2; sa2.stride[1] = 2ull * 2 * o.x2->W * o.x2->ld;   // every other pixel / row
-    }
-    fill_strides(sa2);
-    sb2.base = o.w2->w;
-    sb2.dim[0] = o.w2->cin_pad; sb2.dim[1] = o.w2->rows;
-    sb2.stride[0] = o.w2->cin_pad * 2ull; sb2.stride[1] = 2ull * o.w2->rows * o.w2->cin_pad; sb2.stride[2] = sb2.stride[1];
-    sb2.stride[3] = sb2.stride[1];
-    sb2.box[0] = 64; sb2.box[1] = p.BN;
-    fill_strides(sb2);
+    sa2 = act_view("conv x2", *o.x2, o.subpixel_phase, {64, tw, th, tn});
+    sb2 = pw_view("conv w2", *o.w2, p.BN);
     for (int t = 0; t < taps; ++t) { p.tap_src[t] = 0; p.tap_kc[t] = p.kchunks; }
     const int t2 = taps;
     for (int d = 0; d < 5; ++d) p.tap_a[t2][d] = 0;
@@ -1636,45 +1656,23 @@ Act Engine::vt_proj(Plan& P, const Act& x, int B, int ntok, const PW& wv) {
   I2IT_CHECK(x.C == wv.cin || x.C == wv.cin_pad, "vt_proj: width mismatch");
   const int C = wv.rows, ldv = round_up(ntok, 8);
   Act vt = alloc_act(P, B, 1, C, ldv, ldv);      // [B][C rows][ldv]; "C" field carries the padded token count
-  TmapSpec sa, sb;
+  Act tokens = x;                                 // as [B, 1, ntok, C]
+  tokens.N = B; tokens.H = 1; tokens.W = ntok;
+  const TmapSpec sa = pw_view("vt_proj weight", wv, 128), sb = act_view("vt_proj x", tokens, -1, {});
   TapGemmParams p;
   std::memset(&p, 0, sizeof p);
-  sa.base = wv.w;
-  sa.dim[0] = wv.cin_pad; sa.dim[1] = C;
-  sa.stride[0] = wv.cin_pad * 2ull; sa.stride[1] = 2ull * C * wv.cin_pad; sa.stride[2] = sa.stride[1]; sa.stride[3] = sa.stride[1];
-  sa.box[0] = 64; sa.box[1] = 128;
-  fill_strides(sa);
-  sb.base = x.p;
-  sb.dim[0] = x.C; sb.dim[1] = ntok; sb.dim[2] = 1; sb.dim[3] = B; sb.dim[4] = 1;
-  sb.stride[0] = x.ld * 2ull; sb.stride[1] = 2ull * ntok * x.ld; sb.stride[2] = 2ull * ntok * x.ld; sb.stride[3] = sb.stride[2];
-  fill_strides(sb);
-  p.tdim[0] = ceil_div(C, 128); p.tdim[1] = 1; p.tdim[2] = B; p.tdim[3] = 1;
-  p.box[0] = 128; p.box[1] = 1; p.box[2] = 1; p.box[3] = 1;
-  p.ext[0] = C; p.ext[1] = 1; p.ext[2] = B; p.ext[3] = 1;
-  p.a_mul[0] = 128;
-  p.b_mul[0] = 0; p.b_mul[1] = 1; p.b_mul[2] = 0;
-  const long long m_tiles = 1ll * p.tdim[0] * B;
-  p.N = ntok;
-  p.BN = plan_bn(P, m_tiles, ntok, false);
-  p.n_tiles = ceil_div(ntok, p.BN);
-  sb.box[0] = 64; sb.box[1] = p.BN;
-  p.num_taps = 1;
-  p.kchunks = ceil_div(x.C, 64);
   p.out = vt.p;
   p.ostride[0] = ldv; p.ostride[1] = 0; p.ostride[2] = static_cast<long long>(C) * ldv; p.ostride[3] = 0;
-  p.ocol = 1;
   p.bias = wv.bias;
   p.bias_mode = wv.bias ? TG_BIAS_ROW : TG_BIAS_NONE;
   p.alpha = 1.f;
-  p.err = d_err;
   SelSpec sel{};
   if (wv.dir) {   // mixed-direction plan: the weight is the row operand, so the selection takes A and the row bias; t[2] = image
     sel.x = sa; sel.x.base = wv.w_alt;
     sel.s.dir = wv.dir; sel.s.bias = wv.bias_alt; sel.s.dim = 2; sel.s.div = 1; sel.s.sel_a = 1;
   }
-  launch_gemm(P, sa, sb, p, false, "tapgemm:vt",
-              wv.cin, 2.0 * (1.0 * C * wv.cin + 1.0 * B * ntok * wv.cin + 1.0 * B * C * ntok), nullptr, nullptr,
-              wv.dir ? &sel : nullptr);
+  launch_rows(P, sa, sb, p, C, 1, B, 0, 0, 1, ntok, x.C, 0, "tapgemm:vt", wv.cin,
+              2.0 * (1.0 * C * wv.cin + 1.0 * B * ntok * wv.cin + 1.0 * B * C * ntok), wv.dir ? &sel : nullptr);
   return vt;
 }
 
@@ -1698,37 +1696,15 @@ Act Engine::attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B,
   const int kvb = (kv_batch == B) ? 1 : 0;
 
   {  // S = alpha * Q K^T   (fp32 logits)
-    TmapSpec sa, sb;
+    const TmapSpec sa = heads_view("attention Q", q, d, Nq, heads, B, {64, 128}),
+                   sb = heads_view("attention K", k, d, Nk, heads, kv_batch, {});
     TapGemmParams p;
     std::memset(&p, 0, sizeof p);
-    sa.base = q.p;
-    sa.dim[0] = d; sa.dim[1] = Nq; sa.dim[2] = heads; sa.dim[3] = B;
-    sa.stride[0] = q.ld * 2ull; sa.stride[1] = d * 2ull; sa.stride[2] = 2ull * Nq * q.ld; sa.stride[3] = sa.stride[2];
-    sa.box[0] = 64; sa.box[1] = 128;
-    fill_strides(sa);
-    sb.base = k.p;
-    sb.dim[0] = d; sb.dim[1] = Nk; sb.dim[2] = heads; sb.dim[3] = kv_batch;
-    sb.stride[0] = k.ld * 2ull; sb.stride[1] = d * 2ull; sb.stride[2] = 2ull * Nk * k.ld; sb.stride[3] = sb.stride[2];
-    fill_strides(sb);
-    p.tdim[0] = ceil_div(Nq, 128); p.tdim[1] = heads; p.tdim[2] = B; p.tdim[3] = 1;
-    p.box[0] = 128; p.box[1] = 1; p.box[2] = 1; p.box[3] = 1;
-    p.ext[0] = Nq; p.ext[1] = heads; p.ext[2] = B; p.ext[3] = 1;
-    p.a_mul[0] = 128; p.a_mul[1] = 1; p.a_mul[2] = 1;
-    p.b_mul[0] = 1; p.b_mul[1] = kvb; p.b_mul[2] = 0;
-    const long long m_tiles = 1ll * p.tdim[0] * heads * B;
-    p.N = Nk;
-    p.BN = plan_bn(P, m_tiles, Nk, false);
-    p.n_tiles = ceil_div(Nk, p.BN);
-    sb.box[0] = 64; sb.box[1] = p.BN;
-    p.num_taps = 1;
-    p.kchunks = d / 64;
     p.out = S;
     p.out_fp32 = 1;
     p.ostride[0] = lds; p.ostride[1] = static_cast<long long>(Nq) * lds; p.ostride[2] = static_cast<long long>(heads) * Nq * lds;
-    p.ocol = 1;
     p.alpha = 1.0f / sqrtf(static_cast<float>(d));
-    p.err = d_err;
-    launch_gemm(P, sa, sb, p, false, "tapgemm:attn_qk", d,
+    launch_rows(P, sa, sb, p, Nq, heads, B, 1, 1, kvb, Nk, d, 0, "tapgemm:attn_qk", d,
                 2.0 * B * heads * (1.0 * Nq * d + 1.0 * Nk * d) + 4.0 * rows * Nk);
   }
   {  // P = softmax(S)
@@ -1751,75 +1727,44 @@ Act Engine::attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B,
     }
   }
   {  // O = P V   (V given transposed: [kvB][C][ldv])
-    TmapSpec sa, sb;
+    const long long plane = 1ll * Nq * lds, img = plane * heads;
+    const TmapSpec sa("attention P", Pm, {Nk, Nq, heads, B}, {lds, plane, img, img}, {64, 128}),
+                   sb = vt_view(vt, Nk, d, heads, kv_batch, {});
     TapGemmParams p;
     std::memset(&p, 0, sizeof p);
-    sa.base = Pm;
-    sa.dim[0] = Nk; sa.dim[1] = Nq; sa.dim[2] = heads; sa.dim[3] = B;
-    sa.stride[0] = lds * 2ull; sa.stride[1] = 2ull * Nq * lds; sa.stride[2] = 2ull * heads * Nq * lds; sa.stride[3] = sa.stride[2];
-    sa.box[0] = 64; sa.box[1] = 128;
-    fill_strides(sa);
-    const int ldv = vt.ld;
-    sb.base = vt.p;
-    sb.dim[0] = Nk; sb.dim[1] = d; sb.dim[2] = heads; sb.dim[3] = kv_batch;
-    sb.stride[0] = ldv * 2ull; sb.stride[1] = 2ull * d * ldv; sb.stride[2] = 2ull * C * ldv; sb.stride[3] = sb.stride[2];
-    fill_strides(sb);
-    p.tdim[0] = ceil_div(Nq, 128); p.tdim[1] = heads; p.tdim[2] = B; p.tdim[3] = 1;
-    p.box[0] = 128; p.box[1] = 1; p.box[2] = 1; p.box[3] = 1;
-    p.ext[0] = Nq; p.ext[1] = heads; p.ext[2] = B; p.ext[3] = 1;
-    p.a_mul[0] = 128; p.a_mul[1] = 1; p.a_mul[2] = 1;
-    p.b_mul[0] = 1; p.b_mul[1] = kvb; p.b_mul[2] = 0;
-    const long long m_tiles = 1ll * p.tdim[0] * heads * B;
-    p.N = d;
-    p.BN = std::min(d, 256);
-    p.n_tiles = ceil_div(d, p.BN);
-    sb.box[0] = 64; sb.box[1] = p.BN;
-    p.num_taps = 1;
-    p.kchunks = ceil_div(Nk, 64);
     p.out = out.p;
     p.ostride[0] = out.ld; p.ostride[1] = d; p.ostride[2] = static_cast<long long>(Nq) * out.ld;
-    p.ocol = 1;
     p.alpha = 1.f;
-    p.err = d_err;
-    launch_gemm(P, sa, sb, p, false, "tapgemm:attn_pv", Nk,
+    launch_rows(P, sa, sb, p, Nq, heads, B, 1, 1, kvb, d, Nk, std::min(d, 256), "tapgemm:attn_pv", Nk,
                 2.0 * (1.0 * rows * Nk + 1.0 * B * heads * Nk * d + 1.0 * rows * d));
   }
   return out;
 }
 
-Act Engine::flash_attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B, int Nq, int Nk, int heads, int kv_batch,
-                            bool causal) {
+// the FlashParams both fused attentions fill: query tiles of bm rows, out [B * Nq][out.ld]
+static FlashParams flash_params(const Act& out, int B, int Nq, int Nk, int heads, int kv_batch, int d, int bm, int* err) {
   I2IT_CHECK(kv_batch == B || kv_batch == 1, "attention: kv batch must be 1 or B");
-  const int d = FA_D, C = heads * d;
-  Act out = alloc_act(P, B, 1, Nq, C);
-  TmapSpec sq, sk, sv;
-  sq.base = q.p;
-  sq.dim[0] = d; sq.dim[1] = Nq; sq.dim[2] = heads; sq.dim[3] = B;
-  sq.stride[0] = q.ld * 2ull; sq.stride[1] = d * 2ull; sq.stride[2] = 2ull * Nq * q.ld; sq.stride[3] = sq.stride[2];
-  sq.box[0] = 64; sq.box[1] = FA_BM;
-  fill_strides(sq);
-  sk.base = k.p;
-  sk.dim[0] = d; sk.dim[1] = Nk; sk.dim[2] = heads; sk.dim[3] = kv_batch;
-  sk.stride[0] = k.ld * 2ull; sk.stride[1] = d * 2ull; sk.stride[2] = 2ull * Nk * k.ld; sk.stride[3] = sk.stride[2];
-  sk.box[0] = 64; sk.box[1] = FA_BN;
-  fill_strides(sk);
-  const int ldv = vt.ld;
-  sv.base = vt.p;
-  sv.dim[0] = Nk; sv.dim[1] = d; sv.dim[2] = heads; sv.dim[3] = kv_batch;
-  sv.stride[0] = ldv * 2ull; sv.stride[1] = 2ull * d * ldv; sv.stride[2] = 2ull * C * ldv; sv.stride[3] = sv.stride[2];
-  sv.box[0] = FA_BN; sv.box[1] = d;
-  fill_strides(sv);
   FlashParams fp;
   std::memset(&fp, 0, sizeof fp);
   fp.Nq = Nq; fp.Nk = Nk; fp.heads = heads; fp.B = B;
-  fp.q_tiles = ceil_div(Nq, FA_BM);
+  fp.q_tiles = ceil_div(Nq, bm);
   fp.kv_bmul = (kv_batch == B) ? 1 : 0;
   fp.scale_log2e = (1.0f / sqrtf(static_cast<float>(d))) * 1.4426950408889634f;
   fp.out = out.p;
   fp.ldo = out.ld;
-  fp.err = d_err;
+  fp.err = err;
+  return fp;
+}
+
+Act Engine::flash_attention(Plan& P, const Act& q, const Act& k, const Act& vt, int B, int Nq, int Nk, int heads, int kv_batch,
+                            bool causal) {
+  const int d = FA_D, C = heads * d;
+  Act out = alloc_act(P, B, 1, Nq, C);
+  FlashParams fp = flash_params(out, B, Nq, Nk, heads, kv_batch, d, FA_BM, d_err);
   fp.causal = causal ? 1 : 0;
-  const CUtensorMap tq = encode_tmap(sq, dtype), tk = encode_tmap(sk, dtype), tv = encode_tmap(sv, dtype);
+  const CUtensorMap tq = encode_tmap(heads_view("attention Q", q, d, Nq, heads, B, {64, FA_BM}), dtype),
+                    tk = encode_tmap(heads_view("attention K", k, d, Nk, heads, kv_batch, {64, FA_BN}), dtype),
+                    tv = encode_tmap(vt_view(vt, Nk, d, heads, kv_batch, {FA_BN, d}), dtype);
   const int grid = fp.q_tiles * heads * B, dt = dtype;
   char shp[96];
   snprintf(shp, sizeof shp, "B=%d h=%d Nq=%d Nk=%d d=%d", B, heads, Nq, Nk, d);
@@ -1830,36 +1775,14 @@ Act Engine::flash_attention(Plan& P, const Act& q, const Act& k, const Act& vt, 
 }
 
 Act Engine::flash_attention512(Plan& P, const Act& q, const Act& k, const Act& vt, int B, int Nq, int Nk, int kv_batch) {
-  I2IT_CHECK(kv_batch == B || kv_batch == 1, "attention: kv batch must be 1 or B");
   const int d = FA5_D;
   Act out = alloc_act(P, B, 1, Nq, d);
-  TmapSpec sq, sk, sv;
-  sq.base = q.p;
-  sq.dim[0] = d; sq.dim[1] = Nq; sq.dim[2] = B;
-  sq.stride[0] = q.ld * 2ull; sq.stride[1] = 2ull * Nq * q.ld;
-  sq.box[0] = 64; sq.box[1] = FA5_BM;
-  fill_strides(sq);
-  sk.base = k.p;
-  sk.dim[0] = d; sk.dim[1] = Nk; sk.dim[2] = kv_batch;
-  sk.stride[0] = k.ld * 2ull; sk.stride[1] = 2ull * Nk * k.ld;
-  sk.box[0] = 64; sk.box[1] = FA5_BN;
-  fill_strides(sk);
-  const int ldv = vt.ld;
-  sv.base = vt.p;
-  sv.dim[0] = Nk; sv.dim[1] = d; sv.dim[2] = kv_batch;
-  sv.stride[0] = ldv * 2ull; sv.stride[1] = 2ull * d * ldv;
-  sv.box[0] = FA5_BN; sv.box[1] = 64;
-  fill_strides(sv);
-  FlashParams fp;
-  std::memset(&fp, 0, sizeof fp);
-  fp.Nq = Nq; fp.Nk = Nk; fp.heads = 1; fp.B = B;
-  fp.q_tiles = ceil_div(Nq, FA5_BM);
-  fp.kv_bmul = (kv_batch == B) ? 1 : 0;
-  fp.scale_log2e = (1.0f / sqrtf(static_cast<float>(d))) * 1.4426950408889634f;
-  fp.out = out.p;
-  fp.ldo = out.ld;
-  fp.err = d_err;
-  const CUtensorMap tq = encode_tmap(sq, dtype), tk = encode_tmap(sk, dtype), tv = encode_tmap(sv, dtype);
+  const FlashParams fp = flash_params(out, B, Nq, Nk, 1, kv_batch, d, FA5_BM, d_err);
+  // 3-D maps: the kernel addresses (channel or key, token or channel, image)
+  const CUtensorMap tq = encode_tmap(TmapSpec("attention Q", q.p, {d, Nq, B}, {q.ld, 1ll * Nq * q.ld}, {64, FA5_BM}), dtype),
+                    tk = encode_tmap(TmapSpec("attention K", k.p, {d, Nk, kv_batch}, {k.ld, 1ll * Nk * k.ld}, {64, FA5_BN}), dtype),
+                    tv = encode_tmap(TmapSpec("attention V^T", vt.p, {Nk, d, kv_batch}, {vt.ld, 1ll * d * vt.ld}, {FA5_BN, 64}),
+                                     dtype);
   const long long grid = 2ll * fp.q_tiles * B;
   I2IT_CHECK(grid < (1ll << 31), "attention: too many query tiles");
   const int dt = dtype;

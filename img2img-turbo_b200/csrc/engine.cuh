@@ -27,6 +27,13 @@ struct TmapSpec {
   uint64_t dim[5] = {1, 1, 1, 1, 1};
   uint64_t stride[4] = {16, 16, 16, 16};   // bytes, dims 1..4
   uint32_t box[5] = {1, 1, 1, 1, 1};
+  TmapSpec() = default;
+  // A view of a 16-bit tensor, innermost dimension first; dimensions left out have extent 1 (box 1).  stride[i] is the step of
+  // dimension i + 1 in elements.  A dimension of extent 1 keeps its stride when that is a whole multiple of 16 bytes and
+  // otherwise takes the 16-byte placeholder TMA accepts; any other stride must be a multiple of 8 elements, or an Error
+  // naming the operand `what` is thrown (TMA cannot express such a pitch).
+  TmapSpec(const char* what, const void* base, std::initializer_list<long long> dims,
+           std::initializer_list<long long> strides, std::initializer_list<int> boxes);
 };
 CUtensorMap encode_tmap(const TmapSpec& s, int dtype);
 
@@ -409,6 +416,13 @@ class Engine {
   struct SelSpec { TmapSpec x, x2; TapGemmSel s; };
   void launch_gemm(Plan& P, const TmapSpec& sa, TmapSpec sb, const TapGemmParams& p, bool out_from_io, const char* kind,
                    double k_valid, double bytes, const TmapSpec* sa2 = nullptr, const TmapSpec* sb2 = nullptr,
+                   const SelSpec* sel = nullptr);
+  // launch_gemm for a single-tap GEMM over 128-row tiles of [batch][heads][M] rows (V^T projection, attention QK and PV):
+  // fills p's tile space, N, BN (bn 0: plan_bn's choice), n_tiles, kchunks (K-wide), ocol, err and sb's 64 x BN box.  A's
+  // head and image coordinates advance by a_step per tile, B's by b_head and b_img (0: one operand for every head / image).
+  // p brings the output, its strides, out_fp32, alpha and the bias.
+  void launch_rows(Plan& P, const TmapSpec& sa, TmapSpec sb, TapGemmParams p, int M, int heads, int batch, int a_step,
+                   int b_head, int b_img, int N, int K, int bn, const char* kind, double k_valid, double bytes,
                    const SelSpec* sel = nullptr);
   bool use_idres = true, use_pdl = false, trace_on = false, use_tmaout = true, use_gnepi = true, use_splitk = true, use_catfuse = true, use_ostg2 = true, use_lean = true, sync_each = false;
   bool tma_eligible(const TapGemmParams& p, bool out_from_io) const;

@@ -345,6 +345,8 @@ int i2it_read_prepared(i2it_handle* h, const char* key, void* w, size_t w_elems,
 
 /* ---- diagnostic single-op entry points (used by tests/ to check each kernel against the oracle) ----
  * Activations NHWC with pixel stride ld (elements); weights fp32 device pointers in PyTorch layout.
+ * Every pitch an op loads through TMA must be a multiple of 8 elements (16 bytes): ldx and ld2 of the conv ops,
+ * ldq / ldk / ldv of i2it_op_attention and ldx of i2it_op_vt_proj.  Any other pitch is refused before anything is launched.
  * All are synchronous on `stream`. */
 /* The output is [N, Ho, Wo, Cout] (Cout/2 for GEGLU) with Ho = ceil(H / stride): an odd map is zero-padded to even
  * (as F.conv2d(stride=2, padding=1) does).  The asymmetric VAE padding needs even H and W. */
